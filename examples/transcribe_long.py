@@ -1,4 +1,4 @@
-"""End-to-end example on a B200: long-form transcription of 16 kHz mono WAV files with segments, text and word timestamps.
+"""End-to-end example on an H100: long-form transcription of 16 kHz mono WAV files with segments, text and word timestamps.
 
   python examples/transcribe_long.py --weights /path/to/whisper-large-v3 audio1.wav audio2.wav [--vad] [--word-timestamps]
 

@@ -1,5 +1,5 @@
 /*
- * wkb200.h - C ABI of libwkb200.so: the Blackwell (sm_100a) implementation of WhisperKit's hot path
+ * wkb200.h - C ABI of libwkb200.so: the Hopper (sm_90a) implementation of WhisperKit's hot path
  *            PCM -> log-mel -> audio encoder -> KV-cached text decoder -> logits filters -> sampler.
  *
  * Every entry point is what a Swift (or Python ctypes) host binds to replace one member of the
@@ -31,7 +31,7 @@
  * (wk_mel, wk_encode, wk_filter_sample, wk_tensor_*) serialise internally; a wk_session (the per-task DecodingInputs of
  * TranscribeTask.swift:83 plus its own mel/encoder workspace and CUDA streams) belongs to one thread at a time, and different
  * sessions of one model run concurrently.  wk_tensor results own their device buffer until wk_tensor_free.
- * There is NO CPU fallback: every compute entry point fails with WK_ERR_MODELS_UNAVAILABLE if no sm_100 device is present.
+ * There is NO CPU fallback: every compute entry point fails with WK_ERR_MODELS_UNAVAILABLE if no sm_90 (Hopper) device is present.
  */
 #ifndef WKB200_H
 #define WKB200_H
@@ -423,7 +423,7 @@ wk_status wk_last_timings(wk_model* m, float* ms6);
 void* wk_model_stream(wk_model* m);
 
 /* ---- kernel-level test/bench hooks (used by tests/ and bench.py; device pointers) ---- */
-/* C[M,N] = A[M,K] * W[N,K]^T (+bias) with the tcgen05 GEMM; out_dtype WK_DTYPE_BF16/F16/F32. */
+/* C[M,N] = A[M,K] * W[N,K]^T (+bias) with the wgmma GEMM; out_dtype WK_DTYPE_BF16/F16/F32. */
 wk_status wk_test_gemm(wk_model* m, const void* a, const void* w, const float* bias, void* out, int32_t M, int32_t N, int32_t K,
                        int32_t in_dtype, int32_t out_dtype, int32_t gelu);
 /* out[M,N] (f32, in place) += A[M,K] * W[N,K]^T + bias: the residual-update epilogue of the encoder's out-proj / FC2. */

@@ -1,5 +1,5 @@
 """Known-answer vectors transcribed from the reference's own unit tests
-(`/root/reference/Tests/WhisperKitTests/UnitTests.swift:1982-2115`): toy logits, token
+(`Tests/WhisperKitTests/UnitTests.swift:1982-2115` of the reference repository): toy logits, token
 histories and the exact expected -inf patterns for the four LogitsFiltering impls.
 Shared by the oracle tests (CPU) and the CUDA sampler tests (GPU)."""
 import numpy as np

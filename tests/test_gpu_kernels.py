@@ -1,4 +1,4 @@
-"""Kernel-level parity tests on the B200 (through the C ABI test hooks of libwkb200.so).
+"""Kernel-level parity tests on the H100 (through the C ABI test hooks of libwkb200.so).
 References: torch fp32 on the same 16-bit-rounded inputs (floating-point kernels), the CPU oracle (mel),
 the reference's own known-answer vectors (filters)."""
 import ctypes as C
@@ -66,9 +66,8 @@ def test_gemm_tcgen05_vs_torch(toy, dt, M, N, K, gelu, out32):
 @pytest.mark.parametrize("dt", ["bf16", "f16"])
 @pytest.mark.parametrize("M,N,K", [(3000, 1280, 1280), (4500, 1280, 1280), (4097, 1280, 5120), (6000, 384, 384), (9000, 1280, 256)])
 def test_gemm_residual_update_in_place(toy, dt, M, N, K):
-    """out += A W^T + bias in place (the f32 residual stream; encoder out-proj / FC2), below and above the row count at which the
-    CTA-pair kernel with the staged, transposed epilogue takes over (4096), with ragged last row tiles; every element must be touched
-    exactly once (the epilogue prefetches residual values one chunk / one tile ahead)."""
+    """out += A W^T + bias in place (the f32 residual stream; encoder out-proj / FC2), small and encoder-sized row counts with ragged
+    last row tiles; every element must be touched exactly once (the epilogue reads and writes the residual in place)."""
     tdt, wdt = TD[dt]
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     a = (torch.randn(M, K, device="cuda", generator=g) * 0.5).to(tdt)

@@ -25,9 +25,9 @@ from oracle import model_ref as M  # noqa: E402
 
 LV3 = dict(endToken=50257, englishToken=50259, noSpeechToken=50363, noTimestampsToken=50364, specialTokenBegin=50257,
            startOfPreviousToken=50362, startOfTranscriptToken=50258, timeTokenBegin=50365, transcribeToken=50360, translateToken=50359)
-# logits tolerance (relative to the row's largest |logit|): f16 meets north_star's 1e-3 (measured on B200: 7.1e-4 at 32 decoder layers,
-# 5.1e-4 / 4.4e-4 at 4 / 2 layers).  bf16 does NOT: measured 5.2e-3 / 3.3e-3 / 3.0e-3 (32 / 4 / 2 layers) against its same-policy twin and
-# 4.3e-3 against the fp32 oracle - the 8-bit mantissa of every stored activation; its bound here is the measured error with headroom.
+# logits tolerance (relative to the row's largest |logit|): f16 is held to north_star's 1e-3.  bf16 cannot be: the 8-bit mantissa of every
+# stored activation puts its error against the same-policy twin and the fp32 oracle at a few 1e-3, so its bound is wider (the test prints
+# the measured errors).
 TOL_TWIN = {"f16": 1e-3, "bf16": 7e-3}
 TOL_FP32 = {"f16": 2e-3, "bf16": 1.5e-2}    # against the fp32 oracle: the storage policy's own rounding is part of the difference
 

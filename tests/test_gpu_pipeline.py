@@ -588,8 +588,8 @@ def test_transcribe_audio_text_and_words_with_library_tokenizer():
 
 
 def test_fused_decoder_chains_match_the_launch_per_phase_path():
-    """csrc/fused_chain.cu (WKB200_FUSED=1: persistent phase chains with grid barriers; measured slower than the default on B200, kept as
-    an opt-in) keeps the arithmetic and its order: tokens and logits must be bit-identical to the launch-per-phase schedule, at toy widths
+    """csrc/fused_chain.cu (WKB200_FUSED=1: persistent phase chains with grid barriers; kept as an opt-in, off by
+    default) keeps the arithmetic and its order: tokens and logits must be bit-identical to the launch-per-phase schedule, at toy widths
     and at d = 1280 / H = 20 / V = 51866."""
     import subprocess
     import sys

@@ -1,30 +1,10 @@
-"""CPU checks of the closed-form approximations the CUDA kernels use (constants restated here; numpy emulates the f32 arithmetic):
-the polynomial exp2 of the encoder attention (attention_tcgen05.cu: fa_ex2_poly2) and the erf GELU of the FC1 epilogue
-(common.cuh: gelu_erf / gelu_erf2).  They bound the approximation error itself; the kernels are checked end to end in the -m gpu tests."""
+"""CPU check of the closed-form approximation the CUDA kernels use for the erf GELU of the FC1 epilogue (common.cuh: gelu_erf /
+gelu_erf2; constants restated here, numpy emulates the f32 arithmetic).  It bounds the approximation error itself; the kernels are checked
+end to end in the -m gpu tests."""
 import numpy as np
 from scipy.special import erf
 
 F = np.float32
-
-
-def test_polynomial_exp2_of_the_attention_kernel():
-    x = np.concatenate([np.linspace(-140, 8, 400001), [-np.inf, -126.0, -125.5, -0.5, 0.0, 0.5, 7.99, 8.0]]).astype(F)
-    xc = np.maximum(x, F(-126))
-    magic = F(12582912.0)                      # 1.5 * 2^23: the low mantissa bits of t hold round(x)
-    t = (xc + magic).astype(F)
-    nf = (t - magic).astype(F)
-    f = (xc - nf).astype(F)
-    assert np.abs(f).max() <= 0.5
-    r = (f * F(0.05517146) + F(0.24261086)).astype(F)
-    r = (r * f + F(0.69326097)).astype(F)
-    r = (r * f + F(0.9999281)).astype(F)
-    bits = (r.view(np.int32).astype(np.int64) + ((t.view(np.int32).astype(np.int64) << 23) & 0xFFFFFFFF)) & 0xFFFFFFFF
-    got = bits.astype(np.uint32).view(F)
-    ref = np.exp2(xc.astype(np.float64))
-    rel = np.abs(got / ref - 1)
-    live = xc > -120                           # (below: the clamp region, probabilities ~1e-36 that round to nothing)
-    assert rel[live].max() < 8e-5, rel[live].max()
-    assert np.all(np.isfinite(got)) and got.min() >= 0
 
 
 def test_erf_gelu_of_the_fc1_epilogue():

@@ -1,6 +1,6 @@
-"""whisperkit_b200 - Blackwell (sm_100a) implementation of WhisperKit's hot path behind its protocol surface.
+"""whisperkit_b200 - Hopper (sm_90a) implementation of WhisperKit's hot path behind its protocol surface.
 
-The compute lives in libwkb200.so (hand-written CUDA: tcgen05/TMA GEMMs, fused log-mel, attention, fused
+The compute lives in libwkb200.so (hand-written CUDA: wgmma/TMA GEMMs, fused log-mel, attention, fused
 filter+sampler); this package is the thin host mirror of the reference interface over the C ABI
 (include/wkb200.h).  Importing the package is cheap; the shared library is loaded on first use and its
 absence is an error (there is no CPU / PyTorch fallback).

@@ -10,7 +10,7 @@ Class / method names follow WhisperKit so parity tests read like the reference's
   SpecialTokens                           Sources/WhisperKit/Core/Models.swift:1111-1149
   WhisperKit.transcribe(audioArrays:)     Sources/WhisperKit/Core/WhisperKit.swift:667-812
 
-All arithmetic happens in libwkb200.so (sm_100a kernels); this module only marshals arguments.
+All arithmetic happens in libwkb200.so (sm_90a kernels); this module only marshals arguments.
 """
 from __future__ import annotations
 

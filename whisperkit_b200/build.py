@@ -1,4 +1,4 @@
-"""In-tree build of libwkb200.so (nvcc, sm_100a only) and of the test-only C oracles.
+"""In-tree build of libwkb200.so (nvcc, sm_90a only) and of the test-only C oracles.
 
 `python -m whisperkit_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.
 """
@@ -16,9 +16,9 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 BUILD = os.path.join(PKG, "_build")
 LIB = os.path.join(PKG, "libwkb200.so")
-SOURCES = ["gemm_tcgen05.cu", "attention_tcgen05.cu", "mel.cu", "encoder_ops.cu", "decoder_ops.cu", "cross_attention_mq.cu", "engine.cu", "session.cu", "longform.cu", "wordtiming.cu", "tokenizer.cu", "fused_chain.cu", "writers.cu", "comm.cu"]
+SOURCES = ["gemm_wgmma.cu", "attention_wgmma.cu", "mel.cu", "encoder_ops.cu", "decoder_ops.cu", "cross_attention_mq.cu", "engine.cu", "session.cu", "longform.cu", "wordtiming.cu", "tokenizer.cu", "fused_chain.cu", "writers.cu", "comm.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--use_fast_math=false",
 ]
 

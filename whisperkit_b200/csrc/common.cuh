@@ -1,4 +1,4 @@
-// Common device helpers for the wkb200 kernels (sm_100a only).
+// Common device helpers for the wkb200 kernels (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -13,7 +13,6 @@ namespace wk {
 // ------------------------------------------------------------------ 16-bit type traits
 template <typename T> struct T16;
 template <> struct T16<__nv_bfloat16> {
-    static constexpr int kUmmaFormat = 1;  // cute::UMMA::F16F32Format::BF16
     __device__ __forceinline__ static float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
     __device__ __forceinline__ static __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
     __device__ __forceinline__ static uint32_t pack2(float a, float b) {
@@ -26,7 +25,6 @@ template <> struct T16<__nv_bfloat16> {
     }
 };
 template <> struct T16<__half> {
-    static constexpr int kUmmaFormat = 0;  // F16
     __device__ __forceinline__ static float to_f(__half v) { return __half2float(v); }
     __device__ __forceinline__ static __half from_f(float v) { return __float2half_rn(v); }
     __device__ __forceinline__ static uint32_t pack2(float a, float b) {
@@ -52,38 +50,11 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return 0.5f * x * (1.0f + copysignf(erf_abs, x));
 }
 
-// packed f32x2 arithmetic (FFMA2 / FADD2 / FMUL2 on sm_100): one issue slot for two lanes of work
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 rd, ra, rb, rc;\n\t"
-        "mov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y)
-        : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rd;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "add.rn.f32x2 rd, ra, rb;\n\t"
-        "mov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y)
-        : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rd;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "mul.rn.f32x2 rd, ra, rb;\n\t"
-        "mov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y)
-        : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-// gelu_erf on two values at once: the same formula, the FMA-pipe part packed (the FC1 epilogue is bound by its instruction issue)
+// f32 pair arithmetic: the pair helpers keep the epilogue code written two values at a time
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+// gelu_erf on two values at once (the FC1 epilogue is bound by its instruction issue: ex2.approx instead of __expf's range handling)
 __device__ __forceinline__ float2 gelu_erf2(float2 x) {
     const float2 z = make_float2(fabsf(x.x) * 0.70710678118654752440f, fabsf(x.y) * 0.70710678118654752440f);
     const float2 den = fma2(make_float2(0.3275911f, 0.3275911f), z, make_float2(1.0f, 1.0f));
@@ -187,8 +158,8 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
         "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-// The same loads for a CONVERGED warp (every lane calls, the instruction is predicated on the elect.sync lane - see tc_mma_f16_elect below
-// for why: UTMALDG takes uniform-register operands as well).
+// The same loads for a CONVERGED warp: every lane calls, the instruction is predicated on the lane elect.sync picks, so the issue
+// path stays straight-line code (UTMALDG takes uniform-register operands; from an `if (lane == 0)` branch the compiler rebuilds them).
 __device__ __forceinline__ void tma_load_2d_elect(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1) {
     asm volatile(
         "{\n\t.reg .pred q;\n\t"
@@ -219,92 +190,6 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
             smem_u32(smem_dst)),
         "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
         : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (bf16/f16 in, f32 accumulate)
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// The same instructions for a CONVERGED warp: every lane executes the call, the instruction itself is predicated (inside the asm) on the
-// lane elect.sync picks.  UTCHMMA / UTCBAR take uniform-register operands; issued from an `if (lane == 0)` branch the compiler has to
-// rebuild each operand with an ELECT / R2UR.BROADCAST / BRA.U.ANY loop (~125 clocks per MMA on B200 - as long as a 128x256x16 MMA runs),
-// with elect.sync the issue path is straight-line code.
-__device__ __forceinline__ void tc_mma_f16_elect(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tc_commit_elect(uint64_t* bar) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar))
-        : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets lane (base+i), columns [c, c+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128-byte-swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major: 1) | SBO>>4 [32,46) = 1024B between
-// 8-row groups | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): c=F32, a/b format, K-major both, N>>3, M>>4
-__device__ __forceinline__ uint32_t make_idesc_f16(int fmt, int M, int N) {
-    uint32_t d = 0;
-    d |= 1u << 4;                         // c_format F32
-    d |= (uint32_t)fmt << 7;              // a_format
-    d |= (uint32_t)fmt << 10;             // b_format
-    d |= (uint32_t)(N >> 3) << 17;        // n_dim
-    d |= (uint32_t)(M >> 4) << 24;        // m_dim
-    return d;
 }
 
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)

@@ -1,4 +1,4 @@
-// Decoder-side kernels: everything one autoregressive step needs besides the (swap-AB, split-K) tcgen05 GEMMs.
+// Decoder-side kernels: everything one autoregressive step needs besides the (swap-AB, split-K) wgmma GEMMs.
 //
 // Reference behaviour restated on the device (so the host sees only final token IDs):
 //   decodeText loop state machine            Sources/WhisperKit/Core/TextDecoder.swift:566-686

@@ -85,9 +85,9 @@ wk_status layernorm_f32_to_f32(const float* x, const float* gamma, const float* 
     return launch_ln<float>(x, gamma, beta, out, rows, d, stream);
 }
 
-// Encoder attention lives in attention_tcgen05.cu (TMA + tcgen05 + TMEM); this is only its entry point.
+// Encoder attention lives in attention_wgmma.cu (TMA + wgmma); this is only its entry point.
 wk_status encoder_attention(const void* qkv, void* out, int B, int T, int n_heads, int dtype, cudaStream_t stream) {
-    return encoder_attention_tcgen05(qkv, out, B, T, n_heads, dtype, stream);
+    return encoder_attention_wgmma(qkv, out, B, T, n_heads, dtype, stream);
 }
 
 // =====================================================================================================

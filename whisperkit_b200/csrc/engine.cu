@@ -1,7 +1,7 @@
 // libwkb200 engine: the model object (weights, mel tables, alignment heads), weight ingestion, the mel + encoder schedule, the
 // piecewise protocol entry points wk_mel / wk_encode and the kernel-level hooks.  Decode sessions and the window scheduler are in
 // session.cu.  Host-side control flow mirrors the reference's per-window body
-// (Sources/WhisperKit/Core/TranscribeTask.swift:116-278); all arithmetic runs in the sm_100a kernels of this directory.
+// (Sources/WhisperKit/Core/TranscribeTask.swift:116-278); all arithmetic runs in the sm_90a kernels of this directory.
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -32,10 +32,8 @@ const char* last_error_cstr() { return g_err; }
 static std::atomic<long long> g_launches{0};
 static std::atomic<int> g_pdl{-1};
 int pdl_mode() {
-    // Programmatic dependent launch along the decode step.  Measured on B200 (64 windows, 63 steps, ms per hot-path pass): off 495-498,
-    // every kernel (63) 480-489, GEMM + split-K reduce (48) 480-481, reduce only (32) 488; on top of 48: + cross-attention (its K chunks
-    // are static and prefetched before griddepcontrol.wait) 473, + embed 478, + self-attention 486 (worse), + sampler 481 (neutral).
-    // Mask 53 = embed | cross-attention | GEMM | reduce: the kernels with a real prologue to hide under the upstream kernel's tail.
+    // Programmatic dependent launch along the decode step.  Mask 53 = embed | cross-attention (its K chunks are static and prefetched
+    // before griddepcontrol.wait) | GEMM | reduce: the kernels with a real prologue to hide under the upstream kernel's tail.
     // WKB200_PDL_MASK (read once per process) overrides it for A/B measurements.
     int v = g_pdl.load(std::memory_order_relaxed);
     if (v < 0) {
@@ -53,9 +51,8 @@ void launch_counter_sub(long long n) { g_launches.fetch_sub(n); }
 
 int choose_splits(int tiles, int total_kb, int num_sms) {
     // Split-K depth of a decoder swap-AB GEMM: the deepest split that still fits ONE wave of CTAs (tiles * s <= SMs), so every SM that
-    // takes part streams its share of the weights exactly once.  Measured with HBM-cold weights on B200 (tools/microbench_cold.py,
-    // 64 windows): one SM sustains only ~40 GB/s, so too few CTAs starve (d x d: s=1 11.0 us, s=10 6.1 us) while a second wave costs
-    // more than it saves (FC1: s=2 8.5 us, s=4 9.6 us; QKV: s=4 7.3 us, s=5 9.1 us; FC2: s=10 8.1 us, s=20 9.4 us).
+    // takes part streams its share of the weights exactly once: one SM alone cannot pull HBM bandwidth, so too few CTAs starve, while a
+    // second wave costs more than the extra parallelism saves (tools/microbench_cold.py times the choices with HBM-cold weights).
     int best = 1;
     for (int s = 1; s <= total_kb && s <= 20; ++s) {   // 20 = kMaxSplits of the fused reduce kernels
         if (total_kb % s) continue;
@@ -224,7 +221,6 @@ static bool resolve_name(wk_model* m, const std::string& name, Dest* out) {
 }
 
 // ---------------------------------------------------------------------------------------------- mel + encoder schedule
-bool gemm_pair_enabled();
 GemmDesc plain_gemm(const void* a, int64_t M, int K, const void* w, int N, int dtype, int mode, void* out, int64_t ld_out,
                     const float* bias, int gelu) {
     GemmDesc g;
@@ -234,16 +230,7 @@ GemmDesc plain_gemm(const void* a, int64_t M, int K, const void* w, int N, int d
     g.m_rows_per_batch = (int)M; g.n = N; g.k = K; g.taps = 1;
     g.bn = N >= 256 ? 256 : round_up(N, 16);
     g.splits = 1; g.mode = mode; g.gelu = gelu; g.out = out; g.ld_out = ld_out; g.out_rows_per_batch = M; g.bias = bias;
-    g.pair = gemm_pair_enabled() && M >= 4096;   // encoder-sized products: CTA pairs with the weight tile multicast
     return g;
-}
-
-bool gemm_pair_enabled() {
-    // 2-CTA multicast variant of the encoder GEMMs: on (parity suite green with it; encoder QKV 0.746 -> 0.714 ms, cross-KV projection
-    // 18.0 -> 16.3 ms, encoder pass 176.0 -> 173.8 ms at 64 windows on B200).  WKB200_GEMM_PAIR=0 (read once per process) keeps the
-    // single-CTA kernel reachable for A/B timing.
-    static const bool on = !(getenv("WKB200_GEMM_PAIR") && atoi(getenv("WKB200_GEMM_PAIR")) == 0);
-    return on;
 }
 
 wk_status mel_run(wk_model* m, EncWorkspace* ws, const float* pcm, int64_t n, int64_t stride, const int32_t* samples_per_window,
@@ -290,7 +277,7 @@ wk_status encode_chunk(wk_model* m, EncWorkspace* ws, const void* mel, int B, vo
         g.splits = 1; g.mode = GEMM_OUT_T16; g.gelu = 1;
         g.out = (char*)ws->h1 + (size_t)d * 2;  // row 0 of every window is the zero pad
         g.ld_out = d; g.out_rows_per_batch = kMelRows; g.bias = m->conv1_b;
-        WK_CHECK(gemm_tcgen05(g, m->num_sms, s));
+        WK_CHECK(gemm_wgmma(g, m->num_sms, s));
     }
     // conv2 (k=3, stride 2, pad 1) + GELU + positional embedding -> residual stream x (f32)
     {
@@ -306,17 +293,17 @@ wk_status encode_chunk(wk_model* m, EncWorkspace* ws, const void* mel, int B, vo
         g.bn = d >= 256 ? 256 : round_up(d, 16);
         g.splits = 1; g.mode = GEMM_OUT_F32_GELU_POS; g.gelu = 1;
         g.out = ws->x; g.ld_out = d; g.out_rows_per_batch = T; g.bias = m->conv2_b; g.pos = m->enc_pos; g.ld_pos = d;
-        WK_CHECK(gemm_tcgen05(g, m->num_sms, s));
+        WK_CHECK(gemm_wgmma(g, m->num_sms, s));
     }
     for (int li = 0; li < c.enc_layers; ++li) {
         EncLayer& l = m->enc[li];
         WK_CHECK(layernorm_f32_to_16(ws->x, l.ln1.g, l.ln1.b, ws->xn, M, d, dt, s));
-        WK_CHECK(gemm_tcgen05(plain_gemm(ws->xn, M, d, l.wqkv, 3 * d, dt, GEMM_OUT_T16, ws->qkv, 3 * d, l.bqkv, 0), m->num_sms, s));
+        WK_CHECK(gemm_wgmma(plain_gemm(ws->xn, M, d, l.wqkv, 3 * d, dt, GEMM_OUT_T16, ws->qkv, 3 * d, l.bqkv, 0), m->num_sms, s));
         WK_CHECK(encoder_attention(ws->qkv, ws->attn, B, T, c.n_heads, dt, s));
-        WK_CHECK(gemm_tcgen05(plain_gemm(ws->attn, M, d, l.wo, d, dt, GEMM_OUT_F32_ADD, ws->x, d, l.bo, 0), m->num_sms, s));
+        WK_CHECK(gemm_wgmma(plain_gemm(ws->attn, M, d, l.wo, d, dt, GEMM_OUT_F32_ADD, ws->x, d, l.bo, 0), m->num_sms, s));
         WK_CHECK(layernorm_f32_to_16(ws->x, l.ln2.g, l.ln2.b, ws->xn, M, d, dt, s));
-        WK_CHECK(gemm_tcgen05(plain_gemm(ws->xn, M, d, l.w1, 4 * d, dt, GEMM_OUT_T16, ws->ffn, 4 * d, l.b1, 1), m->num_sms, s));
-        WK_CHECK(gemm_tcgen05(plain_gemm(ws->ffn, M, 4 * d, l.w2, d, dt, GEMM_OUT_F32_ADD, ws->x, d, l.b2, 0), m->num_sms, s));
+        WK_CHECK(gemm_wgmma(plain_gemm(ws->xn, M, d, l.w1, 4 * d, dt, GEMM_OUT_T16, ws->ffn, 4 * d, l.b1, 1), m->num_sms, s));
+        WK_CHECK(gemm_wgmma(plain_gemm(ws->ffn, M, 4 * d, l.w2, d, dt, GEMM_OUT_F32_ADD, ws->x, d, l.b2, 0), m->num_sms, s));
     }
     WK_CHECK(layernorm_f32_to_16(ws->x, m->enc_ln.g, m->enc_ln.b, enc_out, M, d, dt, s));
     return WK_OK;
@@ -332,14 +319,14 @@ using namespace wk;
 extern "C" {
 
 const char* wk_last_error(void) { return wk::last_error_cstr(); }
-const char* wk_version(void) { return "wkb200 0.2 (sm_100a)"; }
+const char* wk_version(void) { return "wkb200 0.3 (sm_90a)"; }
 
 int32_t wk_device_available(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return 0;
     cudaDeviceProp p;
     if (cudaGetDeviceProperties(&p, 0) != cudaSuccess) return 0;
-    return p.major == 10 ? 1 : 0;
+    return p.major == 9 ? 1 : 0;   // the kernels are built for sm_90a only (wgmma, TMA, setmaxnreg)
 }
 
 void wk_default_config(const char* variant, wk_model_config* c) {
@@ -386,7 +373,7 @@ wk_status wk_detect_variant(int32_t logits_dim, int32_t encoder_dim, const char*
 wk_status wk_model_create(const wk_model_config* cfg, int32_t device, wk_model** out) {
     if (!cfg || !out) { set_error("wk_model_create: null argument"); return WK_ERR_INVALID_ARGUMENT; }
     if (!wk_device_available()) {
-        set_error("no sm_100 CUDA device visible: libwkb200 has no CPU fallback");
+        set_error("no sm_90 (Hopper) CUDA device visible: libwkb200 has no CPU fallback");
         return WK_ERR_MODELS_UNAVAILABLE;
     }
     if (cfg->d_model != cfg->n_heads * 64 || cfg->d_model % 128 != 0 || (cfg->n_mels != 80 && cfg->n_mels != 128) ||
@@ -454,7 +441,7 @@ wk_status wk_model_set_tensor(wk_model* m, const char* name, const void* data, i
 
 // ---------------------------------------------------------------------------------------------- safetensors loader
 // HuggingFace checkpoint directory: config.json + *.safetensors (8-byte LE header length, JSON header, raw tensors).
-// The reference loads CoreML bundles instead (WhisperKit.swift:358-442); on B200 weights come from safetensors.
+// The reference loads CoreML bundles instead (WhisperKit.swift:358-442); here weights come from safetensors.
 namespace {
 struct JsonScan {
     const char* p; const char* end;
@@ -957,7 +944,7 @@ wk_status wk_test_gemm(wk_model* m, const void* a, const void* w, const float* b
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
     const int mode = out_dtype == WK_DTYPE_F32 ? GEMM_OUT_F32 : GEMM_OUT_T16;
-    WK_CHECK(gemm_tcgen05(plain_gemm(a, M, K, w, N, in_dtype, mode, out, N, bias, gelu), m->num_sms, m->stream));
+    WK_CHECK(gemm_wgmma(plain_gemm(a, M, K, w, N, in_dtype, mode, out, N, bias, gelu), m->num_sms, m->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
     return WK_OK;
 }
@@ -967,7 +954,7 @@ wk_status wk_test_gemm_residual(wk_model* m, const void* a, const void* w, const
     if (!m || !a || !w || !out) return WK_ERR_INVALID_ARGUMENT;
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
-    WK_CHECK(gemm_tcgen05(plain_gemm(a, M, K, w, N, in_dtype, GEMM_OUT_F32_ADD, out, N, bias, 0), m->num_sms, m->stream));
+    WK_CHECK(gemm_wgmma(plain_gemm(a, M, K, w, N, in_dtype, GEMM_OUT_F32_ADD, out, N, bias, 0), m->num_sms, m->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
     return WK_OK;
 }
@@ -996,7 +983,7 @@ wk_status wk_test_gemm_splitk(wk_model* m, const void* w, const void* x, float* 
     g.b = x; g.b_rows = rows_x; g.b_ld = K; g.in_dtype = in_dtype;
     g.m_rows_per_batch = N; g.n = rows_x; g.k = K; g.taps = 1; g.bn = rows_x; g.splits = sp;
     g.mode = GEMM_OUT_PARTIAL_T; g.out = partial; g.ld_out = N; g.out_rows_per_batch = N; g.partial_cols = rows_x;
-    wk_status r = gemm_tcgen05(g, m->num_sms, m->stream);
+    wk_status r = gemm_wgmma(g, m->num_sms, m->stream);
     if (r == WK_OK) {
         const long long n = (long long)rows_x * N;
         reduce_partials_kernel<<<(unsigned)((n + 255) / 256), 256, 0, m->stream>>>(partial, sp, rows_x, N, rows_x, out);

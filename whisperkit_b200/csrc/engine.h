@@ -88,7 +88,7 @@ struct wk_tensor {
 struct wk_model {
     wk_model_config cfg;
     int device = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     cudaStream_t stream = nullptr;   // the piecewise API (wk_mel, wk_encode, wk_filter_sample, readbacks) is enqueued here
     std::mutex api_mu;               // ... one host thread at a time: the handle itself is immutable once finalized
     bool finalized = false;

@@ -1,16 +1,16 @@
 // fused_chain.cu - decoder phase chains: one persistent kernel runs a CHAIN of decoder phases that today are separate launches:
 //     swap-AB split-K GEMM -> split-K reduce (+bias +residual +LayerNorm | +bias +GELU) -> GEMM -> ...
-// with a grid-wide barrier between phases instead of a kernel boundary.  Motivation (profiles/r01_summary.md section 6): a decoder GEMM
-// launch is ~5.2 us of fixed cost around ~0.9 us of weight streaming, 11 such launches per layer; inside one kernel TMEM, mbarriers and
-// tensor maps are set up once, the WEIGHT tiles of the next GEMM phase are put in flight before the barrier (weights are static), and
+// with a grid-wide barrier between phases instead of a kernel boundary.  Motivation: a decoder GEMM launch is a few
+// microseconds of fixed cost around about one microsecond of weight streaming, 11 such launches per layer; inside one kernel the mbarriers
+// and tensor maps are set up once, the WEIGHT tiles of the next GEMM phase are put in flight before the barrier (weights are static), and
 // a phase boundary costs one barrier.  Chains per decoder layer (engine.cu, decoder_forward):
 //     B: out-proj GEMM -> reduce+LN -> cross-Q GEMM                                                  (between self- and cross-attention)
 //     C: cross-out GEMM -> reduce+LN -> FC1 -> reduce+GELU -> FC2 -> reduce+LN -> next layer's QKV GEMM  (between cross- and self-attention)
 //
-// Structure: grid = one CTA per SM (all co-resident), 320 threads.  GEMM phase: warp 0 = TMA producer, warp 1 = tcgen05 MMA issuer,
-// warps 2-9 = epilogue (transposed f32 partial store), work item = (128-row weight tile, K split), one per CTA (single wave by the
-// split rule).  Reduce phase: all 320 threads, CTA b reduces batch rows b, b + grid, ... in the fixed split order (deterministic).  Pipeline state
-// (ring stage / parity, accumulator parity) lives in registers across phases.  Memory ordering at a phase boundary: every thread
+// Structure: grid = one CTA per SM (all co-resident), 384 threads = 3 warpgroups.  GEMM phase: warp 0 = TMA producer, warpgroups 1 and 2
+// = wgmma consumers (64 weight rows each, accumulator in registers) whose epilogue stores the transposed f32 partials, work item =
+// (128-row weight tile, K split), one per CTA (single wave by the split rule).  Reduce phase: all 384 threads, CTA b reduces batch rows
+// b, b + grid, ... in the fixed split order (deterministic).  Pipeline state (ring stage / parity) lives in registers across phases.  Memory ordering at a phase boundary: every thread
 // fences its generic-proxy global writes towards the async proxy (the next GEMM phase reads activations with TMA), then
 // bar.sync + __threadfence + atomic arrive / acquire spin (the cooperative-groups grid.sync recipe).
 #include <cuda_bf16.h>
@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 #define WK_CHECK_STATUS(expr)             \
     do {                                  \
@@ -32,9 +33,9 @@ namespace wk {
 
 namespace {
 
-constexpr int kM = 128, kK = 64, kUK = 16;
+constexpr int kM = 128, kK = 64;
 constexpr int kStageABytes = kM * kK * 2;
-constexpr int kThreads = 320;
+constexpr int kThreads = 384;
 constexpr int kRingMax = 8;
 constexpr int kMaxSplitsR = 20;
 
@@ -51,8 +52,7 @@ struct ChainK {
     PhaseK ph[kChainMaxPhases];
     float* partial; float* x;
     int B, Bp, d;
-    uint32_t idesc;
-    int stages, stage_b_bytes, tmem_cols, acc_stride;
+    int stages, stage_b_bytes;
     unsigned int* counters;
     unsigned int* reset;
 };
@@ -120,7 +120,7 @@ __device__ __forceinline__ void reduce_ln_row(const ChainK& p, const PhaseK& P, 
             s += a.x + a.y + a.z + a.w;
         }
     }
-    // block_sum over 320 threads (10 warps)
+    // block_sum over kThreads threads
     auto bsum = [&](float val) -> float {
         val = warp_sum(val);
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -175,7 +175,7 @@ __device__ __forceinline__ void reduce_gelu_all(const ChainK& p, const PhaseK& P
     }
 }
 
-template <typename T>
+template <typename T, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 decoder_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainK p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -184,30 +184,21 @@ decoder_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainK p) {
     uint8_t* tail = smem + (size_t)p.stages * stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
     uint64_t* empty_bar = full_bar + kRingMax;
-    uint64_t* tfull_bar = empty_bar + kRingMax;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    float* scratch = reinterpret_cast<float*>(tmem_slot + 4);   // 32 floats
+    float* scratch = reinterpret_cast<float*>(empty_bar + kRingMax);   // 32 floats
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_launch_dependents();
     if (warp == 0 && lane == 0) {
         for (int g = 0; g < kChainMaxGemms; ++g) { tma_prefetch_desc(&maps.a[g]); tma_prefetch_desc(&maps.b[g]); }
-        for (int i = 0; i < p.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 8); }
+        for (int i = 0; i < p.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }   // empty: one arrive per consumer warp
         fence_barrier_init();
     }
-    if (warp == 1) { tmem_alloc(tmem_slot, p.tmem_cols); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     // ---- pipeline state that survives the phases
     int p_stage = 0; uint32_t p_phase = 0;      // producer (warp 0, lane 0)
     int pre_stage0 = 0, pre_n = 0, pre_for = -1; // weight tiles already in flight for GEMM phase `pre_for`
-    int m_stage = 0; uint32_t m_phase = 0;      // MMA issuer (warp 1)
-    int acc_it = 0;                             // accumulator use count (MMA warp and epilogue warps keep their own copy in step)
+    int m_stage = 0; uint32_t m_phase = 0;      // consumer warpgroups (both walk the ring in step)
 
     auto work_of = [&](const PhaseK& P, int* tile, int* split) -> bool {
         const int w = blockIdx.x;
@@ -266,55 +257,47 @@ decoder_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainK p) {
                     }
                     pre_for = -1;
                 }
-            } else if (has && warp == 1) {
-                // ===================== MMA issuer =====================
-                const int acc = acc_it & 1;
-                const uint32_t acc_phase = (acc_it >> 1) & 1;
-                mbar_wait_bounded(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * p.acc_stride;
+            } else if (has && warp >= 4) {
+                // ===================== wgmma consumers: weight rows [64 cw, 64 cw + 64) of the tile =====================
+                const int cw = (warp >> 2) - 1;
+                float acc[BN / 2];
+                int prev = -1;
                 for (int kb = 0; kb < P.kb_per_split; ++kb) {
                     mbar_wait_bounded(&full_bar[m_stage], m_phase);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t sa = smem_u32(smem + (size_t)m_stage * stage_bytes);
-                        const uint64_t adesc = make_kmajor_sw128_desc(sa);
-                        const uint64_t bdesc = make_kmajor_sw128_desc(sa + kStageABytes);
+                    const uint32_t sa = smem_u32(smem + (size_t)m_stage * stage_bytes);
+                    const uint64_t adesc = wgmma_desc_sw128(sa + cw * 64 * 128);
+                    const uint64_t bdesc = wgmma_desc_sw128(sa + kStageABytes);
+                    wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < kK / kUK; ++k)
-                            tc_mma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), p.idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                        tc_commit(&empty_bar[m_stage]);
-                        if (kb == P.kb_per_split - 1) tc_commit(&tfull_bar[acc]);
+                    for (int k = 0; k < kK / 16; ++k)
+                        Wgmma<T, BN>::ss(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (prev >= 0) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
                     }
-                    __syncwarp();
+                    prev = m_stage;
                     if (++m_stage == p.stages) { m_stage = 0; m_phase ^= 1; }
                 }
-            } else if (has && warp >= 2) {
-                // ===================== epilogue: transposed f32 partial store [split][b][n] =====================
-                const int quarter = warp & 3, csub = (warp - 2) >> 2;
-                const int acc = acc_it & 1;
-                const uint32_t acc_phase = (acc_it >> 1) & 1;
-                const int row = tile * kM + quarter * 32 + lane;
-                const bool row_ok = row < P.n;
-                mbar_wait_bounded(&tfull_bar[acc], acc_phase);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + acc * p.acc_stride + ((uint32_t)(quarter * 32) << 16);
-                for (int c = csub * 32; c < p.Bp; c += 64) {
-                    uint32_t r[32];
-                    __syncwarp();
-                    tmem_ld_32x32(taddr + c, r);
-                    tmem_ld_wait();
-                    if (row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (c + j < p.Bp) p.partial[((long long)split * p.Bp + c + j) * P.n + row] = __uint_as_float(r[j]);
-                    }
-                }
-                tc_fence_before();
+                wgmma_wait<0>();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                // ===================== epilogue: transposed f32 partial store [split][b][n] =====================
+                const int c_lo = 2 * (lane & 3);
+#pragma unroll
+                for (int hf = 0; hf < 2; ++hf) {
+                    const int row = tile * kM + cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hf;
+                    if (row >= P.n) continue;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * j + c_lo + e;
+                            if (col < p.Bp) p.partial[((long long)split * p.Bp + col) * P.n + row] = acc[4 * j + 2 * hf + e];
+                        }
+                }
             }
-            if (has) ++acc_it;   // every thread of a CTA that had work advances its accumulator parity in step
         } else {
             // the producer thread first puts the NEXT GEMM phase's weight tiles in flight (all ring stages are free: the grid barrier
             // after the previous GEMM phase implies its MMAs have retired), then joins the reduction
@@ -328,10 +311,28 @@ decoder_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainK p) {
         }
         if (ph + 1 < p.n_phases) grid_barrier(p.counters + ph, gridDim.x, P.kind != 0);
     }
+}
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, p.tmem_cols); }
+template <typename T, int BN>
+cudaError_t launch_chain(const ChainMaps& maps, const ChainK& p, int grid, size_t smem, int pdl, cudaStream_t stream) {
+    static bool attr = false;
+    if (!attr) {
+        const cudaError_t e = cudaFuncSetAttribute(decoder_chain_kernel<T, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 210 * 1024);
+        if (e != cudaSuccess) return e;
+        attr = true;
+    }
+    return launch_k(decoder_chain_kernel<T, BN>, dim3(grid), dim3(kThreads), smem, stream, pdl, maps, p);
+}
+
+template <typename T>
+cudaError_t launch_chain_n(int bn, const ChainMaps& maps, const ChainK& p, int grid, size_t smem, int pdl, cudaStream_t stream) {
+    switch (bn) {
+        case 16: return launch_chain<T, 16>(maps, p, grid, smem, pdl, stream);
+        case 32: return launch_chain<T, 32>(maps, p, grid, smem, pdl, stream);
+        case 64: return launch_chain<T, 64>(maps, p, grid, smem, pdl, stream);
+        case 128: return launch_chain<T, 128>(maps, p, grid, smem, pdl, stream);
+        default: return launch_chain<T, 256>(maps, p, grid, smem, pdl, stream);
+    }
 }
 
 }  // namespace
@@ -346,14 +347,8 @@ wk_status decoder_chain(const ChainDesc& c, int num_sms, cudaStream_t stream) {
     memset(&maps, 0, sizeof(maps));
     memset(&p, 0, sizeof(p));
     p.n_phases = c.n_phases; p.partial = c.partial; p.x = c.x; p.B = c.B; p.Bp = c.Bp; p.d = c.d; p.counters = c.counters; p.reset = c.reset_counters;
-    p.idesc = 0;
-    {
-        const uint32_t fmt = c.dtype == WK_DTYPE_F16 ? 0u : 1u;
-        uint32_t id = 0;
-        id |= 1u << 4; id |= fmt << 7; id |= fmt << 10; id |= (uint32_t)(c.Bp >> 3) << 17; id |= (uint32_t)(kM >> 4) << 24;
-        p.idesc = id;
-    }
-    p.stage_b_bytes = c.Bp * kK * 2;
+    const int bn = wgmma_tile_n(c.Bp);   // wgmma N: Bp rounded up to a power of two (rows past Bp are zero-filled by TMA)
+    p.stage_b_bytes = bn * kK * 2;
     if (p.stage_b_bytes % 1024) p.stage_b_bytes = (p.stage_b_bytes + 1023) / 1024 * 1024;
     int n_gemm = 0, max_kb = 1, last_gemm = -1;
     for (int i = 0; i < c.n_phases; ++i) {
@@ -365,7 +360,7 @@ wk_status decoder_chain(const ChainDesc& c, int num_sms, cudaStream_t stream) {
             k.map = n_gemm; k.n = s.n; k.splits = s.splits; k.kb_per_split = s.k / kK / s.splits; k.tiles = (s.n + kM - 1) / kM;
             if (k.tiles * k.splits > num_sms) { set_error("decoder_chain: GEMM phase %d needs %d CTAs (> %d SMs)", i, k.tiles * k.splits, num_sms); return WK_ERR_INVALID_ARGUMENT; }
             WK_CHECK_STATUS(make_tmap_2d(&maps.a[n_gemm], s.w, c.dtype, (uint64_t)s.k, (uint64_t)s.n, (uint64_t)s.k, kK, kM));
-            WK_CHECK_STATUS(make_tmap_2d(&maps.b[n_gemm], s.act, c.dtype, (uint64_t)s.k, (uint64_t)c.Bp, (uint64_t)s.k, kK, (uint32_t)c.Bp));
+            WK_CHECK_STATUS(make_tmap_2d(&maps.b[n_gemm], s.act, c.dtype, (uint64_t)s.k, (uint64_t)c.Bp, (uint64_t)s.k, kK, (uint32_t)bn));
             max_kb = std::max(max_kb, k.kb_per_split);
             last_gemm = i;
             ++n_gemm;
@@ -383,21 +378,11 @@ wk_status decoder_chain(const ChainDesc& c, int num_sms, cudaStream_t stream) {
     const int stage_bytes = kStageABytes + p.stage_b_bytes;
     p.stages = std::min(kRingMax, std::max(2, max_kb));
     while ((size_t)p.stages * stage_bytes + 2048 > 200 * 1024 && p.stages > 2) --p.stages;
-    p.acc_stride = 32; while (p.acc_stride < c.Bp) p.acc_stride <<= 1;
-    p.tmem_cols = std::max(32, 2 * p.acc_stride);
     const size_t smem = (size_t)p.stages * stage_bytes + 1024 + 1024;
-    cudaError_t e;
-    if (c.dtype == WK_DTYPE_F16) {
-        static bool attr = false;
-        if (!attr) { e = cudaFuncSetAttribute(decoder_chain_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 210 * 1024); if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(chain): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; } attr = true; }
-        e = launch_k(decoder_chain_kernel<__half>, dim3(num_sms), dim3(kThreads), smem, stream, c.pdl ? 16 : 0, maps, p);
-    } else {
-        static bool attr = false;
-        if (!attr) { e = cudaFuncSetAttribute(decoder_chain_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 210 * 1024); if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(chain): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; } attr = true; }
-        e = launch_k(decoder_chain_kernel<__nv_bfloat16>, dim3(num_sms), dim3(kThreads), smem, stream, c.pdl ? 16 : 0, maps, p);
-    }
+    cudaError_t e = c.dtype == WK_DTYPE_F16 ? launch_chain_n<__half>(bn, maps, p, num_sms, smem, c.pdl ? 16 : 0, stream)
+                                            : launch_chain_n<__nv_bfloat16>(bn, maps, p, num_sms, smem, c.pdl ? 16 : 0, stream);
     count_launch();
-    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("decoder_chain launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
     return WK_OK;
 }

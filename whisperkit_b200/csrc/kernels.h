@@ -12,7 +12,7 @@ void set_error(const char* fmt, ...);
 const char* last_error_cstr();
 void count_launch(int n = 1);
 
-// ---------------------------------------------------------------- GEMM (gemm_tcgen05.cu)
+// ---------------------------------------------------------------- GEMM (gemm_wgmma.cu)
 enum GemmMode {
     GEMM_OUT_T16 = 0,        // out16[row, col] = act(acc + bias[col])
     GEMM_OUT_F32_ADD = 1,    // out32[row, col] += acc + bias[col]           (residual update in place)
@@ -61,10 +61,11 @@ struct GemmDesc {
     int pdl;                 // launch with programmatic dependent launch (decode-step chain)
     int max_stages;          // 0 = as many smem stages as fit; >0 caps the ring (lets other kernels co-reside on the SM)
     int a_static;            // A operand (weights) does not depend on the upstream kernel: with PDL its first tiles are fetched before griddepcontrol.wait
-    int pair;                // run as 2-CTA clusters sharing the B (weight) tile by TMA multicast (plain 2-D, single-split GEMMs)
 };
 
-wk_status gemm_tcgen05(const GemmDesc& d, int num_sms, cudaStream_t stream);
+wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream);
+// the wgmma tile width (N) a GEMM with bn output columns per tile runs with: bn rounded up to a power of two >= 16
+int wgmma_tile_n(int bn);
 
 // ---------------------------------------------------------------- mel (mel.cu)
 struct MelTables;  // device tables (window, twiddles, sparse filterbank)
@@ -83,8 +84,8 @@ wk_status layernorm_f32_to_16(const float* x, const float* gamma, const float* b
 wk_status layernorm_f32_to_f32(const float* x, const float* gamma, const float* beta, float* out, int64_t rows, int d,
                                cudaStream_t stream);
 wk_status encoder_attention(const void* qkv, void* out, int B, int T, int n_heads, int dtype, cudaStream_t stream);
-// tcgen05/TMA implementation (attention_tcgen05.cu) behind encoder_attention()
-wk_status encoder_attention_tcgen05(const void* qkv, void* out, int B, int T, int n_heads, int dtype, cudaStream_t stream);
+// TMA + wgmma implementation (attention_wgmma.cu) behind encoder_attention()
+wk_status encoder_attention_wgmma(const void* qkv, void* out, int B, int T, int n_heads, int dtype, cudaStream_t stream);
 wk_status transpose_to_host_layout(const void* src, float* dst, int64_t B, int64_t rows, int64_t cols, int64_t src_rows_alloc,
                                    int64_t src_row_off, int64_t src_ld, int dtype, cudaStream_t stream);
 wk_status fill_random_16(void* dst, int64_t n, uint64_t seed, float std, float mean, int dtype, cudaStream_t stream);

@@ -29,7 +29,7 @@ struct wk_session {
     int max_batch = 0;        // decode slots
     int batch = 0;            // rows the step runs over: slots [0, batch) (x beam rows per slot with beam search)
     int bound_windows = 0;    // windows bound by wk_session_set_encoder_output (cross K/V blocks 0 .. bound_windows - 1)
-    int bp = 16;              // batch padded to the UMMA N granule
+    int bp = 16;              // batch padded to a multiple of 16 (the GEMM tile N granule)
     cudaStream_t stream = nullptr;      // decode stream
     cudaStream_t enc_stream = nullptr;  // mel + encoder of the batched entry
     EncWorkspace ws;                    // this session's mel / encoder activations (allocated on first use)
@@ -86,7 +86,7 @@ static wk_status dec_gemm(wk_session* s, const void* w, int N, int K, const void
     g.pdl = 1; g.a_static = 1;
     if ((size_t)g.splits * s->bp * N > s->partial_elems) { set_error("partial workspace too small"); return WK_ERR_DECODING_FAILED; }
     *splits_out = g.splits;
-    return gemm_tcgen05(g, m->num_sms, s->stream);
+    return gemm_wgmma(g, m->num_sms, s->stream);
 }
 
 // The fused phase chains hold every SM with a CTA that waits on grid-wide barriers.  Two such grids from different sessions could each
@@ -192,7 +192,7 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
         g.m_rows_per_batch = c.vocab; g.n = Bp; g.k = d; g.taps = 1; g.bn = Bp; g.splits = 1;
         g.mode = GEMM_OUT_PARTIAL_T; g.out = s->logits; g.ld_out = c.vocab; g.out_rows_per_batch = c.vocab; g.partial_cols = B;
         g.pdl = 1; g.a_static = 1;
-        WK_CHECK(gemm_tcgen05(g, m->num_sms, st));
+        WK_CHECK(gemm_wgmma(g, m->num_sms, st));
     }
     return WK_OK;
 }
@@ -626,7 +626,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         GemmDesc g = plain_gemm(src, (int64_t)cnt * T, d, m->wckv, 2 * c.dec_layers * d, c.dtype, GEMM_OUT_T16_HEADS,
                                 (char*)s->cross_kv + (size_t)q0 * c.n_heads * T * 64 * 2, 0, m->bckv, 0);
         g.heads_T = T; g.heads_B = s->max_batch; g.heads_H = c.n_heads; g.heads_dmodel = d;
-        return gemm_tcgen05(g, m->num_sms, s->stream);
+        return gemm_wgmma(g, m->num_sms, s->stream);
     };
 
     int64_t finished = 0;
@@ -816,9 +816,8 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     s->m = m;
     s->max_batch = S;
     // A/B switches, read once per session (never on the step path).  WKB200_FUSED=1 runs the decoder's GEMM / reduce phases as persistent
-    // chains with grid barriers (fused_chain.cu): bit-identical, but measured SLOWER on B200 than one PDL-chained launch per phase
-    // (64 windows: 1252 vs 1198 ms per pass; a phase costs ~4.5 us of dependent L2 round trips either way and a grid barrier is no
-    // cheaper than a programmatic kernel boundary), so it is off by default.  WKB200_NO_GRAPH=1 replays nothing.
+    // chains with grid barriers (fused_chain.cu): bit-identical, but a phase costs dependent L2 round trips
+    // either way and a grid barrier is no cheaper than a programmatic kernel boundary, so it is off by default.  WKB200_NO_GRAPH=1 replays nothing.
     if (const char* e = getenv("WKB200_FUSED")) s->knob_fused = atoi(e) != 0;
     s->knob_graph = getenv("WKB200_NO_GRAPH") == nullptr;
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
@@ -940,7 +939,7 @@ wk_status wk_session_set_encoder_output(wk_session* s, const wk_tensor* enc) {
     for (cudaEvent_t e : enc->events) WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, e, 0));
     GemmDesc g = plain_gemm(enc->data, (int64_t)s->batch * T, d, m->wckv, 2 * c.dec_layers * d, c.dtype, GEMM_OUT_T16_HEADS, s->cross_kv, 0, m->bckv, 0);
     g.heads_T = T; g.heads_B = s->max_batch; g.heads_H = c.n_heads; g.heads_dmodel = d;
-    WK_CHECK(gemm_tcgen05(g, m->num_sms, s->stream));
+    WK_CHECK(gemm_wgmma(g, m->num_sms, s->stream));
     cudaEvent_t ev;
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventRecord(ev, s->stream));
@@ -1137,11 +1136,11 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
         int sp;
         switch (which) {
             case 0: return decoder_cross_attention(s->partial, 1, s->bp, m->dec[0].bcq, s->cross_kv, (char*)s->cross_kv + cross_block, s->attn, B, H, T, dt, st);
-            case 1: return gemm_tcgen05(plain_gemm(s->ws.xn, M, d, m->enc[0].w1, 4 * d, dt, GEMM_OUT_T16, s->ws.ffn, 4 * d, m->enc[0].b1, 1), m->num_sms, st);
+            case 1: return gemm_wgmma(plain_gemm(s->ws.xn, M, d, m->enc[0].w1, 4 * d, dt, GEMM_OUT_T16, s->ws.ffn, 4 * d, m->enc[0].b1, 1), m->num_sms, st);
             case 2: return mel_forward(m->mel_tables, s->ws.pcm_dev, B, kWindowSamples, nullptr, s->ws.mel, s->ws.gmax, st);
             case 3: return encoder_attention(s->ws.qkv, s->ws.attn, B, T, H, dt, st);
             case 4: return dec_gemm(s, m->dec[0].wqkv, 3 * d, d, s->xn, &sp);
-            case 5: return gemm_tcgen05(plain_gemm(s->ws.xn, M, d, m->enc[0].wqkv, 3 * d, dt, GEMM_OUT_T16, s->ws.qkv, 3 * d, m->enc[0].bqkv, 0), m->num_sms, st);
+            case 5: return gemm_wgmma(plain_gemm(s->ws.xn, M, d, m->enc[0].wqkv, 3 * d, dt, GEMM_OUT_T16, s->ws.qkv, 3 * d, m->enc[0].bqkv, 0), m->num_sms, st);
             case 6: return dec_gemm(s, m->dec[0].wo, d, d, s->attn, &sp);
             case 7: return dec_gemm(s, m->dec[0].w2, d, 4 * d, s->ffn, &sp);
             case 8: return decoder_reduce_resid_ln(s->partial, choose_splits((d + 127) / 128, d / 64, m->num_sms), s->bp, m->dec[0].bo, m->dec[0].lnx.g, m->dec[0].lnx.b, s->x, s->xn, B, d, dt, st);

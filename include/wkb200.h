@@ -59,7 +59,8 @@ typedef struct wk_model wk_model;
 typedef struct wk_session wk_session;
 typedef struct wk_tensor wk_tensor;
 
-enum { WK_DTYPE_F32 = 0, WK_DTYPE_F16 = 1, WK_DTYPE_BF16 = 2, WK_DTYPE_I32 = 3 };
+enum { WK_DTYPE_F32 = 0, WK_DTYPE_F16 = 1, WK_DTYPE_BF16 = 2, WK_DTYPE_I32 = 3,
+       WK_DTYPE_FP8_E4M3 = 4 /* cross-attention K/V cache only: E4M3 codes + one f32 scale per 64-value row */ };
 
 /* Model dimensions.  The reference reads these off the CoreML model descriptions at run time
  * (TextDecoder.swift:313-331, AudioEncoder.swift:24-38, FeatureExtractor.swift:24-38). */
@@ -84,6 +85,7 @@ typedef struct wk_model_info {
     int32_t has_alignment_heads;
     int32_t is_multilingual; /* logitsSize != 51864 (ModelUtilities.swift:124-126) */
     int32_t dtype, max_batch;
+    int32_t cross_kv_dtype;  /* storage of the cross-attention K/V cache: dtype, or WK_DTYPE_FP8_E4M3 */
 } wk_model_info;
 
 /* SpecialTokens (Models.swift:1111-1149) - supplied by the host tokenizer. */
@@ -161,6 +163,15 @@ wk_status wk_model_load(const char* weights_dir, int32_t device, int32_t max_bat
 /* Seeded synthetic weights generated on the device (benchmarks: no checkpoints are available offline). */
 wk_status wk_model_init_random(wk_model* m, uint64_t seed, float std);
 wk_status wk_model_info_get(const wk_model* m, wk_model_info* out);
+/* Storage of the decoder's cross-attention K/V cache (default: the model's dtype).  WK_DTYPE_FP8_E4M3 stores each
+ * (window, layer, K|V, head, position) row of 64 values as 64 E4M3 codes plus one f32 scale s = amax(|row|) / 448,
+ * code = cvt.rn.satfinite.e4m3(x / s) (s = 0 and zero codes for an all-zero row): 0.53x the bytes the decode loop streams per step
+ * and a cache about half the size; K and V keep 3 mantissa bits (4 fewer than bf16, 7 fewer than f16) under a per-row scale.  Accepts WK_DTYPE_FP8_E4M3 or the model's own dtype;
+ * works after wk_model_create or wk_model_load and must be called before the model's first wk_session_create (WK_ERR_INVALID_ARGUMENT
+ * after that). */
+wk_status wk_model_set_cross_kv_dtype(wk_model* m, int32_t dtype);
+/* The FP8 row quantizer above on the host (the code the GPU projection epilogue runs): x [rows][64] f32 -> codes [rows][64], scales [rows]. */
+wk_status wk_cross_kv_quantize_rows(const float* x, int64_t rows, uint8_t* codes, float* scales);
 void wk_model_free(wk_model* m);
 
 /* ---- tensors (opaque device buffers passed mel -> encoder -> decoder without touching the host) ---- */
@@ -439,6 +450,12 @@ wk_status wk_test_cross_attention(wk_model* m, const float* q, const void* kcros
 /* The beam-search form of the same kernel: groups of kv_div adjacent rows share one K/V block, K/V [B / kv_div][H][T][64]. */
 wk_status wk_test_cross_attention_shared(wk_model* m, const float* q, const void* kcross, const void* vcross, void* out, int32_t B, int32_t H,
                                          int32_t T, int32_t dtype, const int32_t* done, int32_t kv_div);
+/* FP8-cache form of both: K/V codes [B / kv_div][H][T][64] (E4M3) with row scales [B / kv_div][H][T] f32; dtype is the type of out;
+ * kv_div = 1 runs the single-query kernel, 2..8 the beam kernel.  align_out (device, may be NULL): every head also writes its normalised
+ * softmax row to align_out [H][B][T] (the word-timestamp export; runs the single-query kernel whatever kv_div is). */
+wk_status wk_test_cross_attention_fp8(wk_model* m, const float* q, const uint8_t* kcodes, const uint8_t* vcodes, const float* kscale,
+                                      const float* vscale, void* out, int32_t B, int32_t H, int32_t T, int32_t dtype, const int32_t* done,
+                                      int32_t kv_div, float* align_out);
 /* Decoder self-attention kernel alone: qkv [B][3*H*64] f32 of the new token, caches [B][H][224][64] 16-bit (positions < pos[b] valid;
  * row pos[b] is appended), pos [B] device -> out [B][H*64] 16-bit. */
 wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, void* vcache, const int32_t* pos, void* out, int32_t B,
@@ -446,10 +463,12 @@ wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, vo
 
 /* Average device time (ms) of one launch of a named hot kernel on the live buffers, plus its algorithmic work
  * (bytes for HBM-bound kernels, FLOPs for tensor-bound ones): 0 decoder cross-attention, 1 encoder FC1 GEMM,
- * 2 log-mel, 3 encoder attention, 4 decoder QKV swap-AB GEMM, 5 encoder QKV GEMM.  Used by bench.py's roofline. */
+ * 2 log-mel, 3 encoder attention, 4 decoder QKV swap-AB GEMM, 5 encoder QKV GEMM.  Used by bench.py's roofline.
+ * Kernel 0 of a session with an FP8 cross K/V cache runs the FP8 kernel and counts its bytes (codes + row scales). */
 wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t batch, int32_t iters, float* ms_out, double* work_out);
 
-/* Debug readback of an internal device buffer converted to f32 (stage-by-stage parity debugging; see engine.cu). */
+/* Debug readback of an internal device buffer converted to f32 (stage-by-stage parity debugging; see session.cu).  An FP8 cross K/V
+ * cache (which = 15) is returned dequantized: code * row scale. */
 wk_status wk_debug_read(wk_model* m, wk_session* s, int32_t which, int64_t offset_elems, float* dst, int64_t n);
 
 #ifdef __cplusplus

@@ -12,6 +12,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libwkb200.so")
 
 WK_DTYPE_F32, WK_DTYPE_F16, WK_DTYPE_BF16, WK_DTYPE_I32 = 0, 1, 2, 3
+WK_DTYPE_FP8_E4M3 = 4   # cross-attention K/V cache storage only
 
 STATUS_NAMES = {
     0: "ok", -1: "invalidArgument", -2: "modelsUnavailable", -3: "audioProcessingFailed",
@@ -37,7 +38,8 @@ class wk_model_config(C.Structure):
 class wk_model_info(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_mels", "n_audio_ctx", "d_model", "n_heads", "enc_layers", "dec_layers",
                                          "vocab", "kv_embed_dim", "kv_max_len", "window_samples",
-                                         "has_alignment_heads", "is_multilingual", "dtype", "max_batch")]
+                                         "has_alignment_heads", "is_multilingual", "dtype", "max_batch",
+                                         "cross_kv_dtype")]
 
 
 class wk_special_tokens(C.Structure):
@@ -120,6 +122,8 @@ SYMBOLS = [
     ("wk_model_load", I32, [C.c_char_p, I32, I32, I32, C.POINTER(P)]),
     ("wk_model_init_random", I32, [P, C.c_uint64, F32]),
     ("wk_model_info_get", I32, [P, C.POINTER(wk_model_info)]),
+    ("wk_model_set_cross_kv_dtype", I32, [P, I32]),
+    ("wk_cross_kv_quantize_rows", I32, [P, I64, P, P]),
     ("wk_model_free", None, [P]),
     ("wk_tensor_shape", I32, [P, PI64, PI32, PI32]),
     ("wk_tensor_to_host", I32, [P, P, I64]),
@@ -207,6 +211,7 @@ SYMBOLS = [
     ("wk_test_gemm", I32, [P, P, P, P, P, I32, I32, I32, I32, I32, I32]),
     ("wk_test_cross_attention", I32, [P, P, P, P, P, I32, I32, I32, I32, P]),
     ("wk_test_cross_attention_shared", I32, [P, P, P, P, P, I32, I32, I32, I32, P, I32]),
+    ("wk_test_cross_attention_fp8", I32, [P, P, P, P, P, P, P, I32, I32, I32, I32, P, I32, P]),
     ("wk_test_self_attention", I32, [P, P, P, P, P, P, I32, I32, I32, P]),
     ("wk_test_gemm_residual", I32, [P, P, P, P, P, I32, I32, I32, I32]),
     ("wk_test_gemm_splitk", I32, [P, P, P, P, I32, I32, I32, I32, I32]),

@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -36,6 +37,35 @@ template <> struct T16<__half> {
         return __half22float2(t);
     }
 };
+
+// ------------------------------------------------------------------ FP8 (E4M3) cross-attention K/V rows
+// A row of 64 values is stored as 64 E4M3 codes plus one f32 scale s = amax(|row|) / 448; code = cvt.rn.satfinite.e4m3(x / s) and the
+// stored value is code * s.  A row whose amax is 0 gets s = 0 and all-zero codes.  The GEMM epilogue (gemm_wgmma.cu) and the host test
+// entry (wk_cross_kv_quantize_rows) both go through these two functions, so the CPU tests pin the rounding the GPU does.
+constexpr float kFp8E4M3Max = 448.f;
+__host__ __device__ __forceinline__ float fp8_row_scale(float amax) { return amax / kFp8E4M3Max; }
+__host__ __device__ __forceinline__ uint8_t fp8_encode(float x, float s) {
+    return s > 0.f ? (uint8_t)__nv_cvt_float_to_fp8(x / s, __NV_SATFINITE, __NV_E4M3) : (uint8_t)0;
+}
+__host__ __device__ inline void fp8_quantize_row(const float* x, int n, uint8_t* codes, float* scale) {
+    float amax = 0.f;
+    for (int i = 0; i < n; ++i) amax = fmaxf(amax, fabsf(x[i]));
+    const float s = fp8_row_scale(amax);
+    for (int i = 0; i < n; ++i) codes[i] = fp8_encode(x[i], s);
+    *scale = s;
+}
+// code -> value (exact: every E4M3 value is a f16 value)
+__host__ __device__ inline float fp8_decode(uint8_t code) {
+    const __half_raw h = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)code, __NV_E4M3);
+    return __half2float(__half(h));
+}
+// four codes (little-endian in a word) -> two exact f16 pairs (cvt.rn.f16x2.e4m3x2)
+__device__ __forceinline__ void fp8x4_to_half2(uint32_t w, uint32_t& lo, uint32_t& hi) {
+    const __half2_raw a = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w & 0xffffu), __NV_E4M3);
+    const __half2_raw b = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w >> 16), __NV_E4M3);
+    lo = (uint32_t)a.x | ((uint32_t)a.y << 16);
+    hi = (uint32_t)b.x | ((uint32_t)b.y << 16);
+}
 
 __device__ __forceinline__ float gelu_erf(float x) {
     // exact (erf) GELU with erf from Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, far below the 16-bit storage step of the output):

@@ -9,12 +9,16 @@
 //                       B = K tile rows straight from the swizzled ring with ldmatrix
 //   out    = P V        A = P (f32 probabilities from smem, hi + lo split on the fly), B = V tile with ldmatrix.trans
 // Softmax is exact two-pass over the f32 scores in shared memory (one warp per beam row, no block barriers inside).
+// FP8 cache (FP8 = true): the TMA brings 64-byte rows of E4M3 codes, each consumer warp widens its rows exactly to 16-bit (mq_widen_fp8) and
+// the MMA path is unchanged; the K row scale multiplies the scores, p carries the V row scale relative to the block's largest one.
 // 4 consumer warps (each owns a quarter of every tile's keys) + 1 TMA producer warp; the K tiles do not depend on the upstream kernel
 // (the cross K/V cache is written before the decode loop), so the producer starts before griddepcontrol.wait.
 // Reference counterpart: the cross-attention inside TextDecoder.mlmodelc (Sources/WhisperKit/Core/TextDecoder.swift:394-417); beam
 // semantics are the self-oracle's (oracle/beam_ref.py), the reference's own beam sampler being a stub (TokenSampler.swift:254-290).
 #include <stdio.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -53,20 +57,49 @@ template <typename T> __device__ __forceinline__ void mq_split2(float x, float y
     lo = T16<T>::pack2(x - h.x, y - h.y);
 }
 
-template <typename T, int NQ, int STAGES>
+// FP8 cache: a warp widens its 32 rows of the E4M3 tile (rows 32 w .. 32 w + 31, the only rows its ldmatrix reads) exactly to 16-bit into
+// its own 4 KiB buffer, in the 128B-swizzled layout the TMA gives the 16-bit tiles, so the MMA code below is the same for both caches
+template <typename T>
+__device__ __forceinline__ void mq_widen_fp8(const uint8_t* tile, uint8_t* wbuf, int warp, int lane) {
+#pragma unroll 1
+    for (int it = 0; it < 8; ++it) {
+        const int idx = it * 32 + lane, row = idx >> 3, chunk = idx & 7;   // 8 codes -> 16-byte chunk `chunk` of the 16-bit row
+        const uint2 u = *reinterpret_cast<const uint2*>(tile + (warp * 32 + row) * 64 + chunk * 8);
+        uint32_t h[4];
+        fp8x4_to_half2(u.x, h[0], h[1]);
+        fp8x4_to_half2(u.y, h[2], h[3]);
+        if constexpr (!std::is_same<T, __half>::value) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float2 a = T16<__half>::unpack2(h[k]);
+                h[k] = T16<T>::pack2(a.x, a.y);
+            }
+        }
+        *reinterpret_cast<uint4*>(wbuf + row * 128 + ((chunk ^ (row & 7)) << 4)) = make_uint4(h[0], h[1], h[2], h[3]);
+    }
+}
+
+template <typename T, int NQ, int STAGES, bool FP8>
 __global__ void __launch_bounds__(kMqThreads)
 decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
                                   const float* __restrict__ partial, int splits, int Bp, const float* __restrict__ bq, T* __restrict__ out, int H,
-                                  int Tlen, int chunks, const int32_t* __restrict__ done) {
+                                  int Tlen, int chunks, const int32_t* __restrict__ done, const float* __restrict__ kscale,
+                                  const float* __restrict__ vscale) {
+    constexpr int kStage = FP8 ? kMqRows * 64 : kMqStageBytes;   // bytes of one TMA tile
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));   // STAGES x 16 KiB
+    uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));   // STAGES x kStage
     const int Tp = chunks * kMqRows;
-    float* scores = reinterpret_cast<float*>(ring + STAGES * kMqStageBytes);   // [NQ][Tp]: raw scores, then probabilities
+    float* scores = reinterpret_cast<float*>(ring + STAGES * kStage);          // [NQ][Tp]: raw scores, then probabilities
     float* sq = scores + NQ * Tp;                                              // [NQ][64]
     float* red = sq + NQ * 64;                                                 // [4][NQ][64]
     float* stat = red + 4 * NQ * 64;                                           // [NQ] 1 / row sum  (padded to 8)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(stat + 8);
     uint64_t* empty_bar = full_bar + STAGES;
+    // FP8 only: K / V row scales [Tp] each, the V-scale maximum (+ per-warp scratch), the widened 16-bit tiles [4 warps][32 rows][128 B]
+    float* ksc = reinterpret_cast<float*>(empty_bar + STAGES);
+    float* vsc = ksc + Tp;
+    float* vmax_s = vsc + Tp;
+    uint8_t* wbuf = reinterpret_cast<uint8_t*>(vmax_s + 8);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int win = blockIdx.x / H, h = blockIdx.x % H;
@@ -88,8 +121,8 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
                 const int stage = c % STAGES;
                 const uint32_t ph = (c / STAGES) & 1;
                 mbar_wait_bounded(&empty_bar[stage], ph ^ 1);
-                mbar_expect_tx(&full_bar[stage], kMqStageBytes);
-                tma_load_3d(ring + stage * kMqStageBytes, c < chunks ? &tm_k : &tm_v, &full_bar[stage], 0, (c < chunks ? c : c - chunks) * kMqRows,
+                mbar_expect_tx(&full_bar[stage], kStage);
+                tma_load_3d(ring + stage * kStage, c < chunks ? &tm_k : &tm_v, &full_bar[stage], 0, (c < chunks ? c : c - chunks) * kMqRows,
                             (int)blockIdx.x);
             }
         }
@@ -102,7 +135,20 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
         for (int s = 0; s < splits; ++s) q += partial[((long long)s * Bp + r0 + j) * dm + h * 64 + e];
         sq[i] = q * 0.125f;
     }
+    if constexpr (FP8) {   // row scales of this (window, head); keys past Tlen get 0.  V scales are used relative to their maximum
+        float vm = 0.f;
+        for (int t = tid; t < Tp; t += 128) {
+            ksc[t] = t < Tlen ? kscale[(long long)blockIdx.x * Tlen + t] : 0.f;
+            vsc[t] = t < Tlen ? vscale[(long long)blockIdx.x * Tlen + t] : 0.f;
+            vm = fmaxf(vm, vsc[t]);
+        }
+        vm = warp_max(vm);
+        if (lane == 0) vmax_s[warp] = vm;
+    }
     asm volatile("bar.sync 1, 128;" ::: "memory");
+    // FP8: p carries vsc[t] / vmax (at most 1, so the hi + lo split of p keeps its range) and the output is scaled back by vmax
+    const float vmax = FP8 ? fmaxf(fmaxf(vmax_s[0], vmax_s[1]), fmaxf(vmax_s[2], vmax_s[3])) : 1.f;
+    const float inv_vmax = vmax > 0.f ? 1.f / vmax : 0.f;
     const int g = lane >> 2, tq = lane & 3;          // fragment row (query) and column pair
     const int lm = lane >> 3, lr = lane & 7;         // ldmatrix: which of the four 8x8 matrices this lane addresses, and its row
     uint32_t qh[4][2], ql[4][2];                     // A fragments of Q per 16-wide k-step: columns 2tq.. and 8+2tq.., hi and lo halves
@@ -118,7 +164,13 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
     for (int c = 0; c < chunks; ++c) {
         const int stage = c % STAGES;
         mbar_wait_bounded(&full_bar[stage], (c / STAGES) & 1);
-        const uint32_t tile = smem_u32(ring + stage * kMqStageBytes);
+        uint32_t tile = smem_u32(ring + stage * kStage);
+        if constexpr (FP8) {   // widen this warp's rows, release the stage, read the 16-bit copy (same row addressing)
+            mq_widen_fp8<T>(ring + stage * kStage, wbuf + warp * 4096, warp, lane);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            tile = smem_u32(wbuf + warp * 4096) - warp * 4096;
+        }
 #pragma unroll
         for (int gi = 0; gi < 4; ++gi) {
             const int kg = warp * 4 + gi;
@@ -133,10 +185,14 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
                 mq_mma<T>(cacc, qh[ks][0], qh[ks][1], b0, b1);
                 mq_mma<T>(cacc, ql[ks][0], ql[ks][1], b0, b1);
             }
+            if constexpr (FP8) {
+                const int t = c * kMqRows + kg * 8 + 2 * tq;
+                cacc[0] *= ksc[t]; cacc[1] *= ksc[t + 1];
+            }
             if (g < NQ) *reinterpret_cast<float2*>(scores + g * Tp + c * kMqRows + kg * 8 + 2 * tq) = make_float2(cacc[0], cacc[1]);
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (!FP8 && lane == 0) mbar_arrive(&empty_bar[stage]);
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     // ---- exact two-pass softmax, one warp per beam row; keys past Tlen (zero-filled K rows) get probability 0
@@ -153,7 +209,7 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
         }
         for (int t = Tlen + lane; t < Tp; t += 32) sc[t] = 0.f;
         sm = warp_sum(sm);
-        if (lane == 0) stat[j] = 1.f / (sm * kMqPScale);
+        if (lane == 0) stat[j] = (FP8 ? vmax : 1.f) / (sm * kMqPScale);
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     // ---- V phase: out_j[d] = sum_t p_j[t] V[t][d]; warp w takes k-steps 2w, 2w+1 (16 keys each) of every tile, all 64 output columns
@@ -165,13 +221,23 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
     for (int c = chunks; c < 2 * chunks; ++c) {
         const int stage = c % STAGES;
         mbar_wait_bounded(&full_bar[stage], (c / STAGES) & 1);
-        const uint32_t tile = smem_u32(ring + stage * kMqStageBytes);
+        uint32_t tile = smem_u32(ring + stage * kStage);
+        if constexpr (FP8) {   // widen this warp's rows, release the stage, read the 16-bit copy (same row addressing)
+            mq_widen_fp8<T>(ring + stage * kStage, wbuf + warp * 4096, warp, lane);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            tile = smem_u32(wbuf + warp * 4096) - warp * 4096;
+        }
 #pragma unroll
         for (int ki = 0; ki < 2; ++ki) {
             const int ks = warp * 2 + ki;
             const float* pr = scores + g * Tp + (c - chunks) * kMqRows + ks * 16 + 2 * tq;
-            const float2 p0 = g < NQ ? *reinterpret_cast<const float2*>(pr) : make_float2(0.f, 0.f);
-            const float2 p1 = g < NQ ? *reinterpret_cast<const float2*>(pr + 8) : make_float2(0.f, 0.f);
+            float2 p0 = g < NQ ? *reinterpret_cast<const float2*>(pr) : make_float2(0.f, 0.f);
+            float2 p1 = g < NQ ? *reinterpret_cast<const float2*>(pr + 8) : make_float2(0.f, 0.f);
+            if constexpr (FP8) {
+                const float* vs = vsc + (c - chunks) * kMqRows + ks * 16 + 2 * tq;
+                p0.x *= vs[0] * inv_vmax; p0.y *= vs[1] * inv_vmax; p1.x *= vs[8] * inv_vmax; p1.y *= vs[9] * inv_vmax;
+            }
             uint32_t ah0, al0, ah2, al2;
             mq_split2<T>(p0.x, p0.y, ah0, al0);
             mq_split2<T>(p1.x, p1.y, ah2, al2);
@@ -187,7 +253,7 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
             }
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (!FP8 && lane == 0) mbar_arrive(&empty_bar[stage]);
     }
     if (g < NQ) {
 #pragma unroll
@@ -207,30 +273,32 @@ typedef CUresult (*PFN_encodeTiledMq)(CUtensorMap*, CUtensorMapDataType, cuuint3
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 template <int NQ> static constexpr int mq_stages() { return NQ <= 5 ? 4 : 3; }
-template <int NQ> static size_t mq_smem_bytes(int chunks) {
-    return 1024 + (size_t)mq_stages<NQ>() * kMqStageBytes + (size_t)NQ * chunks * kMqRows * 4 + (size_t)NQ * 64 * 4 + (size_t)4 * NQ * 64 * 4 + 8 * 4 +
-           2 * mq_stages<NQ>() * 8 + 64;
+template <int NQ, bool FP8> static size_t mq_smem_bytes(int chunks) {
+    const size_t fp8_extra = FP8 ? (size_t)2 * chunks * kMqRows * 4 + 8 * 4 + 4 * 32 * 128 : 0;   // row scales, V-scale maximum, widened tiles
+    return 1024 + (size_t)mq_stages<NQ>() * (FP8 ? kMqRows * 64 : kMqStageBytes) + (size_t)NQ * chunks * kMqRows * 4 + (size_t)NQ * 64 * 4 +
+           (size_t)4 * NQ * 64 * 4 + 8 * 4 + 2 * mq_stages<NQ>() * 8 + fp8_extra + 64;
 }
 
-template <typename T, int NQ>
+template <typename T, int NQ, bool FP8>
 static wk_status launch_mq(const CUtensorMap& tmk, const CUtensorMap& tmv, const float* partial, int splits, int Bp, const float* bq, void* out, int B, int H,
-                           int Tlen, int chunks, const int32_t* done, cudaStream_t stream) {
+                           int Tlen, int chunks, const int32_t* done, const float* kscale, const float* vscale, cudaStream_t stream) {
     constexpr int ST = mq_stages<NQ>();
-    const size_t smem = mq_smem_bytes<NQ>(chunks);
+    const size_t smem = mq_smem_bytes<NQ, FP8>(chunks);
     if (smem > 227 * 1024) { set_error("decoder_cross_attention (beam): %d encoder positions do not fit shared memory", Tlen); return WK_ERR_INVALID_ARGUMENT; }
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_mq_kernel<T, NQ, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_mq_kernel<T, NQ, ST, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(cross mq): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
         attr_set = true;
     }
-    launch_k(decoder_cross_attention_mq_kernel<T, NQ, ST>, dim3((B / NQ) * H), dim3(kMqThreads), smem, stream, 4, tmk, tmv, partial, splits, Bp, bq, (T*)out, H,
-             Tlen, chunks, done);
+    launch_k(decoder_cross_attention_mq_kernel<T, NQ, ST, FP8>, dim3((B / NQ) * H), dim3(kMqThreads), smem, stream, 4, tmk, tmv, partial, splits, Bp, bq, (T*)out, H,
+             Tlen, chunks, done, kscale, vscale);
     return WK_OK;
 }
 
 wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, void* out, int B, int H,
-                                     int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq) {
+                                     int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq, const float* kscale,
+                                     const float* vscale) {
     if (nq < 2 || nq > 8 || B % nq != 0) { set_error("decoder_cross_attention (beam): %d rows, groups of %d", B, nq); return WK_ERR_INVALID_ARGUMENT; }
     static PFN_encodeTiledMq enc = nullptr;
     if (!enc) {
@@ -243,23 +311,28 @@ wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, c
         enc = reinterpret_cast<PFN_encodeTiledMq>(fp);
     }
     const int chunks = (Tlen + kMqRows - 1) / kMqRows;
+    const bool fp8 = kscale != nullptr;
     CUtensorMap tmk, tmv;
+    const cuuint64_t row_bytes = fp8 ? 64 : 128;   // FP8: unswizzled 64-byte rows of codes, widened by the consumers
     cuuint64_t gdim[3] = {64, (cuuint64_t)Tlen, (cuuint64_t)(B / nq) * H};
-    cuuint64_t gstr[2] = {128, (cuuint64_t)Tlen * 128};
+    cuuint64_t gstr[2] = {row_bytes, (cuuint64_t)Tlen * row_bytes};
     cuuint32_t box[3] = {64, (cuuint32_t)kMqRows, 1};
     cuuint32_t es[3] = {1, 1, 1};
-    const CUtensorMapDataType dt = dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    CUresult r = enc(&tmk, dt, 3, const_cast<void*>(kcross), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+    const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const CUtensorMapSwizzle sw = fp8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
+    CUresult r = enc(&tmk, dt, 3, const_cast<void*>(kcross), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r == CUDA_SUCCESS)
-        r = enc(&tmv, dt, 3, const_cast<void*>(vcross), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+        r = enc(&tmv, dt, 3, const_cast<void*>(vcross), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cross-attention tensor map encode failed: %d", (int)r); return WK_ERR_CUDA; }
     wk_status st = WK_OK;
-#define WK_MQ(N) case N: st = dtype == WK_DTYPE_F16 ? launch_mq<__half, N>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, stream) \
-                                                    : launch_mq<__nv_bfloat16, N>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, stream); break;
+#define WK_MQ_T(N, F) (dtype == WK_DTYPE_F16 ? launch_mq<__half, N, F>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, kscale, vscale, stream) \
+                                           : launch_mq<__nv_bfloat16, N, F>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, kscale, vscale, stream))
+#define WK_MQ(N) case N: st = fp8 ? WK_MQ_T(N, true) : WK_MQ_T(N, false); break;
     switch (nq) { WK_MQ(2) WK_MQ(3) WK_MQ(4) WK_MQ(5) WK_MQ(6) WK_MQ(7) WK_MQ(8) default: break; }
 #undef WK_MQ
+#undef WK_MQ_T
     if (st != WK_OK) return st;
     count_launch();
     cudaError_t e = cudaGetLastError();

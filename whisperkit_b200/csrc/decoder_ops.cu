@@ -418,27 +418,86 @@ wk_status decoder_self_attention(const float* partial, int splits, int Bp, const
 
 // =====================================================================================================
 // cross attention for one query per (b, h) over T encoder positions.  HBM-streaming kernel: each CTA pulls its
-// contiguous K block then V block (T x 64 x 2 B each) through a 4-deep ring of 16 KB bulk-copy stages
-// (cp.async.bulk + mbarrier), a dedicated producer warp keeps the ring full while 4 consumer warps compute.
-// K/V layout [B][H][T][64] (written head-major by the cross-KV GEMM epilogue).
+// contiguous K block then V block through a ring of 16000-byte bulk-copy stages (cp.async.bulk + mbarrier), a dedicated producer warp
+// keeps the ring full while 4 consumer warps compute.  K/V layout [B][H][T][64] (written head-major by the cross-KV GEMM epilogue).
+//   16-bit cache: 128-byte rows, 125 rows per stage, 4 stages; a lane takes 8 values (16 bytes) of a row.
+//   FP8 cache (FP8 = true): 64-byte rows of E4M3 codes with one f32 scale per row ([B][H][T], see fp8_row_scale), 250 rows per stage,
+//   3 stages (3 CTAs per SM, as the 16-bit kernel has); the producer first bulk-loads the block's two scale vectors, a lane widens 16
+//   codes exactly to f32, the K scale multiplies each key's dot product before the softmax and the V scale is folded into p for the P.V
+//   phase - the alignment export stays the normalised softmax row.
 // =====================================================================================================
-static constexpr int kCrossRows = 125;              // rows per stage: 125 * 128 B = 16000 B (multiple of 16)
-static constexpr int kCrossStageBytes = kCrossRows * 128;
-static constexpr int kCrossStages = 4;
+template <bool FP8> struct CrossCfg {
+    static constexpr int kRowBytes = FP8 ? 64 : 128;
+    static constexpr int kRows = FP8 ? 250 : 125;             // rows per stage: kRows * kRowBytes = 16000 B (multiple of 16)
+    static constexpr int kStageBytes = kRows * kRowBytes;
+    static constexpr int kStages = FP8 ? 3 : 4;
+    static constexpr int kLanesPerRow = kRowBytes / 16;       // a lane reads 16 bytes of a row
+    static constexpr int kRowsPerWarp = 32 / kLanesPerRow;    // rows per warp instruction
+    static constexpr int kDims = 64 / kLanesPerRow;           // values per lane
+};
+static constexpr int kCrossRows = CrossCfg<false>::kRows;
 static constexpr int kCrossThreads = 160;           // 4 consumer warps + 1 producer warp
 
-template <typename T>
+__device__ __forceinline__ void fp8x16_to_f32(const uint4 u, float (&x)[16]) {
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        uint32_t lo, hi;
+        fp8x4_to_half2(w[k], lo, hi);
+        const float2 a = T16<__half>::unpack2(lo), b = T16<__half>::unpack2(hi);
+        x[4 * k] = a.x; x[4 * k + 1] = a.y; x[4 * k + 2] = b.x; x[4 * k + 3] = b.y;
+    }
+}
+// q . (this lane's 16 bytes of a K row)
+template <typename T, bool FP8>
+__device__ __forceinline__ float cross_row_dot(const uint8_t* piece, const float (&qv)[CrossCfg<FP8>::kDims]) {
+    const uint4 u = *reinterpret_cast<const uint4*>(piece);
+    if constexpr (FP8) {
+        float x[16];
+        fp8x16_to_f32(u, x);
+        float acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) acc = fmaf(qv[j], x[j], acc);
+        return acc;
+    } else {
+        const float2 a0 = T16<T>::unpack2(u.x), a1 = T16<T>::unpack2(u.y), a2 = T16<T>::unpack2(u.z), a3 = T16<T>::unpack2(u.w);
+        return qv[0] * a0.x + qv[1] * a0.y + qv[2] * a1.x + qv[3] * a1.y + qv[4] * a2.x + qv[5] * a2.y + qv[6] * a3.x + qv[7] * a3.y;
+    }
+}
+// acc += p * (this lane's 16 bytes of a V row)
+template <typename T, bool FP8>
+__device__ __forceinline__ void cross_row_axpy(const uint8_t* piece, float p, float (&acc)[CrossCfg<FP8>::kDims]) {
+    const uint4 u = *reinterpret_cast<const uint4*>(piece);
+    if constexpr (FP8) {
+        float x[16];
+        fp8x16_to_f32(u, x);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) acc[j] = fmaf(p, x[j], acc[j]);
+    } else {
+        const float2 a0 = T16<T>::unpack2(u.x), a1 = T16<T>::unpack2(u.y), a2 = T16<T>::unpack2(u.z), a3 = T16<T>::unpack2(u.w);
+        acc[0] += p * a0.x; acc[1] += p * a0.y; acc[2] += p * a1.x; acc[3] += p * a1.y;
+        acc[4] += p * a2.x; acc[5] += p * a2.y; acc[6] += p * a3.x; acc[7] += p * a3.y;
+    }
+}
+
+template <typename T, bool FP8>
 __global__ void __launch_bounds__(kCrossThreads)
 decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, int Bp, const float* __restrict__ bq,
-                               const T* __restrict__ kcross, const T* __restrict__ vcross, T* __restrict__ out, int B, int H,
-                               int Tlen, const int32_t* __restrict__ done, float* __restrict__ align_scratch, uint32_t align_mask, int kv_div) {
+                               const uint8_t* __restrict__ kcross, const uint8_t* __restrict__ vcross, const float* __restrict__ kscale,
+                               const float* __restrict__ vscale, T* __restrict__ out, int B, int H, int Tlen, const int32_t* __restrict__ done,
+                               float* __restrict__ align_scratch, uint32_t align_mask, int kv_div) {
+    using C = CrossCfg<FP8>;
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* ring = smem;                                                   // kCrossStages * 16000
-    float* scores = reinterpret_cast<float*>(smem + kCrossStages * kCrossStageBytes);  // [Tlen]
-    float* sq = scores + ((Tlen + 3) & ~3);                                 // [64]
+    const int Tp = (Tlen + 3) & ~3;
+    uint8_t* ring = smem;                                                   // C::kStages * 16000
+    float* scores = reinterpret_cast<float*>(smem + C::kStages * C::kStageBytes);   // [Tlen]
+    float* ksc = scores + Tp;                                               // FP8: [Tlen] K row scales
+    float* vsc = ksc + Tp;                                                  // FP8: [Tlen] V row scales
+    float* sq = FP8 ? vsc + Tp : scores + Tp;                               // [64]
     float* red = sq + 64;                                                   // [4][64] + scratch
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(red + 4 * 64 + 32);
-    uint64_t* empty_bar = full_bar + kCrossStages;
+    uint64_t* empty_bar = full_bar + C::kStages;
+    uint64_t* scale_bar = empty_bar + C::kStages;                           // FP8 only
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // grid order: (window, head, beam) - the kv_div rows that share one K/V block are adjacent, so their streams meet in L2
@@ -446,14 +505,15 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
     const int win = wh / H, h = wh % H, b = win * kv_div + beam_j;
     const int kvh = win * H + h;             // K/V block index: [window][head]
     const int dm = H * 64;
-    const int chunks = Tlen / kCrossRows;  // per K and per V
+    const int chunks = Tlen / C::kRows;  // per K and per V
     pdl_launch_dependents();
-    // ended window: skip its 2 x 192 KB K/V stream.  done[] was written by the sampler of the previous step, many kernels upstream, so it
+    // ended window: skip its K/V stream.  done[] was written by the sampler of the previous step, many kernels upstream, so it
     // may be read before griddepcontrol.wait; the load is issued here and consumed after the barrier set-up so that its latency hides
     // under it (the CTA lives ~8 us: a dependent L2 round trip at its start would cost several per cent of the kernel)
     const int ended = done != nullptr ? done[b] : 0;
     if (tid == 0) {
-        for (int i = 0; i < kCrossStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
+        for (int i = 0; i < C::kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
+        if constexpr (FP8) mbar_init(scale_bar, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -464,15 +524,20 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
         // no griddepcontrol.wait here: the cross K/V cache is written once before the decode loop starts, so when this kernel is
         // launched as a programmatic dependent the first K chunks are already in flight while the upstream GEMM drains
         if (lane == 0) {
-            const uint8_t* kb = reinterpret_cast<const uint8_t*>(kcross + (long long)kvh * Tlen * 64);
-            const uint8_t* vb = reinterpret_cast<const uint8_t*>(vcross + (long long)kvh * Tlen * 64);
+            if constexpr (FP8) {
+                mbar_expect_tx(scale_bar, 2u * Tlen * 4);
+                bulk_load_1d(ksc, kscale + (long long)kvh * Tlen, Tlen * 4, scale_bar);
+                bulk_load_1d(vsc, vscale + (long long)kvh * Tlen, Tlen * 4, scale_bar);
+            }
+            const uint8_t* kb = kcross + (long long)kvh * Tlen * C::kRowBytes;
+            const uint8_t* vb = vcross + (long long)kvh * Tlen * C::kRowBytes;
             for (int c = 0; c < 2 * chunks; ++c) {
-                const int stage = c % kCrossStages;
-                const uint32_t ph = (c / kCrossStages) & 1;
+                const int stage = c % C::kStages;
+                const uint32_t ph = (c / C::kStages) & 1;
                 mbar_wait(&empty_bar[stage], ph ^ 1);
-                mbar_expect_tx(&full_bar[stage], kCrossStageBytes);
-                const uint8_t* src = c < chunks ? kb + (long long)c * kCrossStageBytes : vb + (long long)(c - chunks) * kCrossStageBytes;
-                bulk_load_1d(ring + stage * kCrossStageBytes, src, kCrossStageBytes, &full_bar[stage]);
+                mbar_expect_tx(&full_bar[stage], C::kStageBytes);
+                const uint8_t* src = c < chunks ? kb + (long long)c * C::kStageBytes : vb + (long long)(c - chunks) * C::kStageBytes;
+                bulk_load_1d(ring + stage * C::kStageBytes, src, C::kStageBytes, &full_bar[stage]);
             }
         }
         return;
@@ -485,31 +550,27 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
         sq[tid] = q * 0.125f;
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    const int sub = lane & 7;        // 16-byte piece of the 128-byte row: dims sub*8 .. sub*8+7
-    const int rsel = lane >> 3;      // row within a group of 4
-    float qv[8];
+    const int sub = lane % C::kLanesPerRow;   // 16-byte piece of the row: dims sub*kDims .. sub*kDims + kDims - 1
+    const int rsel = lane / C::kLanesPerRow;  // row within the warp's group of kRowsPerWarp
+    float qv[C::kDims];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) qv[j] = sq[sub * 8 + j];
+    for (int j = 0; j < C::kDims; ++j) qv[j] = sq[sub * C::kDims + j];
+    if constexpr (FP8) mbar_wait(scale_bar, 0);
 
-    // K phase: scores[t] = q . K[t]
+    // K phase: scores[t] = q . K[t]  (FP8: ksc[t] * (q . code[t]))
     for (int c = 0; c < chunks; ++c) {
-        const int stage = c % kCrossStages;
-        const uint32_t ph = (c / kCrossStages) & 1;
+        const int stage = c % C::kStages;
+        const uint32_t ph = (c / C::kStages) & 1;
         mbar_wait(&full_bar[stage], ph);
-        const uint8_t* tile = ring + stage * kCrossStageBytes;
+        const uint8_t* tile = ring + stage * C::kStageBytes;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const int r = warp * 4 + rsel + 16 * i;
+            const int r = warp * C::kRowsPerWarp + rsel + 4 * C::kRowsPerWarp * i;
             float acc = 0.f;
-            if (r < kCrossRows) {
-                const uint4 u = *reinterpret_cast<const uint4*>(tile + r * 128 + sub * 16);
-                const float2 a0 = T16<T>::unpack2(u.x), a1 = T16<T>::unpack2(u.y), a2 = T16<T>::unpack2(u.z), a3 = T16<T>::unpack2(u.w);
-                acc = qv[0] * a0.x + qv[1] * a0.y + qv[2] * a1.x + qv[3] * a1.y + qv[4] * a2.x + qv[5] * a2.y + qv[6] * a3.x + qv[7] * a3.y;
-            }
-            acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-            acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-            acc += __shfl_xor_sync(0xffffffffu, acc, 4);
-            if (sub == 0 && r < kCrossRows) scores[c * kCrossRows + r] = acc;
+            if (r < C::kRows) acc = cross_row_dot<T, FP8>(tile + r * C::kRowBytes + sub * 16, qv);
+#pragma unroll
+            for (int o = 1; o < C::kLanesPerRow; o <<= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+            if (sub == 0 && r < C::kRows) scores[c * C::kRows + r] = FP8 ? acc * ksc[c * C::kRows + r] : acc;
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[stage]);
@@ -540,38 +601,36 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
         for (int t = tid; t < Tlen; t += 128) dst[t] = scores[t] * inv;
     }
 
-    // V phase: out[d] = sum_t p[t] V[t][d]
-    float acc[8];
+    // V phase: out[d] = sum_t p[t] V[t][d]  (FP8: p[t] vsc[t] code[t][d])
+    float acc[C::kDims];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+    for (int j = 0; j < C::kDims; ++j) acc[j] = 0.f;
     for (int c = chunks; c < 2 * chunks; ++c) {
-        const int stage = c % kCrossStages;
-        const uint32_t ph = (c / kCrossStages) & 1;
+        const int stage = c % C::kStages;
+        const uint32_t ph = (c / C::kStages) & 1;
         mbar_wait(&full_bar[stage], ph);
-        const uint8_t* tile = ring + stage * kCrossStageBytes;
+        const uint8_t* tile = ring + stage * C::kStageBytes;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const int r = warp * 4 + rsel + 16 * i;
-            if (r < kCrossRows) {
-                const float p = scores[(c - chunks) * kCrossRows + r];
-                const uint4 u = *reinterpret_cast<const uint4*>(tile + r * 128 + sub * 16);
-                const float2 a0 = T16<T>::unpack2(u.x), a1 = T16<T>::unpack2(u.y), a2 = T16<T>::unpack2(u.z), a3 = T16<T>::unpack2(u.w);
-                acc[0] += p * a0.x; acc[1] += p * a0.y; acc[2] += p * a1.x; acc[3] += p * a1.y;
-                acc[4] += p * a2.x; acc[5] += p * a2.y; acc[6] += p * a3.x; acc[7] += p * a3.y;
+            const int r = warp * C::kRowsPerWarp + rsel + 4 * C::kRowsPerWarp * i;
+            if (r < C::kRows) {
+                const int t = (c - chunks) * C::kRows + r;
+                const float p = FP8 ? scores[t] * vsc[t] : scores[t];
+                cross_row_axpy<T, FP8>(tile + r * C::kRowBytes + sub * 16, p, acc);
             }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[stage]);
     }
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], 8);
-        acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], 16);
+    for (int j = 0; j < C::kDims; ++j) {
+#pragma unroll
+        for (int o = C::kLanesPerRow; o < 32; o <<= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");   // red[] (sum) consumed by everyone
     if (rsel == 0) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) red[warp * 64 + sub * 8 + j] = acc[j];
+        for (int j = 0; j < C::kDims; ++j) red[warp * 64 + sub * C::kDims + j] = acc[j];
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     if (tid < 64) {
@@ -580,8 +639,25 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
     }
 }
 
-static size_t cross_smem_bytes(int T) {
-    return (size_t)kCrossStages * kCrossStageBytes + (size_t)((T + 3) & ~3) * 4 + 64 * 4 + (4 * 64 + 32) * 4 + 2 * kCrossStages * 8 + 64;
+template <bool FP8> static size_t cross_smem_bytes(int T) {
+    using C = CrossCfg<FP8>;
+    return (size_t)C::kStages * C::kStageBytes + (size_t)((T + 3) & ~3) * 4 * (FP8 ? 3 : 1) + 64 * 4 + (4 * 64 + 32) * 4 +
+           (2 * C::kStages + (FP8 ? 1 : 0)) * 8 + 64;
+}
+
+template <typename T, bool FP8>
+static wk_status launch_cross(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, const float* kscale,
+                              const float* vscale, void* out, int B, int H, int Tlen, cudaStream_t stream, const int32_t* done, float* align_scratch,
+                              uint32_t align_mask, int kv_div) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_kernel<T, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(cross): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+        attr_set = true;
+    }
+    launch_k(decoder_cross_attention_kernel<T, FP8>, dim3(B * H), dim3(kCrossThreads), cross_smem_bytes<FP8>(Tlen), stream, 4, partial, splits, Bp, bq,
+             (const uint8_t*)kcross, (const uint8_t*)vcross, kscale, vscale, (T*)out, B, H, Tlen, done, align_scratch, align_mask, kv_div);
+    return WK_OK;
 }
 
 // The beam-search form (NQ rows share one K/V block) lives in cross_attention_mq.cu: both products on the tensor cores.
@@ -610,25 +686,21 @@ wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* s
 
 wk_status decoder_cross_attention(const float* partial, int splits, int Bp, const float* bq, const void* kcross,
                                   const void* vcross, void* out, int B, int H, int T, int dtype, cudaStream_t stream,
-                                  const int32_t* done, float* align_scratch, uint32_t align_mask, int kv_div) {
+                                  const int32_t* done, float* align_scratch, uint32_t align_mask, int kv_div, const float* kscale,
+                                  const float* vscale) {
+    const bool fp8 = kscale != nullptr;
     if (kv_div < 1 || B % kv_div != 0) { set_error("decoder_cross_attention: %d rows do not split into groups of %d", B, kv_div); return WK_ERR_INVALID_ARGUMENT; }
-    if (T % kCrossRows != 0) { set_error("decoder_cross_attention: n_audio_ctx %d not a multiple of %d", T, kCrossRows); return WK_ERR_INVALID_ARGUMENT; }
+    if (!fp8 && T % kCrossRows != 0) { set_error("decoder_cross_attention: n_audio_ctx %d not a multiple of %d", T, kCrossRows); return WK_ERR_INVALID_ARGUMENT; }
     if (kv_div > 1 && kv_div <= 8 && align_scratch == nullptr)   // beam search: one CTA per (window, head) serves all beams from one K/V pass
-        return decoder_cross_attention_mq(partial, splits, Bp, bq, kcross, vcross, out, B, H, T, dtype, stream, done, kv_div);
-    const size_t smem = cross_smem_bytes(T);
-    static bool attr_set[2] = {false, false};
-    const int ti = dtype == WK_DTYPE_F16 ? 1 : 0;
-    if (!attr_set[ti]) {
-        cudaError_t e = dtype == WK_DTYPE_F16
-            ? cudaFuncSetAttribute(decoder_cross_attention_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)
-            : cudaFuncSetAttribute(decoder_cross_attention_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(cross): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
-        attr_set[ti] = true;
-    }
-    if (dtype == WK_DTYPE_F16)
-        launch_k(decoder_cross_attention_kernel<__half>, dim3(B * H), dim3(kCrossThreads), smem, stream, 4, partial, splits, Bp, bq, (const __half*)kcross, (const __half*)vcross, (__half*)out, B, H, T, done, align_scratch, align_mask, kv_div);
-    else
-        launch_k(decoder_cross_attention_kernel<__nv_bfloat16>, dim3(B * H), dim3(kCrossThreads), smem, stream, 4, partial, splits, Bp, bq, (const __nv_bfloat16*)kcross, (const __nv_bfloat16*)vcross, (__nv_bfloat16*)out, B, H, T, done, align_scratch, align_mask, kv_div);
+        return decoder_cross_attention_mq(partial, splits, Bp, bq, kcross, vcross, out, B, H, T, dtype, stream, done, kv_div, kscale, vscale);
+    // FP8: the scale vectors are bulk-copied, so T * 4 bytes per (window, head) must keep 16-byte alignment
+    if (fp8 && (T % CrossCfg<true>::kRows != 0 || T % 4 != 0)) { set_error("decoder_cross_attention (fp8): n_audio_ctx %d not a multiple of 500", T); return WK_ERR_INVALID_ARGUMENT; }
+    const bool f16 = dtype == WK_DTYPE_F16;
+    wk_status st = fp8 ? (f16 ? launch_cross<__half, true>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div)
+                              : launch_cross<__nv_bfloat16, true>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div))
+                       : (f16 ? launch_cross<__half, false>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div)
+                              : launch_cross<__nv_bfloat16, false>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div));
+    if (st != WK_OK) return st;
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("decoder_cross_attention launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }

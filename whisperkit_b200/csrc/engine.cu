@@ -695,6 +695,29 @@ wk_status wk_model_info_get(const wk_model* m, wk_model_info* o) {
     o->has_alignment_heads = m->has_alignment_heads;
     o->is_multilingual = c.vocab != 51864;
     o->dtype = c.dtype; o->max_batch = c.max_batch;
+    o->cross_kv_dtype = m->cross_kv_fp8 ? WK_DTYPE_FP8_E4M3 : c.dtype;
+    return WK_OK;
+}
+
+wk_status wk_model_set_cross_kv_dtype(wk_model* m, int32_t dtype) {
+    if (!m) return WK_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> lock(m->api_mu);   // wk_session_create reads the policy and marks the model under the same lock
+    if (m->session_created) { set_error("wk_model_set_cross_kv_dtype: the cross K/V storage is fixed once a session exists"); return WK_ERR_INVALID_ARGUMENT; }
+    if (dtype != WK_DTYPE_FP8_E4M3 && dtype != m->cfg.dtype) {
+        set_error("wk_model_set_cross_kv_dtype: dtype %d is neither WK_DTYPE_FP8_E4M3 nor the model's dtype %d", dtype, m->cfg.dtype);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (dtype == WK_DTYPE_FP8_E4M3 && m->cfg.n_audio_ctx % 500 != 0) {   // the FP8 cross-attention kernel streams 250-row stages
+        set_error("wk_model_set_cross_kv_dtype: the FP8 cache needs n_audio_ctx to be a multiple of 500 (%d)", m->cfg.n_audio_ctx);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    m->cross_kv_fp8 = dtype == WK_DTYPE_FP8_E4M3;
+    return WK_OK;
+}
+
+wk_status wk_cross_kv_quantize_rows(const float* x, int64_t rows, uint8_t* codes, float* scales) {
+    if (!x || !codes || !scales || rows < 0) { set_error("wk_cross_kv_quantize_rows: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
+    for (int64_t r = 0; r < rows; ++r) fp8_quantize_row(x + r * 64, 64, codes + r * 64, scales + r);
     return WK_OK;
 }
 
@@ -1030,6 +1053,28 @@ wk_status wk_test_cross_attention_shared(wk_model* m, const float* q, const void
     cudaError_t e = cudaStreamSynchronize(m->stream);
     cudaFree(zero);
     if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention_shared: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+// the FP8 cache form of both: K/V codes [B / kv_div][H][T][64] u8 with row scales [B / kv_div][H][T] f32 (kv_div = 1: the single-query
+// kernel; 2..8: the beam kernel).  align_out != nullptr: every head exports its softmax row into align_out [H][B][T] (single-query kernel)
+wk_status wk_test_cross_attention_fp8(wk_model* m, const float* q, const uint8_t* kcodes, const uint8_t* vcodes, const float* kscale, const float* vscale,
+                                      void* out, int32_t B, int32_t H, int32_t T, int32_t dtype, const int32_t* done, int32_t kv_div,
+                                      float* align_out) {
+    if (!m || !q || !kcodes || !vcodes || !kscale || !vscale || !out || B < 1 || H < 1 || H > 32 || kv_div < 1) {
+        set_error("wk_test_cross_attention_fp8: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    float* zero = nullptr;
+    WK_CHECK(dmalloc(&zero, (size_t)H * 64));
+    const uint32_t all_heads = H == 32 ? 0xffffffffu : (1u << H) - 1u;
+    wk_status r = decoder_cross_attention(q, 1, B, zero, kcodes, vcodes, out, B, H, T, dtype, m->stream, done, align_out, align_out ? all_heads : 0u,
+                                          kv_div, kscale, vscale);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    cudaFree(zero);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention_fp8: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     return r;
 }
 

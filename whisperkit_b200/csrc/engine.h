@@ -111,6 +111,10 @@ struct wk_model {
     float timings[6] = {0, 0, 0, 0, 0, 0};
     cudaEvent_t ev[8];
     std::atomic<int> live_sessions{0};
+    // cross-attention K/V cache storage: the model dtype, or FP8 E4M3 with per-row scales (wk_model_set_cross_kv_dtype); fixed once the
+    // first session exists.  Both fields are read and written under api_mu.
+    bool cross_kv_fp8 = false;
+    bool session_created = false;
 };
 
 namespace wk {

@@ -3,7 +3,8 @@
 //   D[rows, cols] = A[rows, K] * B[cols, K]^T      (both operands K-major, 16-bit, f32 accumulate in registers)
 //
 // One kernel serves every dense contraction of the Whisper hot path:
-//   * encoder / cross-KV projections: A = activations (M = B*1500 rows), B = weights [N, K]
+//   * encoder / cross-KV projections: A = activations (M = B*1500 rows), B = weights [N, K]; the cross-KV projection scatters head-major
+//     16-bit rows, or (FP8 cache) E4M3 rows with one f32 scale each, quantized in the epilogue (gemm_epilogue_fp8_heads)
 //   * conv stem as implicit GEMM: A is a 3-D tensor map, the 3 taps are extra K-blocks with a row shift
 //   * decoder (M = batch <= 256): swap-AB, A = weights (128 output features per tile), B = activations,
 //     split-K partials written transposed so the next fused reduce(+LN) kernel reads them coalesced.
@@ -51,6 +52,7 @@ struct GemmKParams {
     const float* pos;
     long long ld_pos;
     int heads_T, heads_B, heads_H, heads_dmodel;
+    float* out_scale;
     int a_static;     // see GemmDesc::a_static
 };
 
@@ -99,7 +101,53 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, int spl
     }
 }
 
-template <typename T, int BN>
+// GEMM_OUT_FP8_HEADS epilogue of one thread: rows r_lo and r_lo + 8, columns 8 j + c_lo, + 1.  The 64 columns of a head are j = 8 hh ..
+// 8 hh + 7 of the 4 lanes of a quad (16 values each), so the row's amax is two quad shuffles; every lane then encodes its 16 values and
+// the lane with c_lo == 0 stores the row's scale.  Rows past the tile's valid rows take part in the shuffles but store nothing.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_fp8_heads(const GemmKParams& p, int batch, int tile_row0, int r_lo, int c_lo, int col_base,
+                                                        const float (&acc)[BN / 2]) {
+    static_assert(BN % 64 == 0, "FP8 heads epilogue needs head-aligned N tiles");
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        const int row_in_batch = tile_row0 + r_lo + 8 * half;
+        const long long grow = (long long)batch * p.out_rows_per_batch + row_in_batch;
+        const int b = (int)(grow / p.heads_T);
+        const int tt = (int)(grow - (long long)b * p.heads_T);
+#pragma unroll
+        for (int hh = 0; hh < BN / 64; ++hh) {
+            const int col0 = col_base + hh * 64;   // n is a multiple of 64: a head is wholly inside or wholly past n
+            const bool col_ok = col0 < p.n;
+            float v[16];
+            float amax = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                const int j = hh * 8 + jj;
+                float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+                if (p.bias && col_ok) {
+                    const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * jj + c_lo));
+                    v0 += bb.x; v1 += bb.y;
+                }
+                v[2 * jj] = v0; v[2 * jj + 1] = v1;
+                amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+            }
+            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+            if (!col_ok || row_in_batch >= p.m_rows_per_batch) continue;
+            const int which = col0 / p.heads_dmodel;
+            const int h = (col0 - which * p.heads_dmodel) >> 6;
+            const long long row = (((long long)which * p.heads_B + b) * p.heads_H + h) * p.heads_T + tt;
+            const float s = fp8_row_scale(amax);
+            uint8_t* o = reinterpret_cast<uint8_t*>(p.out) + row * 64 + c_lo;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+                *reinterpret_cast<uint16_t*>(o + 8 * jj) = (uint16_t)(fp8_encode(v[2 * jj], s) | (fp8_encode(v[2 * jj + 1], s) << 8));
+            if (c_lo == 0) p.out_scale[row] = s;
+        }
+    }
+}
+
+template <typename T, int BN, bool FP8_HEADS = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -220,14 +268,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
         const int col_base = n_tile * BN;
+        if constexpr (FP8_HEADS) {
+            gemm_epilogue_fp8_heads<BN>(p, batch, tile_row0, r_lo, c_lo, col_base, acc);
+        } else {
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int row_in_batch = tile_row0 + r_lo + 8 * half;
-            if (row_in_batch >= p.m_rows_per_batch) continue;
-            const long long grow = (long long)batch * p.out_rows_per_batch + row_in_batch;
+            for (int half = 0; half < 2; ++half) {
+                const int row_in_batch = tile_row0 + r_lo + 8 * half;
+                if (row_in_batch >= p.m_rows_per_batch) continue;
+                const long long grow = (long long)batch * p.out_rows_per_batch + row_in_batch;
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j)
-                gemm_epilogue_pair<T>(p, split, grow, row_in_batch, col_base + 8 * j + c_lo, acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
+                for (int j = 0; j < BN / 8; ++j)
+                    gemm_epilogue_pair<T>(p, split, grow, row_in_batch, col_base + 8 * j + c_lo, acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
+            }
         }
     }
 }
@@ -288,21 +340,22 @@ int wgmma_tile_n(int bn) {
     return t;
 }
 
-template <typename T, int BN>
+template <typename T, int BN, bool FP8_HEADS = false>
 static cudaError_t launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKParams& p, int grid, size_t smem, int pdl,
                                cudaStream_t stream) {
     static bool attr_set = false;
     if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<T, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
+        const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<T, BN, FP8_HEADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    return launch_k(gemm_wgmma_kernel<T, BN>, dim3(grid), dim3(kGemmThreads), smem, stream, pdl, tmA, tmB, p);
+    return launch_k(gemm_wgmma_kernel<T, BN, FP8_HEADS>, dim3(grid), dim3(kGemmThreads), smem, stream, pdl, tmA, tmB, p);
 }
 
 template <typename T>
 static cudaError_t launch_gemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKParams& p, int grid, size_t smem, int pdl,
                                  cudaStream_t stream) {
+    if (p.mode == GEMM_OUT_FP8_HEADS) return launch_gemm<T, 256, true>(tmA, tmB, p, grid, smem, pdl, stream);   // bn checked by gemm_wgmma
     switch (p.bn) {
         case 16: return launch_gemm<T, 16>(tmA, tmB, p, grid, smem, pdl, stream);
         case 32: return launch_gemm<T, 32>(tmA, tmB, p, grid, smem, pdl, stream);
@@ -364,6 +417,12 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream) {
     p.pos = d.pos;
     p.ld_pos = d.ld_pos;
     p.heads_T = d.heads_T; p.heads_B = d.heads_B; p.heads_H = d.heads_H; p.heads_dmodel = d.heads_dmodel;
+    p.out_scale = d.out_scale;
+    if (d.mode == GEMM_OUT_FP8_HEADS && (p.bn != 256 || d.n % 64 != 0 || d.heads_dmodel % 64 != 0 || !d.out_scale)) {
+        // the row amax is taken over whole heads inside one N tile
+        set_error("gemm_wgmma: the FP8 heads epilogue needs 256-column tiles and head-aligned columns (bn %d n %d d %d)", p.bn, d.n, d.heads_dmodel);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
 
     CUtensorMap tmA, tmB;
     wk_status st;

@@ -20,6 +20,7 @@ enum GemmMode {
     GEMM_OUT_PARTIAL_T = 3,  // out32[split][col][row] = acc                  (swap-AB split-K partials)
     GEMM_OUT_T16_HEADS = 4,  // out16[which][b][h][t][64] head-major scatter  (cross-attention K/V cache)
     GEMM_OUT_F32 = 5,        // out32[row, col] = acc + bias[col]
+    GEMM_OUT_FP8_HEADS = 6,  // out8[which][b][h][t][64] E4M3 codes + out_scale[which][b][h][t] f32 (FP8 cross-attention K/V cache)
 };
 
 struct GemmDesc {
@@ -58,7 +59,8 @@ struct GemmDesc {
     int64_t ld_pos;
     // HEADS scatter
     int heads_T, heads_B, heads_H, heads_dmodel;
-    int pdl;                 // launch with programmatic dependent launch (decode-step chain)
+    float* out_scale;        // FP8_HEADS: one scale per 64-value row
+    int pdl;                // launch with programmatic dependent launch (decode-step chain)
     int max_stages;          // 0 = as many smem stages as fit; >0 caps the ring (lets other kernels co-reside on the SM)
     int a_static;            // A operand (weights) does not depend on the upstream kernel: with PDL its first tiles are fetched before griddepcontrol.wait
 };
@@ -168,14 +170,18 @@ wk_status decoder_self_attention(const float* partial, int splits, int Bp, const
 // cross attention over T encoder positions; reduces q partials [S][Bp][d]; K/V [B][H][T][64]
 // align_scratch != nullptr: heads h with bit h of align_mask set also write their softmax row (f32, [slot][B][T], slot = rank of h in
 // the mask) - the alignment heads behind the reference decoder's `alignment_heads_weights` output (TextDecoder.swift:310,414)
+// kscale / vscale != nullptr: the FP8 cache - K/V are E4M3 codes [B][H][T][64] with one f32 scale per row ([B][H][T]); dtype is then only
+// the type of `out`
 wk_status decoder_cross_attention(const float* partial, int splits, int Bp, const float* bq, const void* kcross,
                                   const void* vcross, void* out, int B, int H, int T, int dtype, cudaStream_t stream,
-                                  const int32_t* done = nullptr, float* align_scratch = nullptr, uint32_t align_mask = 0, int kv_div = 1);
+                                  const int32_t* done = nullptr, float* align_scratch = nullptr, uint32_t align_mask = 0, int kv_div = 1,
+                                  const float* kscale = nullptr, const float* vscale = nullptr);
 // kv_div > 1 (beam search): row b reads the K/V block of window b / kv_div; the CTAs of one (window, head) are adjacent in the grid so that
 // their K/V stream is shared through L2
 // tensor-core variant for nq = 2..8 rows per K/V block (cross_attention_mq.cu): one K/V stream per (window, head) serves all nq beams
 wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, void* out, int B, int H,
-                                     int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq);
+                                     int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq,
+                                     const float* kscale = nullptr, const float* vscale = nullptr);
 // alignment row of the step just sampled (run AFTER the sampler advanced steps[b] to tokenIndex + 1): out[b][steps[b]][t] =
 // Float16(mean over n_slots of scratch[slot][b][t]) unless done[b] (TextDecoder.updateAlignmentWeights, TextDecoder.swift:272-296:
 // the slice of step tokenIndex lands in row tokenIndex + 1; a completed segment breaks out before the update, :668-674)

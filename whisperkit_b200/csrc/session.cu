@@ -33,7 +33,9 @@ struct wk_session {
     cudaStream_t stream = nullptr;      // decode stream
     cudaStream_t enc_stream = nullptr;  // mel + encoder of the batched entry
     EncWorkspace ws;                    // this session's mel / encoder activations (allocated on first use)
-    void* cross_kv = nullptr;   // [2L][S][H][T][64]
+    void* cross_kv = nullptr;   // [2L][S][H][T][64] model dtype, or E4M3 codes when ckv_fp8
+    float* cross_scale = nullptr;   // ckv_fp8: [2L][S][H][T] row scales
+    bool ckv_fp8 = false;
     void* self_k = nullptr;     // [L][S][H][224][64]
     void* self_v = nullptr;
     float* partial = nullptr; size_t partial_elems = 0;
@@ -89,6 +91,20 @@ static wk_status dec_gemm(wk_session* s, const void* w, int N, int K, const void
     return gemm_wgmma(g, m->num_sms, s->stream);
 }
 
+// Bytes of one cross K/V element, and the projection of `cnt` windows of encoder output `src` ([cnt * T][d]) into slots [q0, q0 + cnt) of
+// the cache in the session's storage policy
+static size_t ckv_esize(const wk_session* s) { return s->ckv_fp8 ? 1 : 2; }
+static GemmDesc cross_kv_gemm(const wk_session* s, const void* src, int cnt, int q0) {
+    const wk_model_config& c = s->m->cfg;
+    const int T = c.n_audio_ctx, H = c.n_heads;
+    GemmDesc g = plain_gemm(src, (int64_t)cnt * T, c.d_model, s->m->wckv, 2 * c.dec_layers * c.d_model, c.dtype,
+                            s->ckv_fp8 ? GEMM_OUT_FP8_HEADS : GEMM_OUT_T16_HEADS, (char*)s->cross_kv + (size_t)q0 * H * T * 64 * ckv_esize(s), 0,
+                            s->m->bckv, 0);
+    g.heads_T = T; g.heads_B = s->max_batch; g.heads_H = H; g.heads_dmodel = c.d_model;
+    if (s->ckv_fp8) g.out_scale = s->cross_scale + (size_t)q0 * H * T;
+    return g;
+}
+
 // The fused phase chains hold every SM with a CTA that waits on grid-wide barriers.  Two such grids from different sessions could each
 // take half of the machine and wait for the other half forever, so a session only uses them while it is the model's sole live session.
 static bool use_fused(const wk_session* s) { return s->knob_fused && s->m->live_sessions.load(std::memory_order_relaxed) == 1; }
@@ -100,7 +116,8 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
     const int d = c.d_model, H = c.n_heads, dt = c.dtype, B = s->batch, Bp = s->bp, T = c.n_audio_ctx;
     cudaStream_t st = s->stream;
     const size_t self_layer = (size_t)s->max_batch * H * kKvMaxLen * 64 * 2;   // bytes per layer
-    const size_t cross_block = (size_t)s->max_batch * H * T * 64 * 2;          // bytes per (layer, k|v)
+    const size_t cross_rows = (size_t)s->max_batch * H * T;                    // rows of 64 per (layer, k|v)
+    const size_t cross_block = cross_rows * 64 * ckv_esize(s);                 // bytes per (layer, k|v)
     const int32_t* pos = explicit_pos ? explicit_pos : s->st.steps;
     // ended rows are skipped by the attention kernels; a burst that starts with every slot live runs the variant without the checks (a
     // row that ends inside it just keeps computing until the next poll, as harmlessly as before it ended)
@@ -118,7 +135,8 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
         return decoder_cross_attention(s->partial, sp, Bp, l.bcq, (char*)s->cross_kv + (size_t)(2 * li) * cross_block,
                                        (char*)s->cross_kv + (size_t)(2 * li + 1) * cross_block, s->attn, B, H, T, dt, st, done,
                                        align ? s->align_scratch + (size_t)m->align_base[li] * B * T : nullptr, align ? m->align_mask[li] : 0u,
-                                       beam_rows ? s->bs.beam : 1);
+                                       beam_rows ? s->bs.beam : 1, s->ckv_fp8 ? s->cross_scale + (2 * li) * cross_rows : nullptr,
+                                       s->ckv_fp8 ? s->cross_scale + (2 * li + 1) * cross_rows : nullptr);
     };
     if (fused) {
         // per layer: self-attention -> chain B (out-proj, reduce+LN, cross-Q) -> cross-attention -> chain C (cross-out, reduce+LN, FC1,
@@ -623,10 +641,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     auto project_cross_kv = [&](int64_t w0, int q0, int cnt) -> wk_status {
         if (!chunk_waited) { WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, s->ev_enc, 0)); chunk_waited = true; }
         const char* src = (const char*)s->ws.enc_out + (size_t)(w0 - chunk_w0) * T * d * 2;
-        GemmDesc g = plain_gemm(src, (int64_t)cnt * T, d, m->wckv, 2 * c.dec_layers * d, c.dtype, GEMM_OUT_T16_HEADS,
-                                (char*)s->cross_kv + (size_t)q0 * c.n_heads * T * 64 * 2, 0, m->bckv, 0);
-        g.heads_T = T; g.heads_B = s->max_batch; g.heads_H = c.n_heads; g.heads_dmodel = d;
-        return gemm_wgmma(g, m->num_sms, s->stream);
+        return gemm_wgmma(cross_kv_gemm(s, src, cnt, q0), m->num_sms, s->stream);
     };
 
     int64_t finished = 0;
@@ -823,7 +838,19 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&s->enc_stream, cudaStreamNonBlocking));
     const int bpm = round_up(S, 16);
-    WK_CHECK(alloc16(&s->cross_kv, (size_t)2 * L * S * H * T * 64));
+    {
+        std::lock_guard<std::mutex> lock(m->api_mu);   // against a concurrent wk_model_set_cross_kv_dtype
+        m->session_created = true;
+        s->ckv_fp8 = m->cross_kv_fp8;
+    }
+    if (s->ckv_fp8) {
+        uint8_t* codes = nullptr;
+        WK_CHECK(dmalloc(&codes, (size_t)2 * L * S * H * T * 64));
+        s->cross_kv = codes;
+        WK_CHECK(dmalloc(&s->cross_scale, (size_t)2 * L * S * H * T));
+    } else {
+        WK_CHECK(alloc16(&s->cross_kv, (size_t)2 * L * S * H * T * 64));
+    }
     WK_CHECK(alloc16(&s->self_k, (size_t)L * S * H * kKvMaxLen * 64));
     WK_CHECK(alloc16(&s->self_v, (size_t)L * S * H * kKvMaxLen * 64));
     // split-K partial workspace: max over the decoder GEMM shapes of splits * N
@@ -897,7 +924,7 @@ void wk_session_free(wk_session* s) {
     s->m->live_sessions.fetch_sub(1);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     if (s->graph_exec_live) cudaGraphExecDestroy(s->graph_exec_live);
-    void* ptrs[] = {s->cross_kv, s->self_k, s->self_v, s->partial, s->x, s->xn, s->attn, s->ffn, s->logits, s->st.tokens, s->st.n_tokens,
+    void* ptrs[] = {s->cross_kv, s->cross_scale, s->self_k, s->self_v, s->partial, s->x, s->xn, s->attn, s->ffn, s->logits, s->st.tokens, s->st.n_tokens,
                     s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error, s->rp_dev,
                     s->pos_dev, s->lang_dev, s->suppress_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, s->align_scratch, s->align_w,
                     s->align_store, s->chain_counters};
@@ -928,8 +955,6 @@ wk_status wk_session_set_encoder_output(wk_session* s, const wk_tensor* enc) {
     if (enc->kind != 1 || enc->owner != m) { set_error("encoder output does not belong to this model"); return WK_ERR_INVALID_ARGUMENT; }
     if (enc->batch < 1 || enc->batch > s->max_batch) { set_error("encoder batch %lld exceeds session max_batch %d", (long long)enc->batch, s->max_batch); return WK_ERR_PREPARE_DECODER_INPUTS; }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
-    const wk_model_config& c = m->cfg;
-    const int d = c.d_model, T = c.n_audio_ctx;
     s->batch = (int)enc->batch;
     s->bound_windows = s->batch;
     s->bs.beam = 1;
@@ -937,9 +962,7 @@ wk_status wk_session_set_encoder_output(wk_session* s, const wk_tensor* enc) {
     // the encoder ran on the model stream; the projection reads its output on the session stream and the tensor remembers the reader
     std::lock_guard<std::mutex> lock(m->api_mu);
     for (cudaEvent_t e : enc->events) WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, e, 0));
-    GemmDesc g = plain_gemm(enc->data, (int64_t)s->batch * T, d, m->wckv, 2 * c.dec_layers * d, c.dtype, GEMM_OUT_T16_HEADS, s->cross_kv, 0, m->bckv, 0);
-    g.heads_T = T; g.heads_B = s->max_batch; g.heads_H = c.n_heads; g.heads_dmodel = d;
-    WK_CHECK(gemm_wgmma(g, m->num_sms, s->stream));
+    WK_CHECK(gemm_wgmma(cross_kv_gemm(s, enc->data, s->batch, 0), m->num_sms, s->stream));
     cudaEvent_t ev;
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventRecord(ev, s->stream));
@@ -1112,7 +1135,10 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
     cudaStream_t st = enc_side ? s->enc_stream : s->stream;
     const int saved_batch = s->batch, saved_bp = s->bp;
     if (!enc_side) { s->batch = B; s->bp = round_up(B, 16); }
-    const size_t cross_block = (size_t)s->max_batch * H * T * 64 * 2;
+    const size_t cross_rows = (size_t)s->max_batch * H * T;
+    const size_t cross_block = cross_rows * 64 * ckv_esize(s);
+    const float* ksc = s->ckv_fp8 ? s->cross_scale : nullptr;
+    const float* vsc = s->ckv_fp8 ? s->cross_scale + cross_rows : nullptr;
     static int32_t* pos100 = nullptr;
     if (which == 9 && !pos100) { std::vector<int32_t> h(256, 100); cudaMalloc(&pos100, 256 * 4); cudaMemcpy(pos100, h.data(), 256 * 4, cudaMemcpyHostToDevice); }
     int rot = 0;
@@ -1135,7 +1161,8 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
     auto run = [&]() -> wk_status {
         int sp;
         switch (which) {
-            case 0: return decoder_cross_attention(s->partial, 1, s->bp, m->dec[0].bcq, s->cross_kv, (char*)s->cross_kv + cross_block, s->attn, B, H, T, dt, st);
+            case 0: return decoder_cross_attention(s->partial, 1, s->bp, m->dec[0].bcq, s->cross_kv, (char*)s->cross_kv + cross_block, s->attn, B, H, T, dt, st,
+                                                   nullptr, nullptr, 0, 1, ksc, vsc);
             case 1: return gemm_wgmma(plain_gemm(s->ws.xn, M, d, m->enc[0].w1, 4 * d, dt, GEMM_OUT_T16, s->ws.ffn, 4 * d, m->enc[0].b1, 1), m->num_sms, st);
             case 2: return mel_forward(m->mel_tables, s->ws.pcm_dev, B, kWindowSamples, nullptr, s->ws.mel, s->ws.gmax, st);
             case 3: return encoder_attention(s->ws.qkv, s->ws.attn, B, T, H, dt, st);
@@ -1163,7 +1190,7 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
         }
     };
     switch (which) {
-        case 0: *work_out = (double)B * H * T * 64 * 2 * 2; break;                         // K + V bytes
+        case 0: *work_out = (double)B * H * T * (64 * (double)ckv_esize(s) + (s->ckv_fp8 ? 4 : 0)) * 2; break;   // K + V bytes (+ FP8 row scales)
         case 1: *work_out = 2.0 * (double)M * d * 4 * d; break;                            // FLOPs
         case 2: *work_out = (double)B * (kWindowSamples * 4.0 + c.n_mels * 3000 * 2.0); break;  // bytes (SURVEY 8d)
         case 3: *work_out = 4.0 * (double)B * H * T * T * 64; break;                       // FLOPs
@@ -1210,7 +1237,8 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
 
 // Debug readback of an internal buffer as f32 (tests/tools only).  which: session encoder workspace 0 mel[Bm,3002,128] 1 h1[Bm,3002,d]
 // 2 x[M,d] 3 xn[M,d] 4 qkv[M,3d] 5 attn[M,d] 6 ffn[M,4d] 7 enc_out[M,d]; decode 10 x[Bp,d] 11 xn[Bp,d] 12 attn[Bp,d]
-// 13 ffn[Bp,4d] 14 logits[S,V] 15 cross_kv (all) 16 self_k (all) 17 self_v (all) 18 partial; 20.. weights
+// 13 ffn[Bp,4d] 14 logits[S,V] 15 cross_kv (all; an FP8 cache is returned dequantized, code * row scale) 16 self_k (all) 17 self_v (all)
+// 18 partial; 20.. weights
 wk_status wk_debug_read(wk_model* m, wk_session* s, int32_t which, int64_t offset_elems, float* dst, int64_t n) {
     if (!m || !dst) return WK_ERR_INVALID_ARGUMENT;
     WK_CUDA_CHECK(cudaSetDevice(m->device));
@@ -1245,6 +1273,17 @@ wk_status wk_debug_read(wk_model* m, wk_session* s, int32_t which, int64_t offse
     }
     if (!src) { set_error("wk_debug_read: unknown or unallocated buffer %d", which); return WK_ERR_INVALID_ARGUMENT; }
     std::lock_guard<std::mutex> lock(m->api_mu);
+    if (which == 15 && s->ckv_fp8) {   // codes [offset, offset + n) and the scales of their rows, dequantized here
+        if (n < 1) return WK_OK;
+        const int64_t r0 = offset_elems / 64, r1 = (offset_elems + n - 1) / 64;
+        std::vector<uint8_t> codes(n);
+        std::vector<float> sc(r1 - r0 + 1);
+        WK_CUDA_CHECK(cudaDeviceSynchronize());
+        WK_CUDA_CHECK(cudaMemcpy(codes.data(), (const uint8_t*)s->cross_kv + offset_elems, n, cudaMemcpyDeviceToHost));
+        WK_CUDA_CHECK(cudaMemcpy(sc.data(), s->cross_scale + r0, sc.size() * 4, cudaMemcpyDeviceToHost));
+        for (int64_t i = 0; i < n; ++i) dst[i] = fp8_decode(codes[i]) * sc[(offset_elems + i) / 64 - r0];
+        return WK_OK;
+    }
     float* tmp = nullptr;
     WK_CUDA_CHECK(cudaMalloc(&tmp, n * 4));
     WK_CUDA_CHECK(cudaDeviceSynchronize());

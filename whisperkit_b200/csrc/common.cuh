@@ -213,6 +213,26 @@ __device__ __forceinline__ void mbar_expect_tx_elect(uint64_t* bar, uint32_t byt
         "@q mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes)
         : "memory");
 }
+// Shared -> global tensor store of one box (the tensor map clips what lies outside the tensor), tracked by bulk async-groups.  The
+// smem writes it reads must be made visible to the async proxy first (fence_proxy_async + a barrier over the writing threads).
+__device__ __forceinline__ void tma_store_3d(const void* tmap, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed bulk store has finished reading shared memory (its source buffer may be rewritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed bulk store has completed (its writes are done)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// barrier over the 128 threads of one warpgroup (named barrier `id`, 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// four 8x8 16-bit matrices to shared memory: lane l gives the address of row l % 8 of matrix l / 8; register i of every lane holds
+// matrix i's elements (row lane / 4, columns 2 (lane % 4), + 1) - the layout of a wgmma accumulator pair
+__device__ __forceinline__ void stmatrix_x4(uint32_t smem_addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
 // 1-D bulk copy global -> shared, completion on an mbarrier (UBLKCP).
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
     asm volatile(

@@ -13,8 +13,9 @@
 //   warpgroup 0   warp 0: TMA producer, cp.async.bulk.tensor (128B swizzle) into a ring of smem stages, mbarrier tx; warps 1-3 idle
 //                 (the warpgroup gives its registers to the consumers with setmaxnreg)
 //   warpgroups 1, 2  consumers: rows [64 * (wg - 1), +64) of the 128-row tile, wgmma m64nBNk16 from shared memory, the accumulator
-//                 in registers, then the fused epilogue straight from those registers to HBM.  A stage is released as soon as the
-//                 wgmma group that read it has retired (wait_group 1 keeps one k-block of MMAs in flight).
+//                 in registers, then the fused epilogue (see GemmEpi: TMA stores through a staging box, or stores from registers).
+//                 A stage is released as soon as the wgmma group that read it has retired (wait_group 1 keeps one k-block of MMAs in
+//                 flight).
 // The WhisperKit reference has no counterpart source for this file: the contraction lives inside
 // AudioEncoder.mlmodelc / TextDecoder.mlmodelc (Sources/WhisperKit/Core/AudioEncoder.swift:59-62,
 // Sources/WhisperKit/Core/TextDecoder.swift:394-417).
@@ -44,7 +45,7 @@ struct GemmKParams {
     int tap_col_off[3];
     int a_is_3d;
     int m_rows_per_batch, n, bn;
-    int stage_b_bytes, stages;
+    int stage_b_bytes, stages, store_bytes;
     int mode, gelu;
     void* out;
     long long ld_out, out_rows_per_batch, partial_cols;
@@ -56,48 +57,171 @@ struct GemmKParams {
     int a_static;     // see GemmDesc::a_static
 };
 
-// fused epilogue of two adjacent accumulator columns (col, col + 1) of one output row
-template <typename T>
-__device__ __forceinline__ void gemm_epilogue_pair(const GemmKParams& p, int split, long long grow, int row_in_batch, int col, float v0,
-                                                   float v1) {
-    if (p.mode == GEMM_OUT_PARTIAL_T) {
-        float* o = reinterpret_cast<float*>(p.out);
-        if (col < p.partial_cols) o[((long long)split * p.partial_cols + col) * p.ld_out + grow] = v0;
-        if (col + 1 < p.partial_cols) o[((long long)split * p.partial_cols + col + 1) * p.ld_out + grow] = v1;
-        return;
+// How a GEMM leaves the accumulator (one kernel instantiation each):
+//   kEpiPartialT  GEMM_OUT_PARTIAL_T, per-pair stores from the registers
+//   kEpiFp8Heads  GEMM_OUT_FP8_HEADS, per-row quantization in registers (gemm_epilogue_fp8_heads)
+//   kEpiStore16   GEMM_OUT_T16 / GEMM_OUT_T16_HEADS and kEpiStore32  GEMM_OUT_F32 / _F32_ADD / _F32_GELU_POS: the per-element math in
+//                 registers, the tile through a shared-memory staging box and TMA bulk tensor stores (gemm_epilogue_store16 / _store32)
+enum GemmEpi { kEpiPartialT = 0, kEpiFp8Heads = 1, kEpiStore16 = 2, kEpiStore32 = 3 };
+static int gemm_epi(int mode) {
+    switch (mode) {
+        case GEMM_OUT_PARTIAL_T: return kEpiPartialT;
+        case GEMM_OUT_FP8_HEADS: return kEpiFp8Heads;
+        case GEMM_OUT_T16: case GEMM_OUT_T16_HEADS: return kEpiStore16;
+        default: return kEpiStore32;
     }
-    if (col >= p.n) return;   // n is a multiple of 32: col + 1 < n as well
-    if (p.bias) {
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-        v0 += bb.x; v1 += bb.y;
+}
+
+// Output staging of the TMA-store epilogues: per consumer warpgroup two boxes of 64 rows x 128 bytes (64 16-bit or 32 f32 columns),
+// 128-byte swizzled like the output tensor map.  While one box drains to global memory the warpgroup fills the other; the consumers
+// go on to the next work item's mainloop as soon as the last box of a tile is handed to TMA.
+static constexpr int kStoreBox = 64 * 128;
+static constexpr int kStoreBytes = 2 /*warpgroups*/ * 2 /*boxes*/ * kStoreBox;
+
+// byte offset of 16-byte chunk `chunk` of row `row` in a 128-byte-swizzled box (16-byte chunk index XOR row % 8)
+__device__ __forceinline__ uint32_t swz128(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
+
+// hand staging box `box` to TMA after the warpgroup has written it.  Thread 0 of the warpgroup first waits until the previous box's
+// store has read shared memory, so that the next chunk may overwrite that box once every thread has passed the barrier.
+__device__ __forceinline__ void store_box_begin(int wg_tid, int cw) {
+    fence_proxy_async();
+    if (wg_tid == 0) bulk_wait_read_all();
+    warpgroup_bar(1 + cw);
+}
+
+// GEMM_OUT_T16 / GEMM_OUT_T16_HEADS epilogue of one consumer warpgroup: rows [row0, row0 + 64) of batch `batch`, columns
+// [col_base, col_base + BN).  Per 64-column chunk: bias, GELU and T16::pack2 in registers, stmatrix into the staging box, one TMA store.
+// T16_HEADS: the chunk is one head; the output map is {64, T, blocks} over the [which][b][h][t][64] cache, so the chunk's 64 rows are one
+// box at (0, t0, block), clipped at T.  When they run past the end of window b, the warpgroup copies rows [T - t0, 64) of the box to the
+// start of block + H (window b + 1) with 16-byte stores: a TMA store box that starts at a negative row is an illegal instruction.
+template <typename T, int BN>
+__device__ __forceinline__ void gemm_epilogue_store16(const GemmKParams& p, const CUtensorMap* tmO, const float (&acc)[BN / 2],
+                                                      uint8_t* stage, int& sbuf, int wg_tid, int cw, int batch, int row0, int col_base) {
+    const int lane = wg_tid & 31;
+    const int q = lane & 3;
+    // stmatrix: lane l addresses row l % 8 of matrix l / 8; matrices (j, rows +0), (j, rows +8), (j + 1, +0), (j + 1, +8)
+    const int mrow = 16 * (wg_tid >> 5) + 8 * ((lane >> 3) & 1) + (lane & 7);
+    const int mj = lane >> 4;
+    const bool heads = p.mode == GEMM_OUT_T16_HEADS;
+    int hb = 0, ht0 = 0;
+    bool straddle = false;
+    if (heads) {
+        hb = row0 / p.heads_T;
+        ht0 = row0 - hb * p.heads_T;
+        straddle = ht0 + 64 > p.heads_T && (hb + 1) * p.heads_T < p.m_rows_per_batch;
     }
-    if (p.gelu) {
-        const float2 g = gelu_erf2(make_float2(v0, v1));
-        v0 = g.x; v1 = g.y;
-    }
-    if (p.mode == GEMM_OUT_T16) {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.out) + grow * p.ld_out + col) = T16<T>::pack2(v0, v1);
-    } else if (p.mode == GEMM_OUT_T16_HEADS) {
-        const int b = (int)(grow / p.heads_T);
-        const int tt = (int)(grow - (long long)b * p.heads_T);
-        const int which = col / p.heads_dmodel;
-        const int rem = col - which * p.heads_dmodel;
-        const int h = rem >> 6;
-        const int dd = rem & 63;
-        T* o = reinterpret_cast<T*>(p.out) + ((((long long)which * p.heads_B + b) * p.heads_H + h) * p.heads_T + tt) * 64 + dd;
-        *reinterpret_cast<uint32_t*>(o) = T16<T>::pack2(v0, v1);
-    } else {
-        float2* o = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + grow * p.ld_out + col);
-        if (p.mode == GEMM_OUT_F32_ADD) {
-            float2 x = *o;
-            x.x += v0; x.y += v1;
-            *o = x;
-        } else if (p.mode == GEMM_OUT_F32_GELU_POS) {
-            const float2 pp = __ldg(reinterpret_cast<const float2*>(p.pos + (long long)row_in_batch * p.ld_pos + col));
-            *o = make_float2(v0 + pp.x, v1 + pp.y);
-        } else {
-            *o = make_float2(v0, v1);
+#pragma unroll
+    for (int c = 0; c < BN / 64; ++c) {
+        const int col0 = col_base + 64 * c;
+        if (col0 >= p.n) break;
+        uint8_t* buf = stage + sbuf * kStoreBox;
+        const uint32_t sb = smem_u32(buf);
+#pragma unroll
+        for (int jp = 0; jp < 4; ++jp) {
+            uint32_t r[4];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int j = 8 * c + 2 * jp + h;
+                const int col = col_base + 8 * j + 2 * q;
+                float v0 = acc[4 * j], v1 = acc[4 * j + 1], v2 = acc[4 * j + 2], v3 = acc[4 * j + 3];
+                if (p.bias && col < p.n) {
+                    const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                    v0 += bb.x; v1 += bb.y; v2 += bb.x; v3 += bb.y;
+                }
+                if (p.gelu) {
+                    const float2 g0 = gelu_erf2(make_float2(v0, v1)), g1 = gelu_erf2(make_float2(v2, v3));
+                    v0 = g0.x; v1 = g0.y; v2 = g1.x; v3 = g1.y;
+                }
+                r[2 * h] = T16<T>::pack2(v0, v1);
+                r[2 * h + 1] = T16<T>::pack2(v2, v3);
+            }
+            stmatrix_x4(sb + swz128(mrow, 2 * jp + mj), r[0], r[1], r[2], r[3]);
         }
+        store_box_begin(wg_tid, cw);
+        int blk = 0;
+        if (heads) {
+            const int which = col0 / p.heads_dmodel;
+            blk = (which * p.heads_B + hb) * p.heads_H + ((col0 - which * p.heads_dmodel) >> 6);
+        }
+        if (wg_tid == 0) {
+            if (heads) tma_store_3d(tmO, buf, 0, ht0, blk);
+            else tma_store_3d(tmO, buf, col0, row0, batch);
+            bulk_commit();
+        }
+        if (straddle) {
+            const int s = p.heads_T - ht0;
+            uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + (long long)(blk + p.heads_H) * p.heads_T * 128;
+            for (int i = wg_tid; i < (64 - s) * 8; i += 128) {
+                const int r = s + (i >> 3), ch = i & 7;
+                *reinterpret_cast<uint4*>(dst + (long long)(r - s) * 128 + ch * 16) = *reinterpret_cast<const uint4*>(buf + swz128(r, ch));
+            }
+        }
+        sbuf ^= 1;
+    }
+}
+
+// GEMM_OUT_F32 / GEMM_OUT_F32_ADD / GEMM_OUT_F32_GELU_POS epilogue of one consumer warpgroup, per 32-column chunk.  F32_ADD: the chunk of
+// the residual x was TMA-loaded into the staging box (chunks 0 and 1 during the tile's mainloop, chunk c + 1 while chunk c is being
+// computed); each thread reads its x from the box and writes x + (acc + bias) back in place before the box is stored.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_store32(const GemmKParams& p, const CUtensorMap* tmO, const float (&acc)[BN / 2],
+                                                      uint8_t* stage, uint64_t* rbar, int& sbuf, uint32_t& rphase, int wg_tid, int cw,
+                                                      int batch, int row0, int col_base) {
+    const int lane = wg_tid & 31;
+    const int q = lane & 3;
+    const int r_top = 16 * (wg_tid >> 5) + (lane >> 2);   // and r_top + 8 (same row % 8, so the same swizzle)
+    const bool add = p.mode == GEMM_OUT_F32_ADD, pos = p.mode == GEMM_OUT_F32_GELU_POS;
+#pragma unroll
+    for (int c = 0; c < BN / 32; ++c) {
+        const int col0 = col_base + 32 * c;
+        if (col0 >= p.n) break;
+        uint8_t* buf = stage + sbuf * kStoreBox;
+        if (add) {
+            if (wg_tid == 0 && c >= 1 && c + 1 < BN / 32 && col0 + 32 < p.n) {
+                bulk_wait_read_all();   // the other box's store (chunk c - 1) has left shared memory
+                mbar_expect_tx(&rbar[sbuf ^ 1], kStoreBox);
+                tma_load_3d(stage + (sbuf ^ 1) * kStoreBox, tmO, &rbar[sbuf ^ 1], col0 + 32, row0, batch);
+            }
+            mbar_wait(&rbar[sbuf], (rphase >> sbuf) & 1u);
+            rphase ^= 1u << sbuf;
+        }
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * c + jj;
+            const int col = col_base + 8 * j + 2 * q;
+            float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+            if (p.bias && col < p.n) {
+                const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                v[0] += bb.x; v[1] += bb.y; v[2] += bb.x; v[3] += bb.y;
+            }
+            if (p.gelu) {
+                const float2 g0 = gelu_erf2(make_float2(v[0], v[1])), g1 = gelu_erf2(make_float2(v[2], v[3]));
+                v[0] = g0.x; v[1] = g0.y; v[2] = g1.x; v[3] = g1.y;
+            }
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                const int r = r_top + 8 * half;
+                float2* s = reinterpret_cast<float2*>(buf + swz128(r, 2 * jj + (q >> 1)) + (q & 1) * 8);
+                float2 o = make_float2(v[2 * half], v[2 * half + 1]);
+                if (add) {
+                    const float2 x = *s;
+                    o = make_float2(x.x + o.x, x.y + o.y);
+                } else if (pos) {
+                    const int row_in_batch = row0 + r;
+                    if (row_in_batch < p.m_rows_per_batch && col < p.n) {
+                        const float2 pp = __ldg(reinterpret_cast<const float2*>(p.pos + (long long)row_in_batch * p.ld_pos + col));
+                        o = make_float2(o.x + pp.x, o.y + pp.y);
+                    }
+                }
+                *s = o;
+            }
+        }
+        store_box_begin(wg_tid, cw);
+        if (wg_tid == 0) {
+            tma_store_3d(tmO, buf, col0, row0, batch);
+            bulk_commit();
+        }
+        sbuf ^= 1;
     }
 }
 
@@ -147,15 +271,19 @@ __device__ __forceinline__ void gemm_epilogue_fp8_heads(const GemmKParams& p, in
     }
 }
 
-template <typename T, int BN, bool FP8_HEADS = false>
+template <typename T, int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+                  const GemmKParams p) {
+    constexpr bool kStore = EPI == kEpiStore16 || EPI == kEpiStore32;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // manual 1024-byte alignment (SWIZZLE_128B atoms are 1024 B)
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int stage_bytes = kStageA + p.stage_b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
+    uint8_t* store_stage = smem + (size_t)p.stages * stage_bytes;   // kStoreBytes for the TMA-store epilogues, else nothing
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(store_stage + p.store_bytes);
     uint64_t* empty_bar = full_bar + kMaxStages;
+    uint64_t* res_bar = empty_bar + kMaxStages;   // [warpgroup][box]: F32_ADD residual loads
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -164,10 +292,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
+        if (kStore) tma_prefetch_desc(&tmO);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
         }
+        for (int i = 0; i < 4; ++i) mbar_init(&res_bar[i], 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -231,8 +361,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ===================== consumer warpgroups =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int cw = (warp >> 2) - 1;                       // 0 / 1: rows [64 cw, 64 cw + 64) of the tile
+    const int wg_tid = threadIdx.x & 127;
     const int r_lo = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: r_lo and r_lo + 8
     const int c_lo = 2 * (lane & 3);                      // and columns 8 j + c_lo, + 1
+    uint8_t* my_stage = store_stage + cw * 2 * kStoreBox;
+    uint64_t* my_res_bar = res_bar + 2 * cw;
+    int sbuf = 0;            // staging box the next chunk goes to
+    uint32_t rphase = 0;     // parity of my_res_bar[0 / 1]
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
@@ -243,6 +378,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int m_tile = t / p.tiles_n;
         const int batch = m_tile / p.tiles_per_batch;
         const int tile_row0 = (m_tile % p.tiles_per_batch) * kBlockM;
+        const int col_base = n_tile * BN;
+        const int wg_row0 = tile_row0 + 64 * cw;         // this warpgroup's first row (in its batch)
+        const bool wg_rows = wg_row0 < p.m_rows_per_batch;
 
         int prev = -1;
         for (int kb = 0; kb < p.kb_per_split; ++kb) {
@@ -255,6 +393,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             for (int k = 0; k < kBlockK / 16; ++k)   // +32 bytes per 16 K elements inside the swizzle row (>> 4 -> +2k)
                 Wgmma<T, BN>::ss(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
             wgmma_commit();
+            if (EPI == kEpiStore32 && kb == 0 && p.mode == GEMM_OUT_F32_ADD && wg_tid == 0 && wg_rows) {
+                // residual chunks 0 and 1 of this tile, fetched while the MMAs run; the boxes are free once the previous tile's stores
+                // have read them
+                bulk_wait_read_all();
+                for (int c = 0; c < 2 && c < BN / 32 && col_base + 32 * c < p.n; ++c) {
+                    const int b = sbuf ^ c;
+                    mbar_expect_tx(&my_res_bar[b], kStoreBox);
+                    tma_load_3d(my_stage + b * kStoreBox, &tmO, &my_res_bar[b], col_base + 32 * c, wg_row0, batch);
+                }
+            }
             wgmma_wait<1>();   // the MMAs of the previous k-block have retired: its stage may be refilled
             if (prev >= 0) {
                 __syncwarp();
@@ -267,21 +415,31 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-        const int col_base = n_tile * BN;
-        if constexpr (FP8_HEADS) {
+        if constexpr (EPI == kEpiFp8Heads) {
             gemm_epilogue_fp8_heads<BN>(p, batch, tile_row0, r_lo, c_lo, col_base, acc);
+        } else if constexpr (EPI == kEpiStore16) {
+            if (wg_rows) gemm_epilogue_store16<T, BN>(p, &tmO, acc, my_stage, sbuf, wg_tid, cw, batch, wg_row0, col_base);
+        } else if constexpr (EPI == kEpiStore32) {
+            if (wg_rows) gemm_epilogue_store32<BN>(p, &tmO, acc, my_stage, my_res_bar, sbuf, rphase, wg_tid, cw, batch, wg_row0, col_base);
         } else {
+            // GEMM_OUT_PARTIAL_T: out32[split][col][row] = acc, columns past partial_cols dropped
+            float* o = reinterpret_cast<float*>(p.out);
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
                 const int row_in_batch = tile_row0 + r_lo + 8 * half;
                 if (row_in_batch >= p.m_rows_per_batch) continue;
                 const long long grow = (long long)batch * p.out_rows_per_batch + row_in_batch;
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j)
-                    gemm_epilogue_pair<T>(p, split, grow, row_in_batch, col_base + 8 * j + c_lo, acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int col = col_base + 8 * j + c_lo;
+                    if (col < p.partial_cols) o[((long long)split * p.partial_cols + col) * p.ld_out + grow] = acc[4 * j + 2 * half];
+                    if (col + 1 < p.partial_cols) o[((long long)split * p.partial_cols + col + 1) * p.ld_out + grow] = acc[4 * j + 2 * half + 1];
+                }
             }
         }
     }
+    // the grid counts as complete (PDL dependents, stream order) only once its bulk stores are done
+    if (kStore && wg_tid == 0) bulk_wait_all();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -314,7 +472,9 @@ static wk_status make_tmap(CUtensorMap* tm, const void* base, int dtype, int ndi
     cuuint32_t es[3] = {1, 1, 1};
     for (int i = 0; i < ndim; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; }
     for (int i = 0; i < ndim - 1; ++i) gstr[i] = strides_bytes[i];
-    CUresult r = enc(tm, dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+    const CUtensorMapDataType ty = dtype == WK_DTYPE_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    CUresult r = enc(tm, ty,
                      (cuuint32_t)ndim, const_cast<void*>(base), gdim, gstr, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -340,28 +500,44 @@ int wgmma_tile_n(int bn) {
     return t;
 }
 
-template <typename T, int BN, bool FP8_HEADS = false>
-static cudaError_t launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKParams& p, int grid, size_t smem, int pdl,
-                               cudaStream_t stream) {
+template <typename T, int BN, int EPI>
+static cudaError_t launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const GemmKParams& p, int grid,
+                               size_t smem, int pdl, cudaStream_t stream) {
     static bool attr_set = false;
     if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<T, BN, FP8_HEADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
+        const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<T, BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    return launch_k(gemm_wgmma_kernel<T, BN, FP8_HEADS>, dim3(grid), dim3(kGemmThreads), smem, stream, pdl, tmA, tmB, p);
+    return launch_k(gemm_wgmma_kernel<T, BN, EPI>, dim3(grid), dim3(kGemmThreads), smem, stream, pdl, tmA, tmB, tmO, p);
+}
+
+// the TMA-store epilogues run 64-, 128- or 256-column tiles (gemm_wgmma rounds bn up to 64 for them)
+template <typename T, int EPI>
+static cudaError_t launch_gemm_store(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const GemmKParams& p, int grid,
+                                     size_t smem, int pdl, cudaStream_t stream) {
+    switch (p.bn) {
+        case 64: return launch_gemm<T, 64, EPI>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        case 128: return launch_gemm<T, 128, EPI>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        default: return launch_gemm<T, 256, EPI>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+    }
 }
 
 template <typename T>
-static cudaError_t launch_gemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKParams& p, int grid, size_t smem, int pdl,
-                                 cudaStream_t stream) {
-    if (p.mode == GEMM_OUT_FP8_HEADS) return launch_gemm<T, 256, true>(tmA, tmB, p, grid, smem, pdl, stream);   // bn checked by gemm_wgmma
+static cudaError_t launch_gemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const GemmKParams& p, int grid,
+                                 size_t smem, int pdl, cudaStream_t stream) {
+    switch (gemm_epi(p.mode)) {
+        case kEpiFp8Heads: return launch_gemm<T, 256, kEpiFp8Heads>(tmA, tmB, tmO, p, grid, smem, pdl, stream);   // bn checked by gemm_wgmma
+        case kEpiStore16: return launch_gemm_store<T, kEpiStore16>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        case kEpiStore32: return launch_gemm_store<T, kEpiStore32>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        default: break;
+    }
     switch (p.bn) {
-        case 16: return launch_gemm<T, 16>(tmA, tmB, p, grid, smem, pdl, stream);
-        case 32: return launch_gemm<T, 32>(tmA, tmB, p, grid, smem, pdl, stream);
-        case 64: return launch_gemm<T, 64>(tmA, tmB, p, grid, smem, pdl, stream);
-        case 128: return launch_gemm<T, 128>(tmA, tmB, p, grid, smem, pdl, stream);
-        default: return launch_gemm<T, 256>(tmA, tmB, p, grid, smem, pdl, stream);
+        case 16: return launch_gemm<T, 16, kEpiPartialT>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        case 32: return launch_gemm<T, 32, kEpiPartialT>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        case 64: return launch_gemm<T, 64, kEpiPartialT>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        case 128: return launch_gemm<T, 128, kEpiPartialT>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+        default: return launch_gemm<T, 256, kEpiPartialT>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
     }
 }
 
@@ -393,13 +569,17 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream) {
     p.n = d.n;
     // wgmma tile width: the requested bn rounded up to a power of two (columns past n / partial_cols are zero-filled by TMA and never stored)
     p.bn = wgmma_tile_n(d.bn);
+    const int epi = gemm_epi(d.mode);
+    const bool tma_store = epi == kEpiStore16 || epi == kEpiStore32;
+    if (tma_store && p.bn < 64) p.bn = 64;   // whole 64-row x 128-byte staging boxes
     p.tiles_n = (d.n + p.bn - 1) / p.bn;
     p.work = p.tiles_per_batch * p.n_batches * p.tiles_n * p.splits;
     p.stage_b_bytes = p.bn * kBlockK * 2;
     // B stage must keep 1024-byte alignment of the following A stage
     if (p.stage_b_bytes % 1024 != 0) p.stage_b_bytes = (p.stage_b_bytes + 1023) / 1024 * 1024;
     const int stage_bytes = kStageA + p.stage_b_bytes;
-    const int smem_budget = kSmemMax - 1024 /*align slack*/ - 256 /*barriers*/;
+    p.store_bytes = tma_store ? kStoreBytes : 0;
+    const int smem_budget = kSmemMax - 1024 /*align slack*/ - 256 /*barriers*/ - p.store_bytes;
     int stages = smem_budget / stage_bytes;
     if (stages > kMaxStages) stages = kMaxStages;
     if (stages > total_kb / p.splits + 2) stages = total_kb / p.splits + 2;
@@ -423,8 +603,16 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream) {
         set_error("gemm_wgmma: the FP8 heads epilogue needs 256-column tiles and head-aligned columns (bn %d n %d d %d)", p.bn, d.n, d.heads_dmodel);
         return WK_ERR_INVALID_ARGUMENT;
     }
+    if (d.mode == GEMM_OUT_T16_HEADS &&
+        (p.n_batches != 1 || d.n % 64 != 0 || d.heads_dmodel % 64 != 0 || d.n % d.heads_dmodel != 0 || d.m_rows_per_batch % d.heads_T != 0)) {
+        // a 64-column chunk is one head; rows are whole windows of heads_T
+        set_error("gemm_wgmma: the 16-bit heads epilogue needs head-aligned columns and whole windows (n %d d %d rows %d T %d)", d.n,
+                  d.heads_dmodel, d.m_rows_per_batch, d.heads_T);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
 
-    CUtensorMap tmA, tmB;
+    CUtensorMap tmA, tmB, tmO;
+    memset(&tmO, 0, sizeof(tmO));
     wk_status st;
     if (p.a_is_3d) {
         uint64_t dims[3] = {(uint64_t)d.a_cols, (uint64_t)d.a_rows, (uint64_t)d.a_batches};
@@ -445,12 +633,28 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream) {
         st = make_tmap(&tmB, d.b, d.in_dtype, 2, dims, str, box);
         if (st != WK_OK) return st;
     }
-    const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + 256;
+    if (d.mode == GEMM_OUT_T16_HEADS) {
+        // the [which][b][h][t][64] cache as {64, T, which * b * h}: the 64 rows of one head of a warpgroup are one box
+        uint64_t dims[3] = {64, (uint64_t)d.heads_T, (uint64_t)(d.n / d.heads_dmodel) * d.heads_B * d.heads_H};
+        uint64_t str[2] = {128, (uint64_t)d.heads_T * 128};
+        uint32_t box[3] = {64, 64, 1};
+        st = make_tmap(&tmO, d.out, d.in_dtype, 3, dims, str, box);
+    } else if (tma_store) {
+        // [batch][rows][ld_out] with m_rows_per_batch valid rows and n valid columns per batch: TMA clips ragged tiles
+        const int out_dtype = epi == kEpiStore16 ? d.in_dtype : WK_DTYPE_F32;
+        const uint64_t es = epi == kEpiStore16 ? 2 : 4;
+        uint64_t dims[3] = {(uint64_t)d.n, (uint64_t)d.m_rows_per_batch, (uint64_t)p.n_batches};
+        uint64_t str[2] = {(uint64_t)d.ld_out * es, (uint64_t)d.out_rows_per_batch * d.ld_out * es};
+        uint32_t box[3] = {(uint32_t)(128 / es), 64, 1};
+        st = make_tmap(&tmO, d.out, out_dtype, 3, dims, str, box);
+    }
+    if (st != WK_OK) return st;
+    const size_t smem_bytes = (size_t)stages * stage_bytes + p.store_bytes + 1024 + 256;
     int grid = p.work < num_sms ? p.work : num_sms;
     if (grid < 1) return WK_OK;
     const int pdl = d.pdl != 0 ? 16 : 0;
-    cudaError_t e = d.in_dtype == WK_DTYPE_F16 ? launch_gemm_n<__half>(tmA, tmB, p, grid, smem_bytes, pdl, stream)
-                                               : launch_gemm_n<__nv_bfloat16>(tmA, tmB, p, grid, smem_bytes, pdl, stream);
+    cudaError_t e = d.in_dtype == WK_DTYPE_F16 ? launch_gemm_n<__half>(tmA, tmB, tmO, p, grid, smem_bytes, pdl, stream)
+                                               : launch_gemm_n<__nv_bfloat16>(tmA, tmB, tmO, p, grid, smem_bytes, pdl, stream);
     count_launch();
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) {

@@ -127,6 +127,16 @@ typedef struct wk_decode_opts {
      * word timestamps do not combine with it. */
     int32_t beam_size;            /* <= 1: greedy / temperature sampling (default) */
     float beam_patience;          /* default 1 */
+    /* DecodingOptions.detectLanguage (Configurations.swift:165,222; TranscribeTask.swift:340-365): on a multilingual model with
+     * language_token < 0, every window detects its language inside the decode loop - TextDecoder.detectLanguage's forward ([SOT] at
+     * position 0) is the loop's own step 0 when the prompt starts with SOT, else one leading step that is not counted in `steps`.
+     * LanguageLogitsFilter over language_tokens + the rung's sampler (argmax at temperature 0, top-k draw with its own Philox counter
+     * above); each temperature-ladder rung detects again.  With use_prefill_prompt, a language token right after the prompt's first SOT
+     * (the <|xx|> prefillDecoderInputs writes, TextDecoder.swift:176-186) is replaced by the detected one; otherwise the language is only
+     * reported (wk_session_languages, wk_transcription_language).  0 = off: a zeroed tail decodes as before. */
+    int32_t detect_language;
+    const int32_t* language_tokens;   /* tokenizer.allLanguageTokens: 1..4096 ids < vocab, one list for every detecting window of a call */
+    int32_t n_language_tokens;
 } wk_decode_opts;
 
 /* Per-window DecodingResult (Models.swift:383-439) in flat arrays; tokens = SOT..EOT slice. */
@@ -223,6 +233,10 @@ wk_status wk_decode_text(wk_session* s, const wk_special_tokens* st, const wk_de
  * live when their burst started (an upper bound of the rows that actually streamed K/V), [2] windows admitted to a slot, [3] ladder
  * re-admissions. */
 wk_status wk_session_stats(const wk_session* s, int64_t* out4);
+/* Language detected for windows [first, first + n) of the session's last batched call (DecodingResult.language as a token id):
+ * tokens[i] = the <|xx|> id from the rung whose result was returned, logprobs[i] = its log-prob (log-softmax over language_tokens at
+ * temperature 0); -1 and 0 for a window that did not detect.  Either output may be NULL. */
+wk_status wk_session_languages(const wk_session* s, int32_t first, int32_t n, int32_t* tokens, float* logprobs);
 /* Device logits of the last step, copied to host (debug / parity). */
 wk_status wk_session_last_logits(wk_session* s, float* logits_out);
 
@@ -328,6 +342,9 @@ wk_status wk_transcription_segments(const wk_transcription* t, wk_segment* segs,
 wk_status wk_transcription_tokens(const wk_transcription* t, int32_t* tokens, float* logprobs, int64_t cap);
 int32_t wk_transcription_word_count(const wk_transcription* t);
 wk_status wk_transcription_word(const wk_transcription* t, int32_t i, wk_word* out);   /* .segment indexes wk_transcription_segments */
+/* TranscriptionResult.language of one stream (TranscribeTask.swift:71,292,352): the language of the stream's last window (in stream time)
+ * that detected one (opts->detect_language), else token -1 and log-prob 0. */
+wk_status wk_transcription_language(const wk_transcription* t, int32_t stream, int32_t* token, float* logprob);
 void wk_transcription_free(wk_transcription* t);
 
 /* ---- word timestamps (SURVEY section 8f row 1) ----

@@ -29,6 +29,22 @@ MAX_TOKEN_CONTEXT = 224  # Constants.maxTokenContext (Models.swift:1334)
 WINDOW_SAMPLES = 480000  # Constants.defaultWindowSamples (Models.swift:1457)
 FALLBACK_REASONS = {0: None, 1: "firstTokenLogProbThreshold", 2: "silence", 3: "compressionRatioThreshold",
                     4: "logProbThreshold"}
+# Whisper's language codes in vocabulary order: <|en|> is englishToken, the rest follow it (Constants.languages, Models.swift)
+LANGUAGE_CODES = (
+    "en zh de es ru ko fr ja pt tr pl ca nl ar sv it id hi fi vi he uk el ms cs ro da hu ta no th ur hr bg lt la mi ml cy sk te fa lv bn "
+    "sr az sl kn et mk br eu is hy ne mn bs kk sq sw gl mr pa si km sn yo so af oc ka be tg sd gu am yi lo uz fo ht ps tk nn mt sa lb "
+    "my bo tl mg as tt haw ln ha ba jw su yue").split()
+
+
+def language_tokens(specialTokens: "SpecialTokens", vocab: int, tokenizer=None) -> List[int]:
+    """tokenizer.allLanguageTokens: the tokenizer's <|xx|> ids, or without one the vocabulary's language block
+    [englishToken, translateToken) (100 ids on large-v3, 99 on the older multilingual vocabularies); [] for an English-only model."""
+    if vocab == 51864:
+        return []
+    if tokenizer is not None:
+        ids = [tokenizer.convertTokenToId(f"<|{c}|>") for c in LANGUAGE_CODES]
+        return [int(i) for i in ids if i is not None and 0 <= i < vocab]
+    return list(range(specialTokens.englishToken, specialTokens.translateToken))
 
 
 def _ptr(x):
@@ -91,6 +107,14 @@ class DecodingOptions:
     seed: int = 0
     beamSize: int = 1                 # extension: the reference's BeamSearchTokenSampler is an unimplemented stub (TokenSampler.swift:254-290)
     beamPatience: float = 1.0
+    # detect each window's language inside the decode loop (multilingual model, no language set); None = !usePrefillPrompt, as the
+    # reference resolves it (Configurations.swift:222)
+    detectLanguage: Optional[bool] = None
+    allLanguageTokens: Optional[List[int]] = None   # tokenizer.allLanguageTokens; WhisperKit.resolveLanguage fills it
+
+    @property
+    def detectsLanguage(self) -> bool:
+        return bool(self.detectLanguage) if self.detectLanguage is not None else not self.usePrefillPrompt
 
     def to_c(self):
         """Returns (struct, keepalive) - keepalive holds the int arrays the struct points into."""
@@ -132,6 +156,9 @@ class DecodingOptions:
         o.word_timestamps = int(self.wordTimestamps)
         o.beam_size = int(self.beamSize)
         o.beam_patience = float(self.beamPatience)
+        o.detect_language = int(self.detectsLanguage)
+        lt, nlt = arr(self.allLanguageTokens)
+        o.language_tokens, o.n_language_tokens = lt, max(nlt, 0)
         return o, keep
 
 
@@ -153,6 +180,10 @@ class DecodingResult:
     currentTokenCount: int = 0
     steps: int = 0
     isFirstTokenLogProbTooLow: bool = False
+    # the language detected in the decode loop (detectLanguage): <|xx|> id, its log-prob, and "xx" when a tokenizer is present
+    languageToken: Optional[int] = None
+    languageLogProb: Optional[float] = None
+    language: Optional[str] = None
 
     @staticmethod
     def from_c(r: wk_decode_result) -> "DecodingResult":
@@ -161,6 +192,29 @@ class DecodingResult:
         fb = DecodingFallback(bool(r.needs_fallback), reason) if reason else None
         return DecodingResult(list(r.tokens[:n]), list(r.token_logprobs[:n]), r.avg_logprob, r.compression_ratio,
                               r.temperature, fb, r.n_current_tokens, r.steps, bool(r.first_token_logprob_too_low))
+
+
+def language_code(tokenizer, token: int) -> str:
+    """DecodingResult.language of a detected <|xx|> token (TextDecoder.swift:516-523): its code, or "en" when the code is unknown."""
+    code = tokenizer.decode([int(token)]).strip()
+    if code.startswith("<|") and code.endswith("|>"):
+        code = code[2:-2]
+    return code if code in LANGUAGE_CODES else "en"
+
+
+def session_languages(lib, session, n: int):
+    """wk_session_languages for windows [0, n) of the session's last batched call: (tokens, logprobs), -1 / 0 = no detection."""
+    tok = (C.c_int32 * max(1, n))()
+    lp = (C.c_float * max(1, n))()
+    check(lib.wk_session_languages(session, 0, n, tok, lp))
+    return [int(v) for v in tok[:n]], [float(v) for v in lp[:n]]
+
+
+def attach_languages(results: List["DecodingResult"], tokens: Sequence[int], logprobs: Sequence[float], tokenizer=None) -> None:
+    for r, t, lp in zip(results, tokens, logprobs):
+        if isinstance(r, DecodingResult) and t >= 0:
+            r.languageToken, r.languageLogProb = int(t), float(lp)
+            r.language = language_code(tokenizer, t) if tokenizer is not None else None
 
 
 _DT = {"f32": WK_DTYPE_F32, "f16": WK_DTYPE_F16, "bf16": WK_DTYPE_BF16}
@@ -430,10 +484,14 @@ class TextDecoder:
             self.bindEncoderOutput(encoderOutput)
         st = specialTokens.to_c()
         n = self.batch
-        bo, keep = make_batch_opts(n, options, prompt, callback, callbackEvery, None)
+        opts = [with_language_tokens(o, specialTokens, self.logitsSize) for o in options] if isinstance(options, (list, tuple)) \
+            else with_language_tokens(options, specialTokens, self.logitsSize)
+        bo, keep = make_batch_opts(n, opts, prompt, callback, callbackEvery, None)
         res = (wk_decode_result * n)()
         check(self.lib.wk_decode_text_ex(self.handle, C.byref(st), C.byref(bo), res))
-        return [DecodingResult.from_c(r) for r in res]
+        out = [DecodingResult.from_c(r) for r in res]
+        attach_languages(out, *session_languages(self.lib, self.handle, n))
+        return out
 
     def detectLanguage(self, encoderOutput: Optional[DeviceTensor], specialTokens: SpecialTokens, allLanguageTokens: Sequence[int],
                        temperature: float = 0.0):
@@ -474,6 +532,14 @@ class TextDecoder:
             self.close()
         except Exception:
             pass
+
+
+def with_language_tokens(opts: DecodingOptions, specialTokens: SpecialTokens, vocab: int, tokenizer=None) -> DecodingOptions:
+    """Fills DecodingOptions.allLanguageTokens when the options detect the language and carry no list."""
+    if opts.allLanguageTokens is not None or not opts.detectsLanguage or vocab == 51864:
+        return opts
+    import dataclasses
+    return dataclasses.replace(opts, allLanguageTokens=language_tokens(specialTokens, vocab, tokenizer))
 
 
 def make_batch_opts(n: int, options, prompt, callback=None, callbackEvery: int = 0, status=None, encoderChunk: int = 0):
@@ -606,7 +672,10 @@ class WhisperKit:
 
     def resolveLanguage(self, opts: DecodingOptions) -> DecodingOptions:
         """DecodingOptions.language -> the "<|xx|>" token id through the tokenizer, as prefillDecoderInputs does with
-        tokenizer.convertTokenToId (TextDecoder.swift:181-186).  No tokenizer = an error, never a silent <|en|>."""
+        tokenizer.convertTokenToId (TextDecoder.swift:181-186).  No tokenizer = an error, never a silent <|en|>.  Options that detect
+        the language get allLanguageTokens (the tokenizer's <|xx|> ids, else the vocabulary's language block)."""
+        if opts.language is None and opts.languageToken is None:
+            return with_language_tokens(opts, self.specialTokens, self.model.info.vocab, self.tokenizer)
         if opts.language is None or opts.languageToken is not None or not self.textDecoder.isModelMultilingual:
             return opts
         if self.tokenizer is None:
@@ -650,4 +719,5 @@ class WhisperKit:
                 out.append(WhisperError(int(status[i]), f"window {i} failed"))
             else:
                 out.append(DecodingResult.from_c(r))
+        attach_languages(out, *session_languages(self.model.lib, self.textDecoder.handle, n), tokenizer=self.tokenizer)
         return out

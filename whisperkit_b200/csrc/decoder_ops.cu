@@ -60,6 +60,9 @@ __global__ void decode_slots_init_kernel(DecodeState st, RowParams* __restrict__
         st.steps[b] = 0;
         st.input_ids[b] = 0;
         st.error[b] = 0;
+        st.lang_token[b] = -1;
+        st.lang_logprob[b] = 0.f;
+        st.lang_state[b] = R.detect == 2 ? kLangLead : 0;
         if (bs.beam > 1) {
             bs.sum_lp[b] = 0.f;
             if (b % bs.beam == 0) bs.n_fin[b / bs.beam] = 0;
@@ -100,7 +103,10 @@ decoder_embed_ln_kernel(const T* __restrict__ emb, const float* __restrict__ pos
         pos = step;
         tok = st.next_token[b];
         bool overwrite = false;
-        if (step < prompt_len) {
+        const int lang_state = st.lang_state[b];
+        if (lang_state == kLangLead) {
+            tok = st.rp[b].lead_token;   // leading language-detection step: [SOT] at position 0 (steps[b] is still 0)
+        } else if (step < prompt_len) {
             const int cur = st.tokens[b * kMaxCtx + step];
             const bool is_ts = cur >= ts_begin, pred_ts = tok >= ts_begin;
             if (!(step == prompt_len - 1 && is_ts && pred_ts)) tok = cur;
@@ -110,6 +116,7 @@ decoder_embed_ln_kernel(const T* __restrict__ emb, const float* __restrict__ pos
         if (tid == 0) {
             if (overwrite) st.tokens[b * kMaxCtx + step] = tok;
             st.input_ids[b] = tok;
+            if (lang_state == kLangLeadRan) st.lang_state[b] = 0;   // the previous step was the leading detection step: this is step 0
         }
     }
     tok = min(max(tok, 0), vocab - 1);   // never index the embedding table out of bounds
@@ -663,21 +670,22 @@ static wk_status launch_cross(const float* partial, int splits, int Bp, const fl
 // The beam-search form (NQ rows share one K/V block) lives in cross_attention_mq.cu: both products on the tensor cores.
 
 __global__ void decoder_align_mean_kernel(const float* __restrict__ scratch, int n_slots, const int32_t* __restrict__ steps,
-                                          const int32_t* __restrict__ done, __half* __restrict__ out, int B, int Tlen, int max_rows) {
+                                          const int32_t* __restrict__ done, const int32_t* __restrict__ lang_state, __half* __restrict__ out,
+                                          int B, int Tlen, int max_rows) {
     const int b = blockIdx.y, t = blockIdx.x * blockDim.x + threadIdx.x;
     // launched after the sampler advanced the row's step: steps[b] = tokenIndex + 1 = the row of this step's slice; a window whose
     // segment just completed (or completed earlier) gets no row - the reference breaks out of its loop before updateAlignmentWeights
-    // (TextDecoder.swift:668-674,709-717)
+    // (TextDecoder.swift:668-674,709-717); nor does the leading language-detection step, which is not a step of decodeText
     const int row = steps[b];
-    if (t >= Tlen || row >= max_rows || done[b]) return;
+    if (t >= Tlen || row >= max_rows || done[b] || (lang_state != nullptr && lang_state[b] == kLangLeadRan)) return;
     float a = 0.f;
     for (int s = 0; s < n_slots; ++s) a += scratch[((long long)s * B + b) * Tlen + t];   // fixed order: deterministic
     out[((long long)b * max_rows + row) * Tlen + t] = __float2half(a / (float)n_slots);
 }
 
-wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* steps, const int32_t* done, void* out_f16, int B, int T,
-                             int max_rows, cudaStream_t stream) {
-    launch_k(decoder_align_mean_kernel, dim3((T + 255) / 256, B), dim3(256), 0, stream, 0, scratch, n_slots, steps, done, (__half*)out_f16, B, T, max_rows);
+wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* steps, const int32_t* done, const int32_t* lang_state,
+                             void* out_f16, int B, int T, int max_rows, cudaStream_t stream) {
+    launch_k(decoder_align_mean_kernel, dim3((T + 255) / 256, B), dim3(256), 0, stream, 0, scratch, n_slots, steps, done, lang_state, (__half*)out_f16, B, T, max_rows);
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("decoder_align_mean launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
@@ -721,6 +729,89 @@ __device__ __forceinline__ ArgMax argmax_better(ArgMax a, ArgMax b) {
     return a;
 }
 
+// block-wide argmax (first maximal index) over srow[lo, V); srow is only read; the result is identical in every thread
+__device__ __forceinline__ ArgMax block_argmax_row(const float* srow, int lo, int V, ArgMax* sarg) {
+    const int tid = threadIdx.x;
+    ArgMax best = {-INFINITY, 0x7fffffff};
+    for (int i = lo + tid; i < V; i += kSamplerThreads) {
+        const float x = srow[i];
+        if (x > best.v) { best.v = x; best.i = i; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        ArgMax other;
+        other.v = __shfl_xor_sync(0xffffffffu, best.v, o);
+        other.i = __shfl_xor_sync(0xffffffffu, best.i, o);
+        best = argmax_better(best, other);
+    }
+    __syncthreads();
+    if ((tid & 31) == 0) sarg[tid >> 5] = best;
+    __syncthreads();
+    best = sarg[tid & 31];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        ArgMax other;
+        other.v = __shfl_xor_sync(0xffffffffu, best.v, o);
+        other.i = __shfl_xor_sync(0xffffffffu, best.i, o);
+        best = argmax_better(best, other);
+    }
+    return best;
+}
+
+// GreedyTokenSampler.update on a filtered row staged in smem, restricted to [lo, V) whose max is `m` and log-sum-exp `lse`:
+// temperature 0 = argmax; > 0 = logits / T, softmax over the whole (filtered) range, top-k, multinomial draw inside the top-k mass,
+// logprob = log softmax prob of the draw (TokenSampler.swift:57-73 / :140-180).  The reference draws with Float.random
+// (non-deterministic); here the draw is Philox(seed, subsequence, offset).  Returns the token in .i (out of [0, V) if the row has no
+// finite logit) and its log-prob in .v; srow is modified at T > 0.
+__device__ __forceinline__ ArgMax sample_row(float* srow, int lo, int V, float m, float lse, float temperature, int top_k, uint64_t seed,
+                                             unsigned long long subsequence, unsigned long long offset, float* scratch, ArgMax* sarg) {
+    const int tid = threadIdx.x;
+    ArgMax best;
+    if (temperature == 0.f) {
+        best = block_argmax_row(srow, lo, V, sarg);
+        best.v = best.v - lse;
+        return best;
+    }
+    const float inv_t = 1.f / temperature;
+    const float zmax = m * inv_t;
+    float z = 0.f;
+    for (int i = lo + tid; i < V; i += kSamplerThreads) {
+        const float x = srow[i];
+        if (x != -INFINITY) z += __expf(x * inv_t - zmax);
+    }
+    z = block_sum(z, scratch);
+    __shared__ float topv[32];
+    __shared__ int topi[32];
+    const int k = top_k < 1 ? 1 : (top_k > 32 ? 32 : top_k);
+    int kk = 0;
+    for (; kk < k; ++kk) {
+        const ArgMax a = block_argmax_row(srow, lo, V, sarg);
+        if (a.v == -INFINITY) break;
+        if (tid == 0) { topv[kk] = __expf(a.v * inv_t - zmax) / z; topi[kk] = a.i; srow[a.i] = -INFINITY; }
+        __syncthreads();
+    }
+    __syncthreads();
+    float mass = 0.f;
+    for (int j = 0; j < kk; ++j) mass += topv[j];
+    curandStatePhilox4_32_10_t rng;
+    curand_init(seed, subsequence, offset, &rng);
+    const float u = 1.f - curand_uniform(&rng);   // [0, 1)
+    const float rnd = u * mass;
+    float acc = 0.f;
+    int chosen = kk > 0 ? kk - 1 : 0;
+    for (int j = 0; j < kk; ++j) {
+        acc += topv[j];
+        if (rnd < acc) { chosen = j; break; }
+    }
+    best.i = kk > 0 ? topi[chosen] : 0x7fffffff;
+    best.v = kk > 0 ? logf(topv[chosen]) : -INFINITY;
+    return best;
+}
+
+// Philox subsequences of the in-loop language detection draws: row b uses kDetectSubsequence + b, apart from the loop's own draws
+// (subsequence b), so that detecting moves no token draw of the decode
+static constexpr unsigned long long kDetectSubsequence = 1ull << 32;
+
 __global__ void __launch_bounds__(kSamplerThreads)
 sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerParams p, DecodeState st,
                const int32_t* __restrict__ tokens_in, int ld_tokens, const int32_t* __restrict__ n_tokens_in,
@@ -743,10 +834,50 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         R.prompt_len = -1; R.sample_begin_ts = p.sample_begin_ts; R.sample_begin_blank = p.sample_begin_blank; R.max_steps = 0;
         R.temperature = p.temperature; R.top_k = p.top_k; R.has_first_thr = 0; R.first_thr = 0.f; R.seed = p.seed;
         R.suppress_off = 0; R.n_suppress = p.n_suppress;
+        R.detect = 0; R.lang_pos = -1; R.n_lang = 0; R.lead_token = 0;
     }
     const int32_t* toks = loop_mode ? st.tokens + b * kMaxCtx : tokens_in + (long long)b * ld_tokens;
-    const int n_tok = loop_mode ? st.n_tokens[b] : n_tokens_in[b];
     const wk_special_tokens& S = p.st;
+
+    if (loop_mode && R.detect) {
+        // DecodingOptions.detectLanguage: this step's logits are those of TextDecoder.detectLanguage (TextDecoder.swift:420-539) - [SOT] at
+        // position 0 - either because the row's step 0 is that forward or because this is the row's leading detection step.
+        // LanguageLogitsFilter alone on the raw row, then the rung's sampler; the <|xx|> slot of the prompt takes the detected language
+        // before a later step forces it (prefillDecoderInputs with the detected language, TranscribeTask.swift:354-357)
+        const bool lead = st.lang_state[b] == kLangLead;
+        if (lead || (R.detect == 1 && st.steps[b] == 0)) {
+            const float* row = logits + (long long)b * ld_logits;
+            for (int i = tid; i < V; i += kSamplerThreads) srow[i] = -INFINITY;
+            __syncthreads();
+            for (int j = tid; j < R.n_lang; j += kSamplerThreads) {
+                const int t = p.detect_tokens[j];
+                if (t >= 0 && t < V) srow[t] = row[t];
+            }
+            __syncthreads();
+            float mx = -INFINITY;
+            for (int i = tid; i < V; i += kSamplerThreads) mx = fmaxf(mx, srow[i]);
+            mx = block_max(mx, scratch);
+            float sm = 0.f;
+            for (int i = tid; i < V; i += kSamplerThreads) {
+                const float x = srow[i];
+                if (x != -INFINITY) sm += __expf(x - mx);
+            }
+            sm = block_sum(sm, scratch);
+            const ArgMax d = sample_row(srow, 0, V, mx, mx + logf(sm), R.temperature, R.top_k, R.seed, kDetectSubsequence + (unsigned long long)b, 0ull,
+                                        scratch, sarg);
+            if (tid == 0) {
+                const bool ok = d.i >= 0 && d.i < V;
+                st.lang_token[b] = ok ? d.i : -1;
+                st.lang_logprob[b] = ok ? d.v : 0.f;
+                if (ok && R.lang_pos >= 0) st.tokens[b * kMaxCtx + R.lang_pos] = d.i;
+                if (lead) st.lang_state[b] = kLangLeadRan;
+            }
+            __syncthreads();
+            // the leading step ends here: no sample, no bookkeeping - the row starts its step 0 next
+            if (lead) return;
+        }
+    }
+    const int n_tok = loop_mode ? st.n_tokens[b] : n_tokens_in[b];
 
     if (tid == 0) {
         // ---- TimestampRulesFilter rule state (LogitsFilter.swift:72-109)
@@ -859,39 +990,12 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         for (int i = tid; i < V; i += kSamplerThreads) filtered_out[(long long)b * V + i] = srow[i];
         __syncthreads();
     }
-    // ---- block-wide argmax (first maximal index) over [lo, V); srow is only read
-    auto block_argmax = [&]() -> ArgMax {
-        ArgMax best = {-INFINITY, 0x7fffffff};
-        for (int i = lo + tid; i < V; i += kSamplerThreads) {
-            const float x = srow[i];
-            if (x > best.v) { best.v = x; best.i = i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            ArgMax other;
-            other.v = __shfl_xor_sync(0xffffffffu, best.v, o);
-            other.i = __shfl_xor_sync(0xffffffffu, best.i, o);
-            best = argmax_better(best, other);
-        }
-        __syncthreads();
-        if ((tid & 31) == 0) sarg[tid >> 5] = best;
-        __syncthreads();
-        best = sarg[tid & 31];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            ArgMax other;
-            other.v = __shfl_xor_sync(0xffffffffu, best.v, o);
-            other.i = __shfl_xor_sync(0xffffffffu, best.i, o);
-            best = argmax_better(best, other);
-        }
-        return best;   // identical in every thread
-    };
     if (loop_mode && p.beam.beam > 1) {
         // beam search: rank the row's (beam + 1) best tokens of the filtered log-softmax, best first (whisper BeamSearchDecoder.update step 1);
         // the per-window merge and every state update happen in beam_update_kernel
         const int k = p.beam.beam + 1;
         for (int kk = 0; kk < k; ++kk) {
-            const ArgMax a = block_argmax();
+            const ArgMax a = block_argmax_row(srow, lo, V, sarg);
             const bool ok = a.v != -INFINITY && a.i >= 0 && a.i < V;   // (a NaN row yields the initial index: no candidate)
             if (tid == 0) {
                 p.beam.cand_tok[b * (kMaxBeam + 1) + kk] = ok ? a.i : -1;
@@ -902,50 +1006,10 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         }
         return;
     }
-    ArgMax best;
-    float lp_sampled = 0.f;
-    if (R.temperature == 0.f) {
-        best = block_argmax();
-        lp_sampled = best.v - lse;
-    } else {
-        // GreedyTokenSampler with temperature (TokenSampler.swift:57-73 / :140-180): logits / T, softmax over the whole
-        // (filtered) vocabulary, top-k, multinomial draw inside the top-k mass, logprob = log softmax prob of the draw.
-        // The reference draws with Float.random (non-deterministic); here the draw is Philox(seed, row, step).
-        const float inv_t = 1.f / R.temperature;
-        const float zmax = (ts_wins ? mts : mall) * inv_t;
-        float z = 0.f;
-        for (int i = lo + tid; i < V; i += kSamplerThreads) {
-            const float x = srow[i];
-            if (x != -INFINITY) z += __expf(x * inv_t - zmax);
-        }
-        z = block_sum(z, scratch);
-        __shared__ float topv[32];
-        __shared__ int topi[32];
-        const int k = R.top_k < 1 ? 1 : (R.top_k > 32 ? 32 : R.top_k);
-        int kk = 0;
-        for (; kk < k; ++kk) {
-            const ArgMax a = block_argmax();
-            if (a.v == -INFINITY) break;
-            if (tid == 0) { topv[kk] = __expf(a.v * inv_t - zmax) / z; topi[kk] = a.i; srow[a.i] = -INFINITY; }
-            __syncthreads();
-        }
-        __syncthreads();
-        float mass = 0.f;
-        for (int j = 0; j < kk; ++j) mass += topv[j];
-        curandStatePhilox4_32_10_t rng;
-        curand_init(R.seed, (unsigned long long)b, (unsigned long long)(loop_mode ? st.steps[b] : n_tok), &rng);
-        const float u = 1.f - curand_uniform(&rng);   // [0, 1)
-        const float rnd = u * mass;
-        float acc = 0.f;
-        int chosen = kk > 0 ? kk - 1 : 0;
-        for (int j = 0; j < kk; ++j) {
-            acc += topv[j];
-            if (rnd < acc) { chosen = j; break; }
-        }
-        best.i = kk > 0 ? topi[chosen] : 0x7fffffff;
-        best.v = 0.f;
-        lp_sampled = kk > 0 ? logf(topv[chosen]) : -INFINITY;
-    }
+    // the row's draw: Philox(seed, row, step) at temperature > 0
+    const ArgMax best = sample_row(srow, lo, V, ts_wins ? mts : mall, lse, R.temperature, R.top_k, R.seed, (unsigned long long)b,
+                                   (unsigned long long)(loop_mode ? st.steps[b] : n_tok), scratch, sarg);
+    const float lp_sampled = best.v;
     if (tid == 0) {
         int tok = best.i;
         float lp = lp_sampled;
@@ -998,6 +1062,7 @@ beam_update_kernel(DecodeState st, BeamState bs, wk_special_tokens S, int max_ct
     pdl_launch_dependents();
     pdl_wait();
     if (st.done[r0]) return;
+    if (st.lang_state[r0] == kLangLeadRan) return;   // the leading language-detection step ranked nothing: no beam bookkeeping
     const RowParams R = st.rp[r0];
     const int step = st.steps[r0], n_tok = st.n_tokens[r0], P = R.prompt_len;
     const int C1 = kMaxBeam + 1;

@@ -106,7 +106,12 @@ struct RowParams {
     int32_t has_first_thr; float first_thr;
     uint64_t seed;
     int32_t suppress_off, n_suppress;   // slice of the session's suppress-token pool
-    int32_t pad_[2];
+    // DecodingOptions.detectLanguage (TranscribeTask.swift:340-365): 0 off; 1 the row's step 0 is the detection forward ([SOT] at
+    // position 0); 2 the prompt does not start with SOT, so one leading detection step runs before step 0
+    int32_t detect;
+    int32_t lang_pos;            // prompt slot of <|xx|> rewritten with the detected language, <0 = report only
+    int32_t n_lang;              // entries of SamplerParams.detect_tokens
+    int32_t lead_token;          // <|startoftranscript|>: what the leading detection step feeds at position 0
 };
 
 struct DecodeState {
@@ -121,7 +126,11 @@ struct DecodeState {
     int32_t* input_ids;   // [Bmax] token fed at this step (written by embed)
     int32_t* error;       // [Bmax] 1 = the sampler saw no finite logit (WhisperError.decodingLogitsFailed)
     const RowParams* rp;  // [Bmax]
+    int32_t* lang_token;  // [Bmax] language detected in the loop, -1 = none
+    float* lang_logprob;  // [Bmax]
+    int32_t* lang_state;  // [Bmax] kLangLead: the leading detection step is next; kLangLeadRan: it was this step's; 0 otherwise
 };
+constexpr int kLangLead = 2, kLangLeadRan = 3;
 
 // Beam search (SURVEY 8f row 2; semantics restated from openai/whisper BeamSearchDecoder in oracle/beam_ref.py - the reference's
 // BeamSearchTokenSampler is a fatalError stub, TokenSampler.swift:254-290).  Decode rows come in groups of `beam` consecutive rows per window.
@@ -146,7 +155,8 @@ struct SamplerParams {
     const int32_t* suppress; // loop mode: the pool RowParams.suppress_off indexes; stateless: the list itself
     const int32_t* language_tokens; int n_language_tokens; int language_sample_begin;
     int max_ctx;             // 224
-    BeamState beam;          // loop mode with beam.beam > 1: the kernel only ranks candidates; beam_update() does the bookkeeping
+    const int32_t* detect_tokens;   // loop mode: allLanguageTokens of the rows with RowParams.detect (in-loop language detection)
+    BeamState beam;         // loop mode with beam.beam > 1: the kernel only ranks candidates; beam_update() does the bookkeeping
     // stateless mode only
     int sample_begin_ts, sample_begin_blank, n_suppress;
     float temperature; int top_k; uint64_t seed;
@@ -185,8 +195,9 @@ wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, c
 // alignment row of the step just sampled (run AFTER the sampler advanced steps[b] to tokenIndex + 1): out[b][steps[b]][t] =
 // Float16(mean over n_slots of scratch[slot][b][t]) unless done[b] (TextDecoder.updateAlignmentWeights, TextDecoder.swift:272-296:
 // the slice of step tokenIndex lands in row tokenIndex + 1; a completed segment breaks out before the update, :668-674)
-wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* steps, const int32_t* done, void* out_f16, int B, int T,
-                             int max_rows, cudaStream_t stream);
+// A row whose step was the leading language-detection step (lang_state, may be NULL) gets no row either.
+wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* steps, const int32_t* done, const int32_t* lang_state,
+                             void* out_f16, int B, int T, int max_rows, cudaStream_t stream);
 wk_status sampler_filter_sample(const float* logits, int64_t ld_logits, SamplerParams p, DecodeState st, const int32_t* tokens,
                                 int ld_tokens, const int32_t* n_tokens, int32_t* token_out, float* logprob_out,
                                 float* filtered_out, int B, cudaStream_t stream);

@@ -239,6 +239,8 @@ struct wk_transcription {
     std::vector<int32_t> tokens;
     std::vector<float> logprobs;
     int windows = 0;
+    // per stream: the detected language of its latest window (in stream time) that detected one, and where that window started
+    std::vector<int32_t> lang; std::vector<float> lang_logprob; std::vector<int64_t> lang_at;
 };
 
 namespace {
@@ -358,6 +360,7 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
         }
     }
     wk_transcription* T = new wk_transcription();
+    T->lang.assign(n_streams, -1); T->lang_logprob.assign(n_streams, 0.f); T->lang_at.assign(n_streams, -1);
     // One round = the next window of EVERY unfinished unit (up to kRoundCap): the window scheduler behind wk_transcribe_windows keeps the
     // session's decode slots full and runs the mel + encoder pass of the following windows under the running decode, so a round is not
     // limited to one slot-load.  Host staging is pinned and kept across calls; the per-window host work that follows a round (segment
@@ -391,6 +394,17 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
         rc = wk_transcribe_windows(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, o, prompt, n_prompt, res.data());
         if (rc != WK_OK) { delete T; return rc; }
         T->windows += (int)active.size();
+        if (o->detect_language) {   // TranscriptionResult.language: the stream keeps the language of its last detecting window
+            std::vector<int32_t> lt(active.size());
+            std::vector<float> ll(active.size());
+            rc = wk_session_languages(s, 0, (int32_t)active.size(), lt.data(), ll.data());
+            if (rc != WK_OK) { delete T; return rc; }
+            for (size_t k = 0; k < active.size(); ++k) {
+                const Unit& u = units[active[k]];
+                const int64_t at = u.offset + u.seek;
+                if (lt[k] >= 0 && at >= T->lang_at[u.stream]) { T->lang[u.stream] = lt[k]; T->lang_logprob[u.stream] = ll[k]; T->lang_at[u.stream] = at; }
+            }
+        }
         const int cols = info.n_audio_ctx;
         if (o->word_timestamps) {   // every window's alignment rows back in one burst (Float16, as the reference's alignmentWeights)
             for (size_t k = 0; k < active.size(); ++k) {
@@ -518,6 +532,12 @@ wk_status wk_transcription_word(const wk_transcription* t, int32_t i, wk_word* o
     const OutWord& w = t->words[i];
     out->word = w.word.c_str(); out->tokens = w.tokens.data(); out->n_tokens = (int32_t)w.tokens.size();
     out->start = w.start; out->end = w.end; out->probability = w.probability; out->segment = w.segment;
+    return WK_OK;
+}
+wk_status wk_transcription_language(const wk_transcription* t, int32_t stream, int32_t* token, float* logprob) {
+    if (!t || stream < 0 || stream >= (int32_t)t->lang.size()) { set_error("wk_transcription_language: stream %d out of range", stream); return WK_ERR_INVALID_ARGUMENT; }
+    if (token) *token = t->lang[stream];
+    if (logprob) *logprob = t->lang_logprob[stream];
     return WK_OK;
 }
 void wk_transcription_free(wk_transcription* t) { delete t; }

@@ -43,6 +43,8 @@ struct wk_session {
     float* logits = nullptr;
     DecodeState st;
     RowParams* rp_dev = nullptr;
+    // lang_dev: allLanguageTokens of wk_detect_language and of in-loop detection.  Fixed at the 4096-entry limit, so its pointer (baked
+    // into the step graphs through SamplerParams.detect_tokens) never changes
     int32_t* pos_dev = nullptr; int32_t* lang_dev = nullptr;
     int32_t* suppress_dev = nullptr; size_t suppress_cap = 0;
     // slot admission staging (pinned host + device)
@@ -51,6 +53,9 @@ struct wk_session {
     // pinned readback of the decode state
     int32_t *h_tokens = nullptr, *h_n_tokens = nullptr, *h_done = nullptr, *h_first_low = nullptr, *h_steps = nullptr, *h_error = nullptr;
     float* h_logprobs = nullptr;
+    int32_t* h_lang_token = nullptr; float* h_lang_logprob = nullptr;
+    // language detected per window of the last batched call (wk_session_languages): -1 / 0 where a window did not detect
+    std::vector<int32_t> win_lang; std::vector<float> win_lang_logprob;
     // step graph, cached across calls: the step depends on the call only through the rows it covers, the alignment export and the
     // special-token ids baked into the sampler's parameters
     cudaGraphExec_t graph_exec = nullptr, graph_exec_live = nullptr;   // the step with / without the ended-row checks in the attention kernels
@@ -224,6 +229,7 @@ static SamplerParams loop_sampler_params(wk_session* s, const wk_special_tokens*
     p.loop_mode = 1;
     p.suppress = s->suppress_dev;
     p.max_ctx = kKvMaxLen;
+    p.detect_tokens = s->lang_dev;
     p.beam = s->bs;
     return p;
 }
@@ -319,7 +325,8 @@ static wk_status enqueue_step(wk_session* s, const wk_special_tokens* st, bool f
     WK_CHECK(sampler_filter_sample(s->logits, m->cfg.vocab, loop_sampler_params(s, st), s->st, nullptr, 0, nullptr, nullptr, nullptr, nullptr, s->batch, s->stream));
     if (s->bs.beam > 1) WK_CHECK(beam_update(s->st, s->bs, *st, kKvMaxLen, s->batch / s->bs.beam, s->stream));
     if (s->align_on)
-        WK_CHECK(decoder_align_mean(s->align_scratch, m->n_align_slots, s->st.steps, s->st.done, s->align_w, s->batch, m->cfg.n_audio_ctx, kKvMaxLen, s->stream));
+        WK_CHECK(decoder_align_mean(s->align_scratch, m->n_align_slots, s->st.steps, s->st.done, s->st.lang_state, s->align_w, s->batch, m->cfg.n_audio_ctx,
+                                    kKvMaxLen, s->stream));
     return WK_OK;
 }
 
@@ -507,6 +514,38 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             fail_window(w, WK_ERR_AUDIO_PROCESSING_FAILED);
         }
     }
+    // ---- in-loop language detection (DecodingOptions.detectLanguage): a multilingual model, no language set (TranscribeTask.swift:341)
+    const bool multilingual = c.vocab != 51864;
+    auto detects = [&](const wk_decode_opts& o) { return o.detect_language != 0 && multilingual && o.language_token < 0; };
+    std::vector<int32_t> lang_list;   // the call's allLanguageTokens: one list for every detecting window (one device buffer)
+    bool any_detect = false;
+    for (int64_t w = 0; w < n; ++w) {
+        const wk_decode_opts& o = opts_of(bo, w);
+        if (status[w] != WK_OK || !detects(o)) continue;
+        if (!o.language_tokens || o.n_language_tokens < 1 || o.n_language_tokens > 4096) {
+            set_error("window %lld: detectLanguage needs 1..4096 language tokens (got %d)", (long long)w, o.language_tokens ? o.n_language_tokens : 0);
+            fail_window(w, WK_ERR_INVALID_ARGUMENT);
+            continue;
+        }
+        bool ok = true;
+        for (int i = 0; i < o.n_language_tokens && ok; ++i)
+            if (o.language_tokens[i] < 0 || o.language_tokens[i] >= c.vocab) {
+                set_error("window %lld: language token %d outside the vocabulary (%d)", (long long)w, o.language_tokens[i], c.vocab);
+                ok = false;
+            }
+        if (ok && any_detect &&
+            ((int)lang_list.size() != o.n_language_tokens || !std::equal(lang_list.begin(), lang_list.end(), o.language_tokens))) {
+            set_error("window %lld: every detecting window of a call must carry the same language tokens", (long long)w);
+            ok = false;
+        }
+        if (!ok) { fail_window(w, WK_ERR_INVALID_ARGUMENT); continue; }
+        if (!any_detect) lang_list.assign(o.language_tokens, o.language_tokens + o.n_language_tokens);
+        any_detect = true;
+    }
+    std::vector<int32_t> lang_sorted(lang_list);
+    std::sort(lang_sorted.begin(), lang_sorted.end());
+    s->win_lang.assign((size_t)n, -1);
+    s->win_lang_logprob.assign((size_t)n, 0.f);
     if (!bound && a.stride < kWindowSamples && !a.spw) { set_error("wk_transcribe_windows: stride < 480000 requires samples_per_window"); return WK_ERR_AUDIO_PROCESSING_FAILED; }
     if (!bo->status)
         for (int64_t w = 0; w < n; ++w) if (status[w] != WK_OK) { set_error("%s", first_err.c_str()); return status[w]; }
@@ -519,6 +558,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
     }
     if (!sup_pool.empty()) WK_CUDA_CHECK(cudaMemcpyAsync(s->suppress_dev, sup_pool.data(), sup_pool.size() * 4, cudaMemcpyHostToDevice, s->stream));
+    if (any_detect) WK_CUDA_CHECK(cudaMemcpyAsync(s->lang_dev, lang_list.data(), lang_list.size() * 4, cudaMemcpyHostToDevice, s->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));   // sup_pool is pageable: the copy must land before it goes out of scope paths below reuse it
     s->align_on = any_words;
     if (any_words) WK_CHECK(ensure_align(s, n));
@@ -559,6 +599,20 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         R.has_first_thr = o.has_first_token_logprob_threshold; R.first_thr = o.first_token_logprob_threshold;
         R.seed = o.seed + (uint64_t)rung;
         R.suppress_off = sup_off[oi]; R.n_suppress = sup_n[oi];
+        // every rung detects again at its own temperature (detectLanguage runs inside decodeWithFallback's loop, TranscribeTask.swift:333-365)
+        R.lead_token = st->start_of_transcript_token;
+        R.lang_pos = -1;
+        if (detects(o)) {
+            R.detect = p[0] == st->start_of_transcript_token ? 1 : 2;
+            R.n_lang = (int32_t)lang_list.size();
+            // usePrefillPrompt: the prompt is rebuilt with the detected language - prefillDecoderInputs puts <|xx|> right after the first
+            // SOT (TextDecoder.swift:176-186); a prompt without a language token there only reports the language
+            if (o.use_prefill_prompt) {
+                const int32_t* sot = std::find(p, p + np, st->start_of_transcript_token);
+                const int i = (int)(sot - p) + 1;
+                if (i < np && std::binary_search(lang_sorted.begin(), lang_sorted.end(), p[i])) R.lang_pos = i;
+            }
+        }
         if (n_adm == 0) cudaEventSynchronize(s->ev_stage);   // the previous round's copies out of the pinned staging have landed
         for (int j = 0; j < beam; ++j) {                     // beam search: `beam` identical rows start the window
             s->h_adm_slots[n_adm] = slot * beam + j;
@@ -707,6 +761,10 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         WK_CUDA_CHECK(cudaMemcpyAsync(s->h_error, s->st.error, rows * 4, cudaMemcpyDeviceToHost, s->stream));
         WK_CUDA_CHECK(cudaMemcpyAsync(s->h_tokens, s->st.tokens, (size_t)rows * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
         WK_CUDA_CHECK(cudaMemcpyAsync(s->h_logprobs, s->st.logprobs, (size_t)rows * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
+        if (any_detect) {
+            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_token, s->st.lang_token, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_logprob, s->st.lang_logprob, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+        }
         if (beam > 1) {
             WK_CUDA_CHECK(cudaMemcpyAsync(s->h_sum_lp, s->bs.sum_lp, rows * 4, cudaMemcpyDeviceToHost, s->stream));
             WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_fin, s->bs.n_fin, Brun * 4, cudaMemcpyDeviceToHost, s->stream));
@@ -794,6 +852,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 continue;
             } else {
                 a.results[w] = r;
+                if (any_detect) { s->win_lang[w] = s->h_lang_token[r0]; s->win_lang_logprob[w] = s->h_lang_logprob[r0]; }   // the returned rung's
             }
             if (s->align_on && status[w] == WK_OK)
                 WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)q * kKvMaxLen * T * 2,
@@ -876,6 +935,9 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CHECK(dmalloc(&s->st.steps, S));
     WK_CHECK(dmalloc(&s->st.input_ids, S));
     WK_CHECK(dmalloc(&s->st.error, S));
+    WK_CHECK(dmalloc(&s->st.lang_token, S));
+    WK_CHECK(dmalloc(&s->st.lang_logprob, S));
+    WK_CHECK(dmalloc(&s->st.lang_state, S));
     WK_CHECK(dmalloc(&s->rp_dev, S));
     s->st.rp = s->rp_dev;
     WK_CHECK(dmalloc(&s->pos_dev, S));
@@ -902,6 +964,8 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CHECK(pinned((void**)&s->h_first_low, (size_t)S * 4));
     WK_CHECK(pinned((void**)&s->h_steps, (size_t)S * 4));
     WK_CHECK(pinned((void**)&s->h_error, (size_t)S * 4));
+    WK_CHECK(pinned((void**)&s->h_lang_token, (size_t)S * 4));
+    WK_CHECK(pinned((void**)&s->h_lang_logprob, (size_t)S * 4));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_enc, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_adm, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_stage, cudaEventDisableTiming));
@@ -925,11 +989,13 @@ void wk_session_free(wk_session* s) {
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     if (s->graph_exec_live) cudaGraphExecDestroy(s->graph_exec_live);
     void* ptrs[] = {s->cross_kv, s->cross_scale, s->self_k, s->self_v, s->partial, s->x, s->xn, s->attn, s->ffn, s->logits, s->st.tokens, s->st.n_tokens,
-                    s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error, s->rp_dev,
+                    s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error,
+                    s->st.lang_token, s->st.lang_logprob, s->st.lang_state, s->rp_dev,
                     s->pos_dev, s->lang_dev, s->suppress_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, s->align_scratch, s->align_w,
                     s->align_store, s->chain_counters};
     for (void* p : ptrs) if (p) cudaFree(p);
-    void* hptrs[] = {s->h_adm_slots, s->h_adm_prompts, s->h_adm_rp, s->h_tokens, s->h_logprobs, s->h_n_tokens, s->h_done, s->h_first_low, s->h_steps, s->h_error};
+    void* hptrs[] = {s->h_adm_slots, s->h_adm_prompts, s->h_adm_rp, s->h_tokens, s->h_logprobs, s->h_n_tokens, s->h_done, s->h_first_low, s->h_steps, s->h_error,
+                     s->h_lang_token, s->h_lang_logprob};
     for (void* p : hptrs) if (p) cudaFreeHost(p);
     enc_ws_free(&s->ws);
     cudaEventDestroy(s->ev_enc); cudaEventDestroy(s->ev_adm); cudaEventDestroy(s->ev_stage);
@@ -1088,6 +1154,16 @@ wk_status wk_transcribe_windows(wk_model* m, wk_session* s, const float* pcm_hos
 wk_status wk_session_stats(const wk_session* s, int64_t* out4) {
     if (!s || !out4) return WK_ERR_INVALID_ARGUMENT;
     memcpy(out4, s->stats, sizeof(s->stats));
+    return WK_OK;
+}
+
+wk_status wk_session_languages(const wk_session* s, int32_t first, int32_t n, int32_t* tokens, float* logprobs) {
+    if (!s || first < 0 || n < 0 || (int64_t)first + n > (int64_t)s->win_lang.size()) {
+        set_error("wk_session_languages: windows [%d, %d) outside the last call's %zu", first, first + n, s ? s->win_lang.size() : (size_t)0);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (tokens && n > 0) memcpy(tokens, s->win_lang.data() + first, (size_t)n * 4);
+    if (logprobs && n > 0) memcpy(logprobs, s->win_lang_logprob.data() + first, (size_t)n * 4);
     return WK_OK;
 }
 

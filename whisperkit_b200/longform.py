@@ -11,7 +11,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import check, wk_segment
-from .api import DecodingOptions, SpecialTokens
+from .api import DecodingOptions, SpecialTokens, language_code
 
 
 @dataclass
@@ -141,9 +141,11 @@ class VADAudioChunker:
 
 def transcribe_streams(kit, audioArrays: Sequence[np.ndarray], options: Optional[DecodingOptions] = None,
                        clipTimestamps: Sequence[float] = (), windowClipTime: float = 1.0, maxWindowSeek: Optional[int] = None,
-                       chunkingStrategy: Optional[str] = None, split_to_word_tokens=None, decode=None, hooks=None):
+                       chunkingStrategy: Optional[str] = None, split_to_word_tokens=None, decode=None, hooks=None,
+                       returnLanguages: bool = False):
     """TranscribeTask.run's seek loop for many audio arrays at once (TranscribeTask.swift:98-279; `chunkingStrategy="vad"`
-    = WhisperKit.swift:878-911).  Returns (segments per stream, number of 30 s windows decoded)."""
+    = WhisperKit.swift:878-911).  Returns (segments per stream, number of 30 s windows decoded); returnLanguages appends each stream's
+    (language token, log-prob) - the last window that detected one (DecodingOptions.detectLanguage), else (-1, 0.0)."""
     opts = kit.resolveLanguage(options or DecodingOptions())   # DecodingOptions.language -> <|xx|> through the tokenizer
     lib = kit.model.lib
     arrs = [np.ascontiguousarray(a, dtype=np.float32) for a in audioArrays]
@@ -181,9 +183,16 @@ def transcribe_streams(kit, audioArrays: Sequence[np.ndarray], options: Optional
                 segs[w.segment].words.append(WordTiming(w.word.decode("utf-8"), [int(w.tokens[k]) for k in range(w.n_tokens)], float(w.start),
                                                         float(w.end), float(w.probability), int(w.segment)))
         windows = lib.wk_transcription_window_count(h)
+        languages = []
+        for i in range(len(arrs)):
+            tok, lpv = C.c_int32(), C.c_float()
+            check(lib.wk_transcription_language(h, i, C.byref(tok), C.byref(lpv)))
+            languages.append((int(tok.value), float(lpv.value)))
     finally:
         lib.wk_transcription_free(h)
     per_stream = [[g for g in segs if g.stream == i] for i in range(len(arrs))]
+    if returnLanguages:
+        return per_stream, windows, languages
     return per_stream, windows
 
 
@@ -193,6 +202,8 @@ class TranscriptionResult:
     text: str
     segments: List[TranscriptionSegment]
     windows: int = 0
+    language: Optional[str] = None        # detected language code (detectLanguage + a tokenizer)
+    languageToken: Optional[int] = None   # detected <|xx|> id
 
 
 def transcribe_audio(kit, audioArrays: Sequence[np.ndarray], options: Optional[DecodingOptions] = None, tokenizer=None,
@@ -206,15 +217,18 @@ def transcribe_audio(kit, audioArrays: Sequence[np.ndarray], options: Optional[D
         raise _lib.WhisperError(-1, "wordTimestamps needs a tokenizer")
     native = tokenizer.hooks() if (tokenizer is not None and opts.wordTimestamps and hasattr(tokenizer, "hooks")) else None
     split = tokenizer.splitToWordTokens if (tokenizer is not None and opts.wordTimestamps and native is None) else None
-    per_stream, windows = transcribe_streams(kit, audioArrays, opts, clipTimestamps=clipTimestamps, chunkingStrategy=chunkingStrategy,
-                                             split_to_word_tokens=split, decode=tokenizer.decode if split is not None else None, hooks=native)
+    per_stream, windows, languages = transcribe_streams(kit, audioArrays, opts, clipTimestamps=clipTimestamps, chunkingStrategy=chunkingStrategy,
+                                                        split_to_word_tokens=split, decode=tokenizer.decode if split is not None else None,
+                                                        hooks=native, returnLanguages=True)
     sb = kit.specialTokens.specialTokenBegin
     out = []
-    for segs in per_stream:
+    for segs, (lang_tok, _) in zip(per_stream, languages):
         text = ""
         if tokenizer is not None:
             for g in segs:
                 g.text = tokenizer.decode([t for t in g.tokens if t < sb] if opts.skipSpecialTokens else g.tokens)
             text = tokenizer.decode([t for g in segs for t in g.tokens if t < sb]).strip(" \t               　")
-        out.append(TranscriptionResult(text, segs, windows))
+        detected = lang_tok >= 0
+        out.append(TranscriptionResult(text, segs, windows, language_code(tokenizer, lang_tok) if detected and tokenizer is not None else None,
+                                       lang_tok if detected else None))
     return out

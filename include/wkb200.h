@@ -137,6 +137,13 @@ typedef struct wk_decode_opts {
     int32_t detect_language;
     const int32_t* language_tokens;   /* tokenizer.allLanguageTokens: 1..4096 ids < vocab, one list for every detecting window of a call */
     int32_t n_language_tokens;
+    /* DecodingResult.noSpeechProb (the reference leaves it 0, TextDecoder.swift:802; semantics of openai/whisper decoding.py): the f32
+     * softmax over all vocab raw logits - no logits filter, no temperature - of the decode step whose input is the prompt's first
+     * <|startoftranscript|>, taken at no_speech_token.  Computed inside the batched decode loop at no extra step; read it with
+     * wk_session_no_speech_probs.  It replaces the 0 of the DecodingFallback silence rule (Models.swift:357-381) and, in
+     * wk_transcribe_streams, of findSeekPointAndSegments' skip rule and wk_segment.no_speech_prob.  A window whose loop ended before its
+     * SOT step has no value (0 is used).  A prompt without <|startoftranscript|> fails its window.  0 = off: a zeroed tail decodes as before. */
+    int32_t compute_no_speech_prob;
 } wk_decode_opts;
 
 /* Per-window DecodingResult (Models.swift:383-439) in flat arrays; tokens = SOT..EOT slice. */
@@ -237,6 +244,9 @@ wk_status wk_session_stats(const wk_session* s, int64_t* out4);
  * tokens[i] = the <|xx|> id from the rung whose result was returned, logprobs[i] = its log-prob (log-softmax over language_tokens at
  * temperature 0); -1 and 0 for a window that did not detect.  Either output may be NULL. */
 wk_status wk_session_languages(const wk_session* s, int32_t first, int32_t n, int32_t* tokens, float* logprobs);
+/* No-speech probability of windows [first, first + n) of the session's last batched call (wk_transcribe_windows(_ex),
+ * wk_decode_text(_ex); opts->compute_no_speech_prob), from the rung whose result was returned; NaN where it was not computed. */
+wk_status wk_session_no_speech_probs(const wk_session* s, int32_t first, int32_t n, float* out);
 /* Device logits of the last step, copied to host (debug / parity). */
 wk_status wk_session_last_logits(wk_session* s, float* logits_out);
 

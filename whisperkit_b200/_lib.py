@@ -66,6 +66,7 @@ class wk_decode_opts(C.Structure):
         ("word_timestamps", C.c_int32),
         ("beam_size", C.c_int32), ("beam_patience", C.c_float),
         ("detect_language", C.c_int32), ("language_tokens", C.POINTER(C.c_int32)), ("n_language_tokens", C.c_int32),
+        ("compute_no_speech_prob", C.c_int32),
     ]
 
 
@@ -146,6 +147,7 @@ SYMBOLS = [
     ("wk_session_last_logits", I32, [P, P]),
     ("wk_session_stats", I32, [P, PI64]),
     ("wk_session_languages", I32, [P, I32, I32, PI32, PF32]),
+    ("wk_session_no_speech_probs", I32, [P, I32, I32, PF32]),
     ("wk_decode_text_ex", I32, [P, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts), C.POINTER(wk_decode_result)]),
     ("wk_transcribe_windows_ex", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts),
                                        C.POINTER(wk_decode_result)]),

@@ -15,6 +15,7 @@ All arithmetic happens in libwkb200.so (sm_90a kernels); this module only marsha
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
@@ -111,6 +112,9 @@ class DecodingOptions:
     # reference resolves it (Configurations.swift:222)
     detectLanguage: Optional[bool] = None
     allLanguageTokens: Optional[List[int]] = None   # tokenizer.allLanguageTokens; WhisperKit.resolveLanguage fills it
+    # compute DecodingResult.noSpeechProb in the decode loop (openai/whisper's rule; the reference leaves it 0), so that noSpeechThreshold
+    # marks silent windows (fallback reason "silence") and the long-form loop skips them
+    computeNoSpeechProb: bool = False
 
     @property
     def detectsLanguage(self) -> bool:
@@ -159,6 +163,7 @@ class DecodingOptions:
         o.detect_language = int(self.detectsLanguage)
         lt, nlt = arr(self.allLanguageTokens)
         o.language_tokens, o.n_language_tokens = lt, max(nlt, 0)
+        o.compute_no_speech_prob = int(self.computeNoSpeechProb)
         return o, keep
 
 
@@ -184,6 +189,7 @@ class DecodingResult:
     languageToken: Optional[int] = None
     languageLogProb: Optional[float] = None
     language: Optional[str] = None
+    noSpeechProb: float = 0.0   # DecodingOptions.computeNoSpeechProb; 0 where it was not computed, as in the reference
 
     @staticmethod
     def from_c(r: wk_decode_result) -> "DecodingResult":
@@ -208,6 +214,19 @@ def session_languages(lib, session, n: int):
     lp = (C.c_float * max(1, n))()
     check(lib.wk_session_languages(session, 0, n, tok, lp))
     return [int(v) for v in tok[:n]], [float(v) for v in lp[:n]]
+
+
+def session_no_speech_probs(lib, session, n: int) -> List[float]:
+    """wk_session_no_speech_probs for windows [0, n) of the session's last batched call; NaN = not computed."""
+    out = (C.c_float * max(1, n))()
+    check(lib.wk_session_no_speech_probs(session, 0, n, out))
+    return [float(v) for v in out[:n]]
+
+
+def attach_no_speech_probs(results: List["DecodingResult"], probs: Sequence[float]) -> None:
+    for r, p in zip(results, probs):
+        if isinstance(r, DecodingResult):
+            r.noSpeechProb = 0.0 if math.isnan(p) else p
 
 
 def attach_languages(results: List["DecodingResult"], tokens: Sequence[int], logprobs: Sequence[float], tokenizer=None) -> None:
@@ -491,6 +510,7 @@ class TextDecoder:
         check(self.lib.wk_decode_text_ex(self.handle, C.byref(st), C.byref(bo), res))
         out = [DecodingResult.from_c(r) for r in res]
         attach_languages(out, *session_languages(self.lib, self.handle, n))
+        attach_no_speech_probs(out, session_no_speech_probs(self.lib, self.handle, n))
         return out
 
     def detectLanguage(self, encoderOutput: Optional[DeviceTensor], specialTokens: SpecialTokens, allLanguageTokens: Sequence[int],
@@ -720,4 +740,5 @@ class WhisperKit:
             else:
                 out.append(DecodingResult.from_c(r))
         attach_languages(out, *session_languages(self.model.lib, self.textDecoder.handle, n), tokenizer=self.tokenizer)
+        attach_no_speech_probs(out, session_no_speech_probs(self.model.lib, self.textDecoder.handle, n))
         return out

@@ -63,6 +63,7 @@ __global__ void decode_slots_init_kernel(DecodeState st, RowParams* __restrict__
         st.lang_token[b] = -1;
         st.lang_logprob[b] = 0.f;
         st.lang_state[b] = R.detect == 2 ? kLangLead : 0;
+        st.no_speech[b] = __int_as_float(0x7fc00000);   // NaN: not computed (yet)
         if (bs.beam > 1) {
             bs.sum_lp[b] = 0.f;
             if (b % bs.beam == 0) bs.n_fin[b / bs.beam] = 0;
@@ -834,7 +835,7 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         R.prompt_len = -1; R.sample_begin_ts = p.sample_begin_ts; R.sample_begin_blank = p.sample_begin_blank; R.max_steps = 0;
         R.temperature = p.temperature; R.top_k = p.top_k; R.has_first_thr = 0; R.first_thr = 0.f; R.seed = p.seed;
         R.suppress_off = 0; R.n_suppress = p.n_suppress;
-        R.detect = 0; R.lang_pos = -1; R.n_lang = 0; R.lead_token = 0;
+        R.detect = 0; R.lang_pos = -1; R.n_lang = 0; R.lead_token = 0; R.no_speech_pos = -1;
     }
     const int32_t* toks = loop_mode ? st.tokens + b * kMaxCtx : tokens_in + (long long)b * ld_tokens;
     const wk_special_tokens& S = p.st;
@@ -875,6 +876,22 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
             __syncthreads();
             // the leading step ends here: no sample, no bookkeeping - the row starts its step 0 next
             if (lead) return;
+        }
+    }
+    if (loop_mode && R.no_speech_pos == st.steps[b] && st.lang_state[b] != kLangLead) {
+        // DecodingResult.noSpeechProb (openai/whisper decoding.py): the softmax of the RAW logits of the step whose input is the prompt's
+        // SOT - before any logits filter, at no temperature - taken at <|nospeech|>.  Fixed-order block reductions: deterministic.
+        // expf, not __expf: the value is compared against a threshold and reported.
+        const float* row = logits + (long long)b * ld_logits;
+        float mx = -INFINITY;
+        for (int i = tid; i < V; i += kSamplerThreads) mx = fmaxf(mx, row[i]);
+        mx = block_max(mx, scratch);
+        float sm = 0.f;
+        for (int i = tid; i < V; i += kSamplerThreads) sm += expf(row[i] - mx);
+        sm = block_sum(sm, scratch);
+        if (tid == 0) {
+            const int ns = S.no_speech_token;
+            st.no_speech[b] = (ns >= 0 && ns < V) ? expf(row[ns] - mx) / sm : __int_as_float(0x7fc00000);
         }
     }
     const int n_tok = loop_mode ? st.n_tokens[b] : n_tokens_in[b];

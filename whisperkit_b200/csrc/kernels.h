@@ -112,6 +112,8 @@ struct RowParams {
     int32_t lang_pos;            // prompt slot of <|xx|> rewritten with the detected language, <0 = report only
     int32_t n_lang;              // entries of SamplerParams.detect_tokens
     int32_t lead_token;          // <|startoftranscript|>: what the leading detection step feeds at position 0
+    // DecodingResult.noSpeechProb: the step (= index of the prompt's first SOT) whose raw logits give it, <0 = off
+    int32_t no_speech_pos;
 };
 
 struct DecodeState {
@@ -129,6 +131,7 @@ struct DecodeState {
     int32_t* lang_token;  // [Bmax] language detected in the loop, -1 = none
     float* lang_logprob;  // [Bmax]
     int32_t* lang_state;  // [Bmax] kLangLead: the leading detection step is next; kLangLeadRan: it was this step's; 0 otherwise
+    float* no_speech;     // [Bmax] softmax(raw logits)[no_speech_token] at step RowParams.no_speech_pos; NaN = not computed
 };
 constexpr int kLangLead = 2, kLangLeadRan = 3;
 

@@ -405,6 +405,13 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
                 if (lt[k] >= 0 && at >= T->lang_at[u.stream]) { T->lang[u.stream] = lt[k]; T->lang_logprob[u.stream] = ll[k]; T->lang_at[u.stream] = at; }
             }
         }
+        // noSpeechProb per window for findSeekPointAndSegments' skip rule and the segments (0 where it was not computed, as before)
+        std::vector<float> nsp(active.size(), 0.f);
+        if (o->compute_no_speech_prob) {
+            rc = wk_session_no_speech_probs(s, 0, (int32_t)active.size(), nsp.data());
+            if (rc != WK_OK) { delete T; return rc; }
+            for (float& v : nsp) if (isnan(v)) v = 0.f;
+        }
         const int cols = info.n_audio_ctx;
         if (o->word_timestamps) {   // every window's alignment rows back in one burst (Float16, as the reference's alignmentWeights)
             for (size_t k = 0; k < active.size(); ++k) {
@@ -421,7 +428,7 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
             wk_segment segs[128];
             int nseg = 0;
             int64_t new_seek = u.seek;
-            rc2 = wk_find_seek_point_and_segments(r.tokens, r.token_logprobs, r.n_tokens, 0.f, r.avg_logprob, r.compression_ratio, r.temperature, o,
+            rc2 = wk_find_seek_point_and_segments(r.tokens, r.token_logprobs, r.n_tokens, nsp[k], r.avg_logprob, r.compression_ratio, r.temperature, o,
                                                   (int32_t)u.segs.size(), u.seek, seg_size[k], kSampleRate, st->time_token_begin, &new_seek, segs, 128, &nseg);
             if (rc2 != WK_OK) return rc2;
             const int64_t prev = u.seek;

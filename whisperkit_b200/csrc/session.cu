@@ -53,9 +53,10 @@ struct wk_session {
     // pinned readback of the decode state
     int32_t *h_tokens = nullptr, *h_n_tokens = nullptr, *h_done = nullptr, *h_first_low = nullptr, *h_steps = nullptr, *h_error = nullptr;
     float* h_logprobs = nullptr;
-    int32_t* h_lang_token = nullptr; float* h_lang_logprob = nullptr;
+    int32_t* h_lang_token = nullptr; float* h_lang_logprob = nullptr; float* h_no_speech = nullptr;
     // language detected per window of the last batched call (wk_session_languages): -1 / 0 where a window did not detect
     std::vector<int32_t> win_lang; std::vector<float> win_lang_logprob;
+    std::vector<float> win_no_speech;   // noSpeechProb per window of the last batched call (wk_session_no_speech_probs), NaN = none
     // step graph, cached across calls: the step depends on the call only through the rows it covers, the alignment export and the
     // special-token ids baked into the sampler's parameters
     cudaGraphExec_t graph_exec = nullptr, graph_exec_live = nullptr;   // the step with / without the ended-row checks in the attention kernels
@@ -253,7 +254,7 @@ static float compression_ratio(const std::vector<int32_t>& toks) {
 
 // finalisation of one window on the host: finalize + slicing + averages (TextDecoder.swift:776-853)
 static void finalize_result(wk_decode_result& r, const int32_t* tokens, const float* lps, int n_tok, int steps, int first_low,
-                            const wk_special_tokens* st, const wk_decode_opts* o, float temperature) {
+                            const wk_special_tokens* st, const wk_decode_opts* o, float temperature, float no_speech_prob) {
     memset(&r, 0, sizeof(r));
     std::vector<int32_t> seg(tokens, tokens + n_tok);
     std::vector<float> slp(lps, lps + n_tok);
@@ -279,10 +280,11 @@ static void finalize_result(wk_decode_result& r, const int32_t* tokens, const fl
     r.avg_logprob = sum / (float)r.n_tokens;
     r.compression_ratio = compression_ratio(words);
     r.temperature = roundf(temperature * 1000.f) / 1000.f;
-    // DecodingFallback (Models.swift:357-381); noSpeechProb is always 0 in the reference (TextDecoder.swift:802)
+    // DecodingFallback (Models.swift:357-381); noSpeechProb is 0 unless the window computes it (the reference's is always 0,
+    // TextDecoder.swift:802)
     r.needs_fallback = 0; r.fallback_reason = 0;
     if (first_low) { r.needs_fallback = 1; r.fallback_reason = 1; }
-    else if (o->has_no_speech_threshold && 0.f > o->no_speech_threshold) { r.needs_fallback = 0; r.fallback_reason = 2; }
+    else if (o->has_no_speech_threshold && no_speech_prob > o->no_speech_threshold) { r.needs_fallback = 0; r.fallback_reason = 2; }
     else if (o->has_compression_ratio_threshold && r.compression_ratio > o->compression_ratio_threshold) { r.needs_fallback = 1; r.fallback_reason = 3; }
     else if (o->has_logprob_threshold && r.avg_logprob < o->logprob_threshold) { r.needs_fallback = 1; r.fallback_reason = 4; }
 }
@@ -546,6 +548,25 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     std::sort(lang_sorted.begin(), lang_sorted.end());
     s->win_lang.assign((size_t)n, -1);
     s->win_lang_logprob.assign((size_t)n, 0.f);
+    // ---- noSpeechProb (compute_no_speech_prob): the value comes from the step that feeds the prompt's first SOT, so that SOT must exist
+    auto sot_index = [&](int64_t w) -> int {
+        const int32_t* p; int np;
+        prompt_of(w, &p, &np);
+        const int32_t* sot = std::find(p, p + np, st->start_of_transcript_token);
+        return sot == p + np ? -1 : (int)(sot - p);
+    };
+    bool any_nsp = false;
+    for (int64_t w = 0; w < n; ++w) {
+        if (status[w] != WK_OK || !opts_of(bo, w).compute_no_speech_prob) continue;
+        if (sot_index(w) < 0) {
+            set_error("window %lld: computeNoSpeechProb needs <|startoftranscript|> (token %d) in the prompt, which has none", (long long)w,
+                      st->start_of_transcript_token);
+            fail_window(w, WK_ERR_PREPARE_DECODER_INPUTS);
+            continue;
+        }
+        any_nsp = true;
+    }
+    s->win_no_speech.assign((size_t)n, NAN);
     if (!bound && a.stride < kWindowSamples && !a.spw) { set_error("wk_transcribe_windows: stride < 480000 requires samples_per_window"); return WK_ERR_AUDIO_PROCESSING_FAILED; }
     if (!bo->status)
         for (int64_t w = 0; w < n; ++w) if (status[w] != WK_OK) { set_error("%s", first_err.c_str()); return status[w]; }
@@ -602,6 +623,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         // every rung detects again at its own temperature (detectLanguage runs inside decodeWithFallback's loop, TranscribeTask.swift:333-365)
         R.lead_token = st->start_of_transcript_token;
         R.lang_pos = -1;
+        R.no_speech_pos = o.compute_no_speech_prob ? sot_index(w) : -1;   // the same step at every rung
         if (detects(o)) {
             R.detect = p[0] == st->start_of_transcript_token ? 1 : 2;
             R.n_lang = (int32_t)lang_list.size();
@@ -765,6 +787,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_token, s->st.lang_token, rows * 4, cudaMemcpyDeviceToHost, s->stream));
             WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_logprob, s->st.lang_logprob, rows * 4, cudaMemcpyDeviceToHost, s->stream));
         }
+        if (any_nsp) WK_CUDA_CHECK(cudaMemcpyAsync(s->h_no_speech, s->st.no_speech, rows * 4, cudaMemcpyDeviceToHost, s->stream));
         if (beam > 1) {
             WK_CUDA_CHECK(cudaMemcpyAsync(s->h_sum_lp, s->bs.sum_lp, rows * 4, cudaMemcpyDeviceToHost, s->stream));
             WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_fin, s->bs.n_fin, Brun * 4, cudaMemcpyDeviceToHost, s->stream));
@@ -841,7 +864,10 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 btok.assign(cd.tok, cd.tok + body); blp.assign(cd.lp, cd.lp + body);
                 seq_tok = btok.data(); seq_lp = blp.data(); seq_n = body;
             }
-            finalize_result(r, seq_tok, seq_lp, seq_n, s->h_steps[r0], s->h_first_low[r0], st, &o, rung_temperature(o, rung));
+            // beam search: every beam of the window is the same forced copy through the prefill, so row r0 holds the value
+            const float nsp = o.compute_no_speech_prob ? s->h_no_speech[r0] : NAN;
+            finalize_result(r, seq_tok, seq_lp, seq_n, s->h_steps[r0], s->h_first_low[r0], st, &o, rung_temperature(o, rung),
+                            isnan(nsp) ? 0.f : nsp);
             if (s->h_error[r0]) {
                 set_error("window %d: no finite logit at decoder step %d", w, s->h_steps[r0] - 1);
                 fail_window(w, WK_ERR_DECODING_LOGITS_FAILED);
@@ -853,6 +879,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             } else {
                 a.results[w] = r;
                 if (any_detect) { s->win_lang[w] = s->h_lang_token[r0]; s->win_lang_logprob[w] = s->h_lang_logprob[r0]; }   // the returned rung's
+                s->win_no_speech[w] = nsp;
             }
             if (s->align_on && status[w] == WK_OK)
                 WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)q * kKvMaxLen * T * 2,
@@ -938,6 +965,7 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CHECK(dmalloc(&s->st.lang_token, S));
     WK_CHECK(dmalloc(&s->st.lang_logprob, S));
     WK_CHECK(dmalloc(&s->st.lang_state, S));
+    WK_CHECK(dmalloc(&s->st.no_speech, S));
     WK_CHECK(dmalloc(&s->rp_dev, S));
     s->st.rp = s->rp_dev;
     WK_CHECK(dmalloc(&s->pos_dev, S));
@@ -966,6 +994,7 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CHECK(pinned((void**)&s->h_error, (size_t)S * 4));
     WK_CHECK(pinned((void**)&s->h_lang_token, (size_t)S * 4));
     WK_CHECK(pinned((void**)&s->h_lang_logprob, (size_t)S * 4));
+    WK_CHECK(pinned((void**)&s->h_no_speech, (size_t)S * 4));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_enc, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_adm, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_stage, cudaEventDisableTiming));
@@ -990,12 +1019,12 @@ void wk_session_free(wk_session* s) {
     if (s->graph_exec_live) cudaGraphExecDestroy(s->graph_exec_live);
     void* ptrs[] = {s->cross_kv, s->cross_scale, s->self_k, s->self_v, s->partial, s->x, s->xn, s->attn, s->ffn, s->logits, s->st.tokens, s->st.n_tokens,
                     s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error,
-                    s->st.lang_token, s->st.lang_logprob, s->st.lang_state, s->rp_dev,
+                    s->st.lang_token, s->st.lang_logprob, s->st.lang_state, s->st.no_speech, s->rp_dev,
                     s->pos_dev, s->lang_dev, s->suppress_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, s->align_scratch, s->align_w,
                     s->align_store, s->chain_counters};
     for (void* p : ptrs) if (p) cudaFree(p);
     void* hptrs[] = {s->h_adm_slots, s->h_adm_prompts, s->h_adm_rp, s->h_tokens, s->h_logprobs, s->h_n_tokens, s->h_done, s->h_first_low, s->h_steps, s->h_error,
-                     s->h_lang_token, s->h_lang_logprob};
+                     s->h_lang_token, s->h_lang_logprob, s->h_no_speech};
     for (void* p : hptrs) if (p) cudaFreeHost(p);
     enc_ws_free(&s->ws);
     cudaEventDestroy(s->ev_enc); cudaEventDestroy(s->ev_adm); cudaEventDestroy(s->ev_stage);
@@ -1164,6 +1193,15 @@ wk_status wk_session_languages(const wk_session* s, int32_t first, int32_t n, in
     }
     if (tokens && n > 0) memcpy(tokens, s->win_lang.data() + first, (size_t)n * 4);
     if (logprobs && n > 0) memcpy(logprobs, s->win_lang_logprob.data() + first, (size_t)n * 4);
+    return WK_OK;
+}
+
+wk_status wk_session_no_speech_probs(const wk_session* s, int32_t first, int32_t n, float* out) {
+    if (!s || !out || first < 0 || n < 0 || (int64_t)first + n > (int64_t)s->win_no_speech.size()) {
+        set_error("wk_session_no_speech_probs: windows [%d, %d) outside the last call's %zu", first, first + n, s ? s->win_no_speech.size() : (size_t)0);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (n > 0) memcpy(out, s->win_no_speech.data() + first, (size_t)n * 4);
     return WK_OK;
 }
 

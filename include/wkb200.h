@@ -487,6 +487,25 @@ wk_status wk_test_cross_attention_fp8(wk_model* m, const float* q, const uint8_t
  * row pos[b] is appended), pos [B] device -> out [B][H*64] 16-bit. */
 wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, void* vcache, const int32_t* pos, void* out, int32_t B,
                                  int32_t H, int32_t dtype, const int32_t* done);
+/* The decoder's swap-AB split-K GEMM alone, configured as the decode step configures it: W [N,K], x [rows_x,K] 16-bit (rows_x = the padded
+ * batch Bp, a multiple of 16 <= 256) -> raw partials [splits][partial_cols][N] f32, written into the caller's buffer and nowhere else.
+ * partial_cols = rows_x is the layer GEMM's form, partial_cols = B < rows_x (splits 1) the logits GEMM's. */
+wk_status wk_test_gemm_partial(wk_model* m, const void* w, const void* x, float* partial_out, int32_t N, int32_t rows_x, int32_t partial_cols,
+                               int32_t K, int32_t dtype, int32_t splits);
+/* The split-K consumers on partials [splits][Bp][n] f32 (rows >= B are never read): kind 0 reduce + bias (may be NULL) + residual x [B][n]
+ * f32 (in place) + LayerNorm -> out16 [B][n]; kind 1 reduce + bias + exact GELU -> out16 [B][n]. */
+wk_status wk_test_decoder_reduce(wk_model* m, int32_t kind, const float* partial, int32_t splits, int32_t Bp, const float* bias, const float* gamma,
+                                 const float* beta, float* x, void* out16, int32_t B, int32_t n, int32_t dtype);
+/* Decoder self-attention on q|k|v split-K partials [splits][Bp][3*H*64] with biases bq / bv [H*64]; caches [B][H][224][64]; anc [B][224]
+ * (may be NULL) names the cache row holding position t of row b (beam search).  The new K/V row goes to row b's own cache. */
+wk_status wk_test_self_attention_splitk(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bq, const float* bv, void* kcache,
+                                        void* vcache, const int32_t* pos, const int32_t* done, const int32_t* anc, void* out, int32_t B, int32_t H,
+                                        int32_t dtype);
+/* Decoder cross-attention on q split-K partials [splits][Bp][H*64] with bias bq; K/V [B / kv_div][H][T][64] 16-bit, or E4M3 codes with row
+ * scales [B / kv_div][H][T] when kscale / vscale are non-NULL; kv_div = 1 runs the single-query kernel, 2..8 the beam kernel. */
+wk_status wk_test_cross_attention_splitk(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bq, const void* kcross,
+                                         const void* vcross, const float* kscale, const float* vscale, void* out, int32_t B, int32_t H, int32_t T,
+                                         int32_t dtype, const int32_t* done, int32_t kv_div);
 
 /* Average device time (ms) of one launch of a named hot kernel on the live buffers, plus its algorithmic work
  * (bytes for HBM-bound kernels, FLOPs for tensor-bound ones): 0 decoder cross-attention, 1 encoder FC1 GEMM,

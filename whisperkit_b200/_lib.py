@@ -221,6 +221,10 @@ SYMBOLS = [
     ("wk_test_gemm_residual", I32, [P, P, P, P, P, I32, I32, I32, I32]),
     ("wk_test_gemm_splitk", I32, [P, P, P, P, I32, I32, I32, I32, I32]),
     ("wk_test_attention", I32, [P, P, P, I32, I32, I32, I32]),
+    ("wk_test_gemm_partial", I32, [P, P, P, P, I32, I32, I32, I32, I32, I32]),
+    ("wk_test_decoder_reduce", I32, [P, I32, P, I32, I32, P, P, P, P, P, I32, I32, I32]),
+    ("wk_test_self_attention_splitk", I32, [P, P, I32, I32, P, P, P, P, P, P, P, P, I32, I32, I32]),
+    ("wk_test_cross_attention_splitk", I32, [P, P, I32, I32, P, P, P, P, P, P, I32, I32, I32, I32, P, I32]),
     ("wk_debug_read", I32, [P, P, I32, I64, P, I64]),
     ("wk_bench_kernel", I32, [P, P, I32, I32, I32, PF32, C.POINTER(C.c_double)]),
 ]

@@ -1094,4 +1094,82 @@ wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, vo
     return r;
 }
 
+// The swap-AB split-K GEMM configured as dec_gemm (partial_cols = rows_x) or the logits GEMM (partial_cols = B < rows_x, splits = 1) configure
+// it, its raw partials [splits][partial_cols][N] f32 written to the caller's buffer
+wk_status wk_test_gemm_partial(wk_model* m, const void* w, const void* x, float* partial_out, int32_t N, int32_t rows_x, int32_t partial_cols,
+                               int32_t K, int32_t dtype, int32_t splits) {
+    if (!m || !w || !x || !partial_out || N < 1 || rows_x < 16 || rows_x > 256 || rows_x % 16 != 0 || partial_cols < 1 || partial_cols > rows_x ||
+        splits < 1) {
+        set_error("wk_test_gemm_partial: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    GemmDesc g;
+    memset(&g, 0, sizeof(g));
+    g.a = w; g.a_rows = N; g.a_cols = K; g.a_ld = K; g.a_batches = 1;
+    g.b = x; g.b_rows = rows_x; g.b_ld = K; g.in_dtype = dtype;
+    g.m_rows_per_batch = N; g.n = rows_x; g.k = K; g.taps = 1; g.bn = rows_x; g.splits = splits;
+    g.mode = GEMM_OUT_PARTIAL_T; g.out = partial_out; g.ld_out = N; g.out_rows_per_batch = N; g.partial_cols = partial_cols;
+    g.pdl = 1; g.a_static = 1;
+    wk_status r = gemm_wgmma(g, m->num_sms, m->stream);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_gemm_partial: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+// The split-K consumers of the FC / out-projection GEMMs on caller-made partials [splits][Bp][n]: kind 0 decoder_reduce_resid_ln (x [B][n]
+// f32 updated in place, out16 = LN(x)), kind 1 decoder_reduce_bias_gelu (out16 = gelu(bias + sum), x / gamma / beta unused)
+wk_status wk_test_decoder_reduce(wk_model* m, int32_t kind, const float* partial, int32_t splits, int32_t Bp, const float* bias, const float* gamma,
+                                 const float* beta, float* x, void* out16, int32_t B, int32_t n, int32_t dtype) {
+    if (!m || !partial || !out16 || B < 1 || Bp < B || splits < 1 || n < 4 || n % 4 != 0 || (kind == 0 && (!gamma || !beta || !x)) ||
+        (kind == 1 && !bias) || kind < 0 || kind > 1) {
+        set_error("wk_test_decoder_reduce: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    wk_status r = kind == 0 ? decoder_reduce_resid_ln(partial, splits, Bp, bias, gamma, beta, x, out16, B, n, dtype, m->stream)
+                            : decoder_reduce_bias_gelu(partial, splits, Bp, bias, out16, B, n, dtype, m->stream);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_decoder_reduce: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+// decoder_self_attention_kernel as the decode step runs it: q|k|v split-K partials [splits][Bp][3*H*64] plus the q / v biases, beam cache
+// ancestry anc [B][224] (may be NULL: every row reads its own cache row)
+wk_status wk_test_self_attention_splitk(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bq, const float* bv, void* kcache,
+                                        void* vcache, const int32_t* pos, const int32_t* done, const int32_t* anc, void* out, int32_t B, int32_t H,
+                                        int32_t dtype) {
+    if (!m || !partial || !bq || !bv || !kcache || !vcache || !pos || !out || B < 1 || Bp < B || splits < 1 || H < 1) {
+        set_error("wk_test_self_attention_splitk: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    wk_status r = decoder_self_attention(partial, splits, Bp, bq, bv, kcache, vcache, pos, done, out, B, H, kKvMaxLen, dtype, m->stream, anc);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_self_attention_splitk: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+// decoder cross-attention as the decode step runs it: q split-K partials [splits][Bp][H*64] plus bq; K/V [B / kv_div][H][T][64] 16-bit, or
+// E4M3 codes with row scales [B / kv_div][H][T] when kscale / vscale are given (kv_div = 1: the single-query kernel, 2..8: the beam kernel)
+wk_status wk_test_cross_attention_splitk(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bq, const void* kcross,
+                                         const void* vcross, const float* kscale, const float* vscale, void* out, int32_t B, int32_t H, int32_t T,
+                                         int32_t dtype, const int32_t* done, int32_t kv_div) {
+    if (!m || !partial || !bq || !kcross || !vcross || !out || B < 1 || Bp < B || splits < 1 || H < 1 || H > 32 || kv_div < 1 || kv_div > 8 ||
+        (kscale == nullptr) != (vscale == nullptr)) {
+        set_error("wk_test_cross_attention_splitk: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    wk_status r = decoder_cross_attention(partial, splits, Bp, bq, kcross, vcross, out, B, H, T, dtype, m->stream, done, nullptr, 0u, kv_div,
+                                          kscale, vscale);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention_splitk: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
 }  // extern "C"

@@ -372,6 +372,26 @@ wk_status wk_session_alignment_weights(wk_session* s, int32_t window, int32_t ro
  * to be truly asynchronous); sync != 0 waits for it and for every copy queued before it. */
 wk_status wk_session_alignment_weights_f16(wk_session* s, int32_t window, int32_t rows, uint16_t* out, int32_t sync);
 
+/* ---- forced alignment of given token sequences (openai-whisper timing.py find_alignment) ----
+ * One teacher-forced decoder pass over every position of every sequence: word timings for any transcript (edited text, subtitles, another
+ * system's output, beam-search results) and the model's per-token log-probs of it.  Sequence w is tokens[offsets[w] .. offsets[w + 1]): the
+ * full decoder input as the decode loop consumes it - prompt, text, EOT (DecodingResult.tokens can be passed back unchanged).  It must hold
+ * 1..224 ids below the vocabulary size; a sequence that does not fails its own window (status[w]; status may be NULL, then the first
+ * failure fails the call), the other windows still run.  Outputs stay in the session until its next call:
+ *   wk_session_alignment_weights(_f16)  rows 0..n of window w: row t + 1 = the alignment heads' mean cross-attention row at input
+ *                                        position t (Float16), row 0 = 0 - the decode loop's layout, ready for wk_find_alignment /
+ *                                        wk_add_word_timestamps
+ *   wk_session_aligned_logprobs          n values: [t] = log softmax(logits[t - 1][:end_token])[tokens[t]] for t >= 1 (raw logits, no
+ *                                        filters, temperature 1), NaN at t = 0 and where tokens[t] >= end_token
+ * Results do not depend on the other windows of the call. */
+/* against the encoder output bound with wk_session_set_encoder_output (n_windows <= bound windows; window w = bound window w) */
+wk_status wk_align_tokens(wk_session* s, const wk_special_tokens* st, const int32_t* tokens, const int32_t* offsets, int64_t n_windows,
+                          int32_t* status);
+/* from PCM, as wk_transcribe_windows takes it (mel, encoder and cross K/V per chunk of the session's slots) */
+wk_status wk_align_windows(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride, const int32_t* samples_per_window,
+                           const wk_special_tokens* st, const int32_t* tokens, const int32_t* offsets, int32_t* status);
+wk_status wk_session_aligned_logprobs(const wk_session* s, int32_t window, int32_t n, float* out);
+
 struct wk_word {                   /* WordTiming (Models.swift:617-633) */
     const char* word;              /* UTF-8, NUL-terminated */
     const int32_t* tokens; int32_t n_tokens;

@@ -183,6 +183,9 @@ SYMBOLS = [
     ("wk_model_set_alignment_heads", I32, [P, PI32, I32]),
     ("wk_session_alignment_weights", I32, [P, I32, I32, P]),
     ("wk_session_alignment_weights_f16", I32, [P, I32, I32, P, I32]),
+    ("wk_align_tokens", I32, [P, C.POINTER(wk_special_tokens), P, P, I64, PI32]),
+    ("wk_align_windows", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), P, P, PI32]),
+    ("wk_session_aligned_logprobs", I32, [P, I32, I32, P]),
     ("wk_words_count", I32, [P]),
     ("wk_words_get", I32, [P, I32, C.POINTER(wk_word)]),
     ("wk_words_free", None, [P]),

@@ -531,6 +531,27 @@ class TextDecoder:
         check(self.lib.wk_session_alignment_weights(self.handle, window, rows, _ptr(out)))
         return out
 
+    def alignTokens(self, encoderOutput: Optional[DeviceTensor], tokenLists: Sequence[Sequence[int]], specialTokens: SpecialTokens,
+                    returnErrors: bool = False):
+        """Forced alignment of one token sequence per bound window (openai-whisper's find_alignment pass): each sequence is the full decoder
+        input - prompt, text, EOT, e.g. DecodingResult.tokens.  Returns per window (alignmentWeights [n+1, 1500] f32, tokenLogProbs [n] f32),
+        the weights in the decode loop's layout for WordTimingSeeker.findAlignment / addWordTimestamps.  With returnErrors a window whose
+        sequence is invalid yields its WhisperError instead of failing the call."""
+        if encoderOutput is not None:
+            self.bindEncoderOutput(encoderOutput)
+        st = specialTokens.to_c()
+        flat, offsets = _flatten_token_lists(tokenLists)
+        n = len(tokenLists)
+        status = (C.c_int32 * n)()
+        check(self.lib.wk_align_tokens(self.handle, C.byref(st), _ptr(flat), _ptr(offsets), n, status))
+        return aligned_results(self.lib, self.handle, tokenLists, status, returnErrors, self.model.info.n_audio_ctx)
+
+    def alignedLogProbs(self, window: int, n: int) -> np.ndarray:
+        """tokenLogProbs of one window of the last alignTokens / WhisperKit.align call."""
+        out = np.empty(n, dtype=np.float32)
+        check(self.lib.wk_session_aligned_logprobs(self.handle, window, n, _ptr(out)))
+        return out
+
     def stats(self) -> dict:
         """Scheduler counters of the last batched call (decode steps launched, live-row steps, admissions, ladder re-admissions)."""
         a = (C.c_int64 * 4)()
@@ -552,6 +573,37 @@ class TextDecoder:
             self.close()
         except Exception:
             pass
+
+
+def _flatten_token_lists(tokenLists: Sequence[Sequence[int]]):
+    """Token sequences -> (flat int32 array, int32 offsets of n + 1 entries), the layout of wk_align_tokens / wk_align_windows."""
+    lens = [len(t) for t in tokenLists]
+    offsets = np.zeros(len(lens) + 1, dtype=np.int32)
+    offsets[1:] = np.cumsum(lens)
+    flat = np.zeros(max(1, int(offsets[-1])), dtype=np.int32)
+    for i, t in enumerate(tokenLists):
+        flat[offsets[i]:offsets[i + 1]] = np.asarray(list(t), dtype=np.int64)
+    return flat, offsets
+
+
+def aligned_results(lib, session, tokenLists, status, returnErrors: bool, n_audio_ctx: int):
+    """Per-window (alignmentWeights [n+1, T], tokenLogProbs [n]) of the session's last align call; failed windows raise (or, with returnErrors,
+    yield their WhisperError)."""
+    out = []
+    for i, t in enumerate(tokenLists):
+        if status[i] != 0:
+            err = WhisperError(int(status[i]), f"window {i}: " + lib.wk_last_error().decode("utf-8", "replace"))
+            if not returnErrors:
+                raise err
+            out.append(err)
+            continue
+        n = len(t)
+        w = np.empty((n + 1, n_audio_ctx), dtype=np.float32)
+        check(lib.wk_session_alignment_weights(session, i, n + 1, _ptr(w)))
+        lp = np.empty(n, dtype=np.float32)
+        check(lib.wk_session_aligned_logprobs(session, i, n, _ptr(lp)))
+        out.append((w, lp))
+    return out
 
 
 def with_language_tokens(opts: DecodingOptions, specialTokens: SpecialTokens, vocab: int, tokenizer=None) -> DecodingOptions:
@@ -742,3 +794,25 @@ class WhisperKit:
         attach_languages(out, *session_languages(self.model.lib, self.textDecoder.handle, n), tokenizer=self.tokenizer)
         attach_no_speech_probs(out, session_no_speech_probs(self.model.lib, self.textDecoder.handle, n))
         return out
+
+    def align(self, audioArrays, tokenLists: Sequence[Sequence[int]], samplesPerWindow: Optional[Sequence[int]] = None,
+              returnErrors: bool = False):
+        """Forced alignment of one token sequence per <=30 s window (audioArrays as transcribe takes them; each sequence the full decoder
+        input: prompt, text, EOT - e.g. a DecodingResult.tokens, beam search included).  Returns per window (alignmentWeights [n+1, 1500] f32,
+        tokenLogProbs [n] f32); words then come from WordTimingSeeker.findAlignment / addWordTimestamps."""
+        a = audioArrays
+        if not hasattr(a, "data_ptr"):
+            a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.ndim == 1:
+            a = a[None]
+        n, stride = int(a.shape[0]), int(a.shape[1])
+        if len(tokenLists) != n:
+            raise ValueError(f"{len(tokenLists)} token sequences for {n} windows")
+        st = self.specialTokens.to_c()
+        flat, offsets = _flatten_token_lists(tokenLists)
+        spw = None if samplesPerWindow is None else (C.c_int32 * n)(*[int(v) for v in samplesPerWindow])
+        status = (C.c_int32 * n)()
+        lib = self.model.lib
+        check(lib.wk_align_windows(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw, C.byref(st), _ptr(flat), _ptr(offsets),
+                                   status))
+        return aligned_results(lib, self.textDecoder.handle, tokenLists, status, returnErrors, self.model.info.n_audio_ctx)

@@ -211,6 +211,25 @@ wk_status decode_slots_init(DecodeState st, RowParams* rp_dev, const int32_t* sl
 // to the finished list, permute token / log-prob histories and cache ancestry to the surviving beams, advance the loop state
 wk_status beam_update(DecodeState st, BeamState beam, wk_special_tokens sp, int max_ctx, int groups, cudaStream_t stream);
 
+// ---- teacher-forced alignment pass (align_pass.cu): rows are (window, position) pairs, 224 rows per window, row w * 224 + t = position t.
+// seq_len[w] = the window's token count (0 = skipped); cross K/V of window w sit in cache block slot0 + w ([slot][H][T][64])
+// x[row] = embedding[row_tok[row]] + positional embedding[t] (f32), 0 where row_tok[row] < 0
+wk_status align_embed(const void* emb, const float* pos_emb, const int32_t* row_tok, float* x, int64_t rows, int d, int dtype, cudaStream_t stream);
+// causal self-attention over the [rows][3d] QKV output (biases already added) -> out [rows][d]
+wk_status align_self_attention(const void* qkv, const int32_t* seq_len, void* out, int nw, int H, int dtype, cudaStream_t stream);
+// q [rows][d] (16-bit) against the layer's cache block; kscale / vscale != nullptr: the FP8 cache.  stats != nullptr: each row's final softmax
+// (max, sum) per head as float pairs [H][stat_rows]
+wk_status align_cross_attention(const void* q, const void* kc, const void* vc, const float* kscale, const float* vscale, const int32_t* seq_len,
+                                int slot0, void* out, float* stats, int64_t stat_rows, int nw, int H, int Tlen, int dtype, cudaStream_t stream);
+// acc[row][T] (f32) += the normalised softmax rows of the heads in `mask`, ascending (first != 0: acc starts at 0)
+wk_status align_export(const void* q, const void* kc, const float* kscale, const float* stats, int64_t stat_rows, const int32_t* seq_len, int slot0,
+                       uint32_t mask, int first, float* acc, int nw, int H, int Tlen, int dtype, cudaStream_t stream);
+// Float16 alignmentWeights [nw][store_rows][T]: row t + 1 = acc[position t] / n_slots, row 0 and rows past the sequence 0
+wk_status align_rows_f16(const float* acc, const int32_t* seq_len, int n_slots, void* out, int nw, int Tlen, int store_rows, cudaStream_t stream);
+// logits rows [r0, r0 + rows) of the pass ([rows][ld] f32): out[r + 1] = log softmax(logits[r][:eot])[row_tok[r + 1]], NaN for targets >= eot
+wk_status align_token_logprobs(const float* logits, int64_t ld, int64_t r0, int64_t rows, const int32_t* row_tok, const int32_t* seq_len, int eot,
+                               float* out, cudaStream_t stream);
+
 // ---- a chain of decoder GEMM / split-K reduce phases in ONE persistent kernel with grid-wide barriers between the phases instead of
 // kernel boundaries (fused_chain.cu)
 wk_status make_tmap_2d(void* tm, const void* base, int dtype, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_cols, uint32_t box_rows);

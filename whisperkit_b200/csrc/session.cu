@@ -65,7 +65,15 @@ struct wk_session {
     // word timestamps: per-head softmax rows of the current step, the [S][224][T] Float16 alignmentWeights of the slots, and the per-window
     // copies handed out by wk_session_alignment_weights
     float* align_scratch = nullptr; void* align_w = nullptr; int align_slots = 0; bool align_on = false;
-    void* align_store = nullptr; int64_t align_store_cap = 0, align_store_n = 0;
+    // align_store_cap is in bytes; align_store_rows rows per window: 224 after a decode, 225 after an align call (row t + 1 = position t)
+    void* align_store = nullptr; int64_t align_store_cap = 0, align_store_n = 0; int align_store_rows = kKvMaxLen;
+    // teacher-forced alignment pass (wk_align_tokens / wk_align_windows): buffers for `al_cap` windows of 224 rows - the f32 alignment
+    // accumulator [rows][T], per-head softmax (max, sum) [H][rows][2], row tokens, sequence lengths, token log-probs, the QKV biases [L][3d];
+    // and the log-probs of the last call on the host, 224 per window
+    int al_cap = 0;
+    float *al_acc = nullptr, *al_stats = nullptr, *al_lp = nullptr, *al_bqkv = nullptr;
+    int32_t *al_tok = nullptr, *al_seq = nullptr;
+    std::vector<float> win_align_lp;
     unsigned int* chain_counters = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_adm = nullptr, ev_stage = nullptr, ev_t[10];
     bool knob_fused = false, knob_graph = true;
@@ -393,6 +401,19 @@ struct CoreArgs {
 
 static const wk_decode_opts& opts_of(const wk_batch_opts* bo, int64_t w) { return bo->n_opts == 1 ? bo->opts[0] : bo->opts[w]; }
 
+// the per-window alignmentWeights handed out by wk_session_alignment_weights: n_windows x rows x T Float16
+static wk_status ensure_align_store(wk_session* s, int64_t n_windows, int rows) {
+    const int64_t need = n_windows * rows * s->m->cfg.n_audio_ctx * 2;
+    if (s->align_store_cap < need) {
+        if (s->align_store) { WK_CUDA_CHECK(cudaStreamSynchronize(s->stream)); cudaFree(s->align_store); s->align_store = nullptr; }
+        WK_CUDA_CHECK(cudaMalloc(&s->align_store, (size_t)need));
+        s->align_store_cap = need;
+    }
+    s->align_store_n = n_windows;
+    s->align_store_rows = rows;
+    return WK_OK;
+}
+
 static wk_status ensure_align(wk_session* s, int64_t n_windows) {
     wk_model* m = s->m;
     const size_t T = m->cfg.n_audio_ctx;
@@ -404,13 +425,7 @@ static wk_status ensure_align(wk_session* s, int64_t n_windows) {
         if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }   // the scratch pointer is baked into the graphs
         if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
     }
-    if (s->align_store_cap < n_windows) {
-        if (s->align_store) { WK_CUDA_CHECK(cudaStreamSynchronize(s->stream)); cudaFree(s->align_store); s->align_store = nullptr; }
-        WK_CUDA_CHECK(cudaMalloc(&s->align_store, (size_t)n_windows * kKvMaxLen * T * 2));
-        s->align_store_cap = n_windows;
-    }
-    s->align_store_n = n_windows;
-    return WK_OK;
+    return ensure_align_store(s, n_windows, kKvMaxLen);
 }
 
 static wk_status ensure_beam(wk_session* s) {
@@ -582,6 +597,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     if (any_detect) WK_CUDA_CHECK(cudaMemcpyAsync(s->lang_dev, lang_list.data(), lang_list.size() * 4, cudaMemcpyHostToDevice, s->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));   // sup_pool is pageable: the copy must land before it goes out of scope paths below reuse it
     s->align_on = any_words;
+    s->win_align_lp.clear();   // the log-probs belong to the last align call only
     if (any_words) WK_CHECK(ensure_align(s, n));
 
     // ---- slots
@@ -901,6 +917,175 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     return WK_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- teacher-forced alignment pass
+// openai-whisper's find_alignment forward (timing.py): every position of a known token sequence through the decoder in one pass, the
+// alignment heads' cross-attention rows and the text tokens' log-probs out of it.  Row w * 224 + t of the encoder workspace is position t
+// of window w; the decoder GEMMs are the encoder's plain wgmma GEMMs over all rows, the attention / export / log-prob kernels are in
+// align_pass.cu.
+static constexpr int kAlignRows = kKvMaxLen + 1;   // alignment rows per window: row t + 1 for input position t, t < 224
+
+static wk_status ensure_align_pass(wk_session* s, int nw) {
+    if (s->al_cap >= nw) return WK_OK;
+    const wk_model_config& c = s->m->cfg;
+    WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
+    void* old[] = {s->al_acc, s->al_stats, s->al_lp, s->al_bqkv, s->al_tok, s->al_seq};
+    for (void* p : old) if (p) cudaFree(p);
+    const size_t R = (size_t)nw * kKvMaxLen;
+    WK_CHECK(dmalloc(&s->al_acc, R * c.n_audio_ctx, false));
+    WK_CHECK(dmalloc(&s->al_stats, R * c.n_heads * 2, false));
+    WK_CHECK(dmalloc(&s->al_lp, R));
+    WK_CHECK(dmalloc(&s->al_bqkv, (size_t)c.dec_layers * 3 * c.d_model));
+    WK_CHECK(dmalloc(&s->al_tok, R));
+    WK_CHECK(dmalloc(&s->al_seq, (size_t)nw));
+    s->al_cap = nw;
+    return WK_OK;
+}
+
+// windows [w_first, w_first + nw) of the call, their cross K/V in cache slots [slot0, slot0 + nw); seq / len: each window's tokens
+// (len 0 = a window that failed validation: no rows, zero alignment rows)
+static wk_status align_chunk(wk_session* s, const wk_special_tokens* st, int slot0, int nw, int64_t w_first, const int32_t* const* seq, const int* len) {
+    wk_model* m = s->m;
+    const wk_model_config& c = m->cfg;
+    const int d = c.d_model, H = c.n_heads, T = c.n_audio_ctx, dt = c.dtype;
+    const int64_t R = (int64_t)nw * kKvMaxLen;
+    cudaStream_t stm = s->stream;
+    EncWorkspace& ws = s->ws;
+    std::vector<int32_t> tok((size_t)R, -1), n(nw);
+    for (int i = 0; i < nw; ++i) {
+        n[i] = len[i];
+        for (int t = 0; t < len[i]; ++t) tok[(size_t)i * kKvMaxLen + t] = seq[i][t];
+    }
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->al_tok, tok.data(), (size_t)R * 4, cudaMemcpyHostToDevice, stm));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->al_seq, n.data(), (size_t)nw * 4, cudaMemcpyHostToDevice, stm));
+    const size_t cross_rows = (size_t)s->max_batch * H * T;
+    const size_t cross_block = cross_rows * 64 * ckv_esize(s);
+    auto gemm = [&](const void* a, int K, const void* w, int N, int mode, void* out, const float* bias, int gelu) {
+        return gemm_wgmma(plain_gemm(a, R, K, w, N, dt, mode, out, N, bias, gelu), m->num_sms, stm);
+    };
+    WK_CHECK(align_embed(m->emb, m->dec_pos, s->al_tok, ws.x, R, d, dt, stm));
+    int first_align = 1;
+    for (int li = 0; li < c.dec_layers; ++li) {
+        const DecLayer& l = m->dec[li];
+        WK_CHECK(layernorm_f32_to_16(ws.x, l.ln1.g, l.ln1.b, ws.xn, R, d, dt, stm));
+        WK_CHECK(gemm(ws.xn, d, l.wqkv, 3 * d, GEMM_OUT_T16, ws.qkv, s->al_bqkv + (size_t)li * 3 * d, 0));
+        WK_CHECK(align_self_attention(ws.qkv, s->al_seq, ws.attn, nw, H, dt, stm));
+        WK_CHECK(gemm(ws.attn, d, l.wo, d, GEMM_OUT_F32_ADD, ws.x, l.bo, 0));
+        WK_CHECK(layernorm_f32_to_16(ws.x, l.lnx.g, l.lnx.b, ws.xn, R, d, dt, stm));
+        WK_CHECK(gemm(ws.xn, d, l.wcq, d, GEMM_OUT_T16, ws.qkv, l.bcq, 0));   // cross-attention queries [R][d]
+        const uint32_t mask = m->align_mask[li];
+        const char* kc = (const char*)s->cross_kv + (size_t)(2 * li) * cross_block;
+        const char* vc = (const char*)s->cross_kv + (size_t)(2 * li + 1) * cross_block;
+        const float* ksc = s->ckv_fp8 ? s->cross_scale + (size_t)(2 * li) * cross_rows : nullptr;
+        const float* vsc = s->ckv_fp8 ? s->cross_scale + (size_t)(2 * li + 1) * cross_rows : nullptr;
+        WK_CHECK(align_cross_attention(ws.qkv, kc, vc, ksc, vsc, s->al_seq, slot0, ws.attn, mask ? s->al_stats : nullptr, R, nw, H, T, dt, stm));
+        if (mask) {
+            WK_CHECK(align_export(ws.qkv, kc, ksc, s->al_stats, R, s->al_seq, slot0, mask, first_align, s->al_acc, nw, H, T, dt, stm));
+            first_align = 0;
+        }
+        WK_CHECK(gemm(ws.attn, d, l.wco, d, GEMM_OUT_F32_ADD, ws.x, l.bco, 0));
+        WK_CHECK(layernorm_f32_to_16(ws.x, l.ln3.g, l.ln3.b, ws.xn, R, d, dt, stm));
+        WK_CHECK(gemm(ws.xn, d, l.w1, 4 * d, GEMM_OUT_T16, ws.ffn, l.b1, 1));
+        WK_CHECK(gemm(ws.ffn, 4 * d, l.w2, d, GEMM_OUT_F32_ADD, ws.x, l.b2, 0));
+    }
+    WK_CHECK(align_rows_f16(s->al_acc, s->al_seq, first_align ? 0 : m->n_align_slots, (char*)s->align_store + (size_t)w_first * kAlignRows * T * 2, nw, T,
+                            kAlignRows, stm));
+    // token log-probs: final LayerNorm, then the tied-embedding GEMM over the rows in chunks that fit the (now free) FC1 buffer, so that the
+    // [rows][vocab] logits never exist whole.  Columns [vocab, Vp) come out 0 (TMA zero-fills the weight rows past the vocabulary).
+    WK_CHECK(layernorm_f32_to_16(ws.x, m->dec_ln.g, m->dec_ln.b, ws.xn, R, d, dt, stm));
+    const int Vp = round_up(c.vocab, 32);
+    const int eot = std::min(st->end_token, c.vocab);
+    const int64_t chunk = std::max<int64_t>(1, (int64_t)ws.max_batch * T * 4 * d * 2 / ((int64_t)Vp * 4));
+    for (int64_t r0 = 0; r0 < R; r0 += chunk) {
+        const int64_t rc = std::min(chunk, R - r0);
+        GemmDesc g = plain_gemm((const char*)ws.xn + (size_t)r0 * d * 2, rc, d, m->emb, Vp, dt, GEMM_OUT_F32, ws.ffn, Vp, nullptr, 0);
+        g.b_rows = c.vocab;
+        WK_CHECK(gemm_wgmma(g, m->num_sms, stm));
+        WK_CHECK(align_token_logprobs((const float*)ws.ffn, Vp, r0, rc, s->al_tok, s->al_seq, eot, s->al_lp, stm));
+    }
+    std::vector<float> lp((size_t)R);
+    WK_CUDA_CHECK(cudaMemcpyAsync(lp.data(), s->al_lp, (size_t)R * 4, cudaMemcpyDeviceToHost, stm));
+    cudaError_t e = cudaStreamSynchronize(stm);
+    if (e != cudaSuccess) { set_error("alignment pass: %s", cudaGetErrorString(e)); return WK_ERR_DECODING_FAILED; }
+    for (int i = 0; i < nw; ++i)
+        for (int t = 1; t < len[i]; ++t) s->win_align_lp[(size_t)(w_first + i) * kKvMaxLen + t] = lp[(size_t)i * kKvMaxLen + t];
+    return WK_OK;
+}
+
+// wk_align_tokens (pcm == nullptr: windows are the bound rows) and wk_align_windows (PCM -> mel -> encoder -> cross K/V per chunk)
+static wk_status align_core(wk_session* s, const wk_special_tokens* st, const float* pcm, int64_t n, int64_t stride, const int32_t* spw,
+                            const int32_t* tokens, const int32_t* offsets, int32_t* status_out) {
+    wk_model* m = s->m;
+    const wk_model_config& c = m->cfg;
+    std::vector<int32_t> st_local((size_t)n, WK_OK);
+    int32_t* status = status_out ? status_out : st_local.data();
+    std::vector<int> len((size_t)n, 0);
+    std::string first_err;
+    for (int64_t w = 0; w < n; ++w) {
+        status[w] = WK_OK;
+        const int64_t cnt = (int64_t)offsets[w + 1] - offsets[w];
+        wk_status code = WK_OK;
+        if (cnt < 1) { set_error("window %lld: empty token sequence", (long long)w); code = WK_ERR_PREPARE_DECODER_INPUTS; }
+        else if (cnt > kKvMaxLen) { set_error("window %lld: %lld tokens exceed the %d-token decoder context", (long long)w, (long long)cnt, kKvMaxLen); code = WK_ERR_PREPARE_DECODER_INPUTS; }
+        else if (offsets[w] < 0) { set_error("window %lld: negative token offset %d", (long long)w, offsets[w]); code = WK_ERR_INVALID_ARGUMENT; }
+        else {
+            for (int64_t i = 0; i < cnt; ++i) {
+                const int32_t v = tokens[offsets[w] + i];
+                if (v < 0 || v >= c.vocab) {
+                    set_error("window %lld: token %d at position %lld outside the vocabulary (%d)", (long long)w, v, (long long)i, c.vocab);
+                    code = WK_ERR_PREPARE_DECODER_INPUTS;
+                    break;
+                }
+            }
+        }
+        if (code == WK_OK && pcm && spw && (spw[w] < 0 || spw[w] > kWindowSamples)) {
+            set_error("window %lld: samples_per_window %d out of range", (long long)w, spw[w]);
+            code = WK_ERR_AUDIO_PROCESSING_FAILED;
+        }
+        if (code != WK_OK) {
+            status[w] = code;
+            if (first_err.empty()) first_err = last_error_cstr();
+            if (!status_out) return code;
+            continue;
+        }
+        len[w] = (int)cnt;
+    }
+    if (pcm && stride < kWindowSamples && !spw) { set_error("wk_align_windows: stride < 480000 requires samples_per_window"); return WK_ERR_AUDIO_PROCESSING_FAILED; }
+    s->align_on = false;
+    WK_CHECK(enc_ws_ensure(m, &s->ws, c.max_batch));
+    WK_CHECK(ensure_align_store(s, n, kAlignRows));
+    s->win_align_lp.assign((size_t)n * kKvMaxLen, NAN);
+    // chunk size: the encoder's batch (PCM) or the rows the encoder workspace holds (bound windows), and the session's slots
+    const int Wc = (int)std::min<int64_t>(n, pcm ? std::min(s->max_batch, s->ws.max_batch) : (int64_t)s->ws.max_batch * c.n_audio_ctx / kKvMaxLen);
+    WK_CHECK(ensure_align_pass(s, Wc));
+    for (int li = 0; li < c.dec_layers; ++li) {   // the self-attention QKV bias [bq | 0 | bv]: the decoder's k projection has none
+        float* b = s->al_bqkv + (size_t)li * 3 * c.d_model;
+        WK_CUDA_CHECK(cudaMemcpyAsync(b, m->dec[li].bq, (size_t)c.d_model * 4, cudaMemcpyDeviceToDevice, s->stream));
+        WK_CUDA_CHECK(cudaMemsetAsync(b + c.d_model, 0, (size_t)c.d_model * 4, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(b + 2 * c.d_model, m->dec[li].bv, (size_t)c.d_model * 4, cudaMemcpyDeviceToDevice, s->stream));
+    }
+    std::vector<const int32_t*> seq((size_t)Wc);
+    for (int64_t w0 = 0; w0 < n; w0 += Wc) {
+        const int cnt = (int)std::min<int64_t>(Wc, n - w0);
+        int slot0 = (int)w0;
+        if (pcm) {
+            std::vector<int32_t> spw_fixed;
+            if (spw) {   // windows that failed validation are encoded as silence
+                spw_fixed.assign(spw + w0, spw + w0 + cnt);
+                for (int i = 0; i < cnt; ++i) if (status[w0 + i] != WK_OK) spw_fixed[i] = 0;
+            }
+            WK_CHECK(mel_run(m, &s->ws, pcm + w0 * stride, cnt, stride, spw ? spw_fixed.data() : nullptr, s->ws.mel, s->stream));
+            WK_CHECK(encode_chunk(m, &s->ws, s->ws.mel, cnt, s->ws.enc_out, s->stream));
+            WK_CHECK(gemm_wgmma(cross_kv_gemm(s, s->ws.enc_out, cnt, 0), m->num_sms, s->stream));
+            slot0 = 0;
+        }
+        for (int i = 0; i < cnt; ++i) seq[i] = tokens + (len[w0 + i] > 0 ? offsets[w0 + i] : 0);
+        WK_CHECK(align_chunk(s, st, slot0, cnt, w0, seq.data(), len.data() + w0));
+    }
+    s->align_on = true;
+    if (!first_err.empty()) set_error("%s", first_err.c_str());   // per-window failures are in status_out; the message of the first one
+    return WK_OK;
+}
+
 }  // namespace wk
 
 // =====================================================================================================
@@ -1021,7 +1206,7 @@ void wk_session_free(wk_session* s) {
                     s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error,
                     s->st.lang_token, s->st.lang_logprob, s->st.lang_state, s->st.no_speech, s->rp_dev,
                     s->pos_dev, s->lang_dev, s->suppress_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, s->align_scratch, s->align_w,
-                    s->align_store, s->chain_counters};
+                    s->align_store, s->chain_counters, s->al_acc, s->al_stats, s->al_lp, s->al_bqkv, s->al_tok, s->al_seq};
     for (void* p : ptrs) if (p) cudaFree(p);
     void* hptrs[] = {s->h_adm_slots, s->h_adm_prompts, s->h_adm_rp, s->h_tokens, s->h_logprobs, s->h_n_tokens, s->h_done, s->h_first_low, s->h_steps, s->h_error,
                      s->h_lang_token, s->h_lang_logprob, s->h_no_speech};
@@ -1206,25 +1391,54 @@ wk_status wk_session_no_speech_probs(const wk_session* s, int32_t first, int32_t
 }
 
 wk_status wk_session_alignment_weights(wk_session* s, int32_t window, int32_t rows, float* out) {
-    if (!s || !out || window < 0 || rows < 0 || rows > kKvMaxLen) { set_error("wk_session_alignment_weights: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
+    if (!s || !out || window < 0 || rows < 0 || rows > s->align_store_rows) { set_error("wk_session_alignment_weights: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (!s->align_on || !s->align_store || window >= s->align_store_n) { set_error("wk_session_alignment_weights: the last decode did not ask for word timestamps (or window %d is outside it)", window); return WK_ERR_INVALID_ARGUMENT; }
     WK_CUDA_CHECK(cudaSetDevice(s->m->device));
     const size_t T = s->m->cfg.n_audio_ctx;
     std::vector<__half> h((size_t)rows * T);
-    WK_CUDA_CHECK(cudaMemcpyAsync(h.data(), (const __half*)s->align_store + (size_t)window * kKvMaxLen * T, h.size() * 2, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(h.data(), (const __half*)s->align_store + (size_t)window * s->align_store_rows * T, h.size() * 2, cudaMemcpyDeviceToHost, s->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
     for (size_t i = 0; i < h.size(); ++i) out[i] = __half2float(h[i]);
     return WK_OK;
 }
 
 wk_status wk_session_alignment_weights_f16(wk_session* s, int32_t window, int32_t rows, uint16_t* out, int32_t sync) {
-    if (!s || !out || window < 0 || rows < 0 || rows > kKvMaxLen) { set_error("wk_session_alignment_weights_f16: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
+    if (!s || !out || window < 0 || rows < 0 || rows > s->align_store_rows) { set_error("wk_session_alignment_weights_f16: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (!s->align_on || !s->align_store || window >= s->align_store_n) { set_error("wk_session_alignment_weights_f16: the last decode did not ask for word timestamps (or window %d is outside it)", window); return WK_ERR_INVALID_ARGUMENT; }
     WK_CUDA_CHECK(cudaSetDevice(s->m->device));
     const size_t T = s->m->cfg.n_audio_ctx;
     if (rows > 0)
-        WK_CUDA_CHECK(cudaMemcpyAsync(out, (const __half*)s->align_store + (size_t)window * kKvMaxLen * T, (size_t)rows * T * 2, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(out, (const __half*)s->align_store + (size_t)window * s->align_store_rows * T, (size_t)rows * T * 2, cudaMemcpyDeviceToHost, s->stream));
     if (sync) WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
+    return WK_OK;
+}
+
+wk_status wk_align_tokens(wk_session* s, const wk_special_tokens* st, const int32_t* tokens, const int32_t* offsets, int64_t n_windows, int32_t* status) {
+    if (!s || !st || !tokens || !offsets || n_windows < 1) { set_error("wk_align_tokens: null argument"); return WK_ERR_INVALID_ARGUMENT; }
+    if (s->bound_windows < 1) { set_error("wk_align_tokens: no encoder output bound"); return WK_ERR_PREPARE_DECODER_INPUTS; }
+    if (n_windows > s->bound_windows) {
+        set_error("wk_align_tokens: %lld token sequences for %d bound windows", (long long)n_windows, s->bound_windows);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(s->m->device));
+    return align_core(s, st, nullptr, n_windows, 0, nullptr, tokens, offsets, status);
+}
+
+wk_status wk_align_windows(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride, const int32_t* samples_per_window,
+                           const wk_special_tokens* st, const int32_t* tokens, const int32_t* offsets, int32_t* status) {
+    if (!m || !s || !pcm_host || !st || !tokens || !offsets || n_windows < 1) { set_error("wk_align_windows: null argument"); return WK_ERR_INVALID_ARGUMENT; }
+    if (s->m != m) { set_error("wk_align_windows: session belongs to another model"); return WK_ERR_INVALID_ARGUMENT; }
+    if (!m->finalized) { set_error("wk_align_windows: model weights not finalized"); return WK_ERR_MODELS_UNAVAILABLE; }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    return align_core(s, st, pcm_host, n_windows, stride, samples_per_window, tokens, offsets, status);
+}
+
+wk_status wk_session_aligned_logprobs(const wk_session* s, int32_t window, int32_t n, float* out) {
+    if (!s || !out || window < 0 || n < 0 || n > kKvMaxLen || (int64_t)(window + 1) * kKvMaxLen > (int64_t)s->win_align_lp.size()) {
+        set_error("wk_session_aligned_logprobs: window %d / %d tokens outside the last align call", window, n);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (n > 0) memcpy(out, s->win_align_lp.data() + (size_t)window * kKvMaxLen, (size_t)n * 4);
     return WK_OK;
 }
 

@@ -1,25 +1,17 @@
-"""End-to-end example on an H100: long-form transcription of 16 kHz mono WAV files with segments, text and word timestamps.
+"""End-to-end example on an H100: long-form transcription of WAV files with segments, text and word timestamps.
 
   python examples/transcribe_long.py --weights /path/to/whisper-large-v3 audio1.wav audio2.wav [--vad] [--word-timestamps]
+                                     [--channel I | --channels I,J,...]
 
-`--weights` is a HuggingFace checkpoint directory (config.json, *.safetensors, tokenizer.json).  Without it the model runs with seeded
-random weights of the large-v3 shape (the token ids are then meaningless; useful as a smoke test of the machinery only)."""
+Files may have any sample rate (1 kHz .. 384 kHz) and channel count, in PCM u8 / s16 / s24 / s32 or float 32; AudioProcessor.loadAudio
+mixes them to mono (all channels summed by default) and resamples them to 16 kHz on the GPU.  `--weights` is a HuggingFace checkpoint
+directory (config.json, *.safetensors, tokenizer.json).  Without it the model runs with seeded random weights of the large-v3 shape (the
+token ids are then meaningless; useful as a smoke test of the machinery only)."""
 import argparse
 import os
 import sys
-import wave
-
-import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-
-def read_wav(path: str) -> np.ndarray:
-    with wave.open(path, "rb") as w:
-        if w.getframerate() != 16000 or w.getnchannels() != 1 or w.getsampwidth() != 2:
-            raise SystemExit(f"{path}: need 16 kHz mono s16 (resample first: the reference does this in AudioProcessor, out of scope here)")
-        pcm = np.frombuffer(w.readframes(w.getnframes()), dtype=np.int16)
-    return pcm.astype(np.float32) / 32768.0          # the reference's s16 -> f32 convention
 
 
 def main():
@@ -32,6 +24,9 @@ def main():
     ap.add_argument("--vad", action="store_true", help="chunkingStrategy .vad: split long audio at silences into independent units")
     ap.add_argument("--word-timestamps", action="store_true")
     ap.add_argument("--write", default=None, metavar="DIR", help="also write <audio>.srt / .vtt / .json there (ResultWriter.swift)")
+    mix = ap.add_mutually_exclusive_group()
+    mix.add_argument("--channel", type=int, default=None, help="transcribe this channel only (ChannelMode.specificChannel)")
+    mix.add_argument("--channels", default=None, help="comma-separated channels to sum (ChannelMode.sumChannels); default: all")
     args = ap.parse_args()
 
     import whisperkit_b200 as wk
@@ -42,7 +37,11 @@ def main():
     if args.word_timestamps and tokenizer is None:
         raise SystemExit("--word-timestamps needs --weights (tokenizer.json)")
     opts = wk.DecodingOptions(wordTimestamps=args.word_timestamps)
-    audio = [read_wav(p) for p in args.audio]
+    if args.channel is not None:
+        mode = wk.ChannelMode.specificChannel(args.channel)
+    else:
+        mode = wk.ChannelMode.sumChannels([int(c) for c in args.channels.split(",")] if args.channels else None)
+    audio = [wk.AudioProcessor.loadAudio(p, mode, session=kit.textDecoder) for p in args.audio]
     results = longform.transcribe_audio(kit, audio, opts, tokenizer=tokenizer, chunkingStrategy="vad" if args.vad else None)
     for path, r in zip(args.audio, results):
         print(f"== {path}: {len(r.segments)} segments, {r.windows} windows decoded in total")

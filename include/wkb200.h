@@ -52,7 +52,8 @@ enum {
     WK_ERR_DECODING_LOGITS_FAILED = -5, /* WhisperError.decodingLogitsFailed                 */
     WK_ERR_DECODING_FAILED = -6,        /* WhisperError.decodingFailed                       */
     WK_ERR_TRANSCRIPTION_FAILED = -7,   /* WhisperError.transcriptionFailed                  */
-    WK_ERR_CUDA = -8                    /* CUDA runtime/driver failure (message has detail)  */
+    WK_ERR_CUDA = -8,                   /* CUDA runtime/driver failure (message has detail)  */
+    WK_ERR_LOAD_AUDIO_FAILED = -9       /* WhisperError.loadAudioFailed                      */
 };
 
 typedef struct wk_model wk_model;
@@ -205,6 +206,55 @@ void wk_tensor_free(wk_tensor* t);
 /* pcm: n_windows rows of `stride` floats (host or device); samples_per_window[i] <= 480000 valid samples
  * (NULL = all 480000); the rest of the window is zero-padded (padOrTrimAudio, AudioProcessor.swift:151-174). */
 wk_status wk_mel(wk_model* m, const float* pcm, int64_t n_windows, int64_t stride, const int32_t* samples_per_window, wk_tensor** mel_out);
+
+/* ---- AudioProcessing: audio at any sample rate and channel layout -> 16 kHz mono f32 ----
+ *   wk_audio_info         AVAudioFile's fileFormat / length       Sources/WhisperKit/Core/Audio/AudioProcessor.swift:251-253
+ *   wk_audio_load         AudioProcessor.loadAudio(fromPath:) /   AudioProcessor.swift:229-305
+ *                         loadAudioAsFloatArray(fromPath:)        AudioProcessor.swift:307-350
+ *   wk_audio_convert      convertToMono + resampleAudio(fromFile:) AudioProcessor.swift:381-450,526-625
+ *                         on interleaved frames in memory
+ *   wk_audio_filter_taps  the resampler's filter design (host)
+ * Files: WAV (RIFF/WAVE) with PCM u8 / s16 / s24 / s32 or IEEE float 32, plain or WAVE_FORMAT_EXTENSIBLE; anything else (compressed
+ * formats, big-endian RIFX, 64-bit float) fails with WK_ERR_LOAD_AUDIO_FAILED and a message naming the format.  Samples become f32 as
+ * AVAudioFile converts them: s16 x / 32768, s24 x / 8388608, s32 float(x) / 2147483648, u8 (x - 128) / 128.
+ * Mono mix: convertToMono exactly, applied per read chunk of max_read_frame_size frames as the reference reads them (sumChannels
+ * rescales each chunk by max|selected channel| / max(max|sum|, 0.0001)).  Resampling: scipy.signal.resample_poly(x, 16000 / g, rate / g)
+ * with its default Kaiser (beta 5) window and zero padding, one continuous filter over the selected range (the reference converts each
+ * read chunk separately); the length is ceil(n * 16000 / rate).  16 kHz input is copied.  Sample rates: integer Hz in [1000, 384000],
+ * else WK_ERR_INVALID_ARGUMENT.  The GPU work runs on the session's stream (sessions on different threads convert concurrently), through
+ * the session's pinned staging and a fixed-size device workspace; session may be NULL (a stream and workspace for the call alone). */
+enum { WK_AUDIO_U8 = 0, WK_AUDIO_S16 = 1, WK_AUDIO_S24 = 2, WK_AUDIO_S32 = 3, WK_AUDIO_F32 = 4 };
+enum { WK_CHANNELS_SUM = 0 /* ChannelMode.sumChannels */, WK_CHANNELS_SPECIFIC = 1 /* ChannelMode.specificChannel */ };
+typedef struct wk_audio_format {
+    int32_t sample_rate, channels;
+    int32_t sample_format;     /* WK_AUDIO_* */
+    int32_t block_align;       /* bytes per interleaved frame */
+    int64_t frames;            /* frames present in the data chunk */
+    int64_t data_offset;       /* byte offset of the first frame in the file */
+} wk_audio_format;
+typedef struct wk_audio_load_opts {   /* all zero = sumChannels(nil), the whole file, default read size, loadAudio */
+    int32_t channel_mode;      /* WK_CHANNELS_SUM or WK_CHANNELS_SPECIFIC */
+    int32_t channel;           /* specificChannel(channel); out of range = channel 0 */
+    const int32_t* channel_indices; int32_t n_channel_indices;   /* sumChannels(indices); NULL or 0 = all channels */
+    int32_t has_end_time;      /* 0 = endTime nil (to the end of the file); else end_time is used */
+    double start_time;         /* seconds, finite and >= 0 */
+    double end_time;           /* seconds (has_end_time != 0); values at or past the end, +inf included, read to the end */
+    int64_t max_read_frame_size;   /* frames per read chunk; <= 0 = Constants.defaultAudioReadFrameSize (1323000) */
+    double piece_seconds;      /* loadAudioAsFloatArray's pieces (600); <= 0 = loadAudio (one piece) */
+    int64_t segment_samples;   /* 16 kHz samples per device segment; <= 0 = at most about 32 MiB of staged input and 4 Mi outputs per
+                                  segment.  Never more than the call's output; never changes the result */
+} wk_audio_load_opts;
+/* Header of a WAV file (host only, no GPU). */
+wk_status wk_audio_info(const char* path, wk_audio_format* out);
+/* Load `path` as 16 kHz mono f32 into out (host or device, capacity cap samples); *n_out = the length.  out == NULL returns the length only. */
+wk_status wk_audio_load(wk_session* s, const char* path, const wk_audio_load_opts* opts, float* out, int64_t cap, int64_t* n_out);
+/* The same for n_frames interleaved frames of `channels` samples in sample_format (host or device; device frames aligned to their sample
+ * size) at sample_rate: the result equals wk_audio_load of a WAV file holding these frames. */
+wk_status wk_audio_convert(wk_session* s, const void* frames, int32_t sample_format, int64_t n_frames, int32_t channels, int32_t sample_rate,
+                           const wk_audio_load_opts* opts, float* out, int64_t cap, int64_t* n_out);
+/* The resampler's filter for sample_rate (host only): up / down = 16000 / rate reduced, and the 2 * 10 * max(up, down) + 1 taps
+ * firwin(., 1 / max(up, down), window=('kaiser', 5.0)) * up in double (n = 0 when up == down == 1).  taps may be NULL (sizes only). */
+wk_status wk_audio_filter_taps(int32_t sample_rate, double* taps, int64_t cap, int32_t* up, int32_t* down, int32_t* n);
 
 /* ---- AudioEncoding ---- */
 wk_status wk_encode(wk_model* m, const wk_tensor* mel, wk_tensor** enc_out);

@@ -9,7 +9,8 @@ from ._lib import WhisperError, load  # noqa: F401
 from .api import (AudioEncoder, DecodingFallback, DecodingOptions, DecodingResult, DeviceTensor,  # noqa: F401
                   FeatureExtractor, Model, SpecialTokens, TextDecoder, WhisperKit, WhisperKitConfig,
                   filter_and_sample)
+from .audio import AudioProcessor, ChannelMode  # noqa: F401
 
 __all__ = ["WhisperKit", "WhisperKitConfig", "DecodingOptions", "DecodingResult", "DecodingFallback", "SpecialTokens",
            "FeatureExtractor", "AudioEncoder", "TextDecoder", "Model", "DeviceTensor", "filter_and_sample",
-           "WhisperError", "load"]
+           "WhisperError", "load", "AudioProcessor", "ChannelMode"]

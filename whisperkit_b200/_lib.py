@@ -17,8 +17,11 @@ WK_DTYPE_FP8_E4M3 = 4   # cross-attention K/V cache storage only
 STATUS_NAMES = {
     0: "ok", -1: "invalidArgument", -2: "modelsUnavailable", -3: "audioProcessingFailed",
     -4: "prepareDecoderInputsFailed", -5: "decodingLogitsFailed", -6: "decodingFailed",
-    -7: "transcriptionFailed", -8: "cudaError",
+    -7: "transcriptionFailed", -8: "cudaError", -9: "loadAudioFailed",
 }
+WK_ERR_INVALID_ARGUMENT, WK_ERR_LOAD_AUDIO_FAILED = -1, -9
+WK_AUDIO_U8, WK_AUDIO_S16, WK_AUDIO_S24, WK_AUDIO_S32, WK_AUDIO_F32 = 0, 1, 2, 3, 4
+WK_CHANNELS_SUM, WK_CHANNELS_SPECIFIC = 0, 1
 
 
 class WhisperError(RuntimeError):
@@ -101,6 +104,17 @@ class wk_word(C.Structure):
                 ("probability", C.c_float), ("segment", C.c_int32)]
 
 
+class wk_audio_format(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("channels", C.c_int32), ("sample_format", C.c_int32), ("block_align", C.c_int32),
+                ("frames", C.c_int64), ("data_offset", C.c_int64)]
+
+
+class wk_audio_load_opts(C.Structure):
+    _fields_ = [("channel_mode", C.c_int32), ("channel", C.c_int32), ("channel_indices", C.POINTER(C.c_int32)),
+                ("n_channel_indices", C.c_int32), ("has_end_time", C.c_int32), ("start_time", C.c_double), ("end_time", C.c_double),
+                ("max_read_frame_size", C.c_int64), ("piece_seconds", C.c_double), ("segment_samples", C.c_int64)]
+
+
 SPLIT_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_char), C.c_int32, C.POINTER(C.c_int32), C.c_int32)
 DECODE_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_char), C.c_int32)
 
@@ -132,6 +146,10 @@ SYMBOLS = [
     ("wk_tensor_to_host_strided", I32, [P, P, I64, I64, I64, I64]),
     ("wk_tensor_free", None, [P]),
     ("wk_mel", I32, [P, P, I64, I64, PI32, C.POINTER(P)]),
+    ("wk_audio_info", I32, [C.c_char_p, C.POINTER(wk_audio_format)]),
+    ("wk_audio_load", I32, [P, C.c_char_p, C.POINTER(wk_audio_load_opts), P, I64, PI64]),
+    ("wk_audio_convert", I32, [P, P, I32, I64, I32, I32, C.POINTER(wk_audio_load_opts), P, I64, PI64]),
+    ("wk_audio_filter_taps", I32, [I32, C.POINTER(C.c_double), I64, PI32, PI32, PI32]),
     ("wk_encode", I32, [P, P, C.POINTER(P)]),
     ("wk_session_create", I32, [P, I32, C.POINTER(P)]),
     ("wk_session_free", None, [P]),

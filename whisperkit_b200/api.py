@@ -699,6 +699,8 @@ class WhisperKitConfig:
     seed: int = 0
     modelFolder: Optional[str] = None            # HuggingFace checkpoint directory: config.json + *.safetensors (+ tokenizer.json / vocab.json)
     crossKVDtype: Optional[str] = None           # "fp8": E4M3 cross-attention K/V cache (Model); None = dtype
+    # audioInputConfig.channelMode: how transcribe(audioPath=...) mixes multi-channel files, ("sum", None | [indices]) or ("channel", i)
+    channelMode: tuple = ("sum", None)
 
 
 class WhisperKit:
@@ -758,11 +760,24 @@ class WhisperKit:
         import dataclasses
         return dataclasses.replace(opts, languageToken=int(tok))
 
-    def transcribe(self, audioArrays, decodeOptions=None, samplesPerWindow: Optional[Sequence[int]] = None, callback=None,
-                   callbackEvery: int = 0, returnErrors: bool = False, encoderChunk: int = 0):
+    def transcribe(self, audioArrays=None, decodeOptions=None, samplesPerWindow: Optional[Sequence[int]] = None, callback=None,
+                   callbackEvery: int = 0, returnErrors: bool = False, encoderChunk: int = 0, *, audioPath: Optional[str] = None,
+                   audioPaths: Optional[Sequence[str]] = None, chunkingStrategy: Optional[str] = None):
         """audioArrays: host float32 [N, stride<=480000-padded] (numpy, or pinned torch CPU tensor).  decodeOptions: one DecodingOptions
         or one per window (transcribeWithOptions' decodeOptionsArray, WhisperKit.swift:716-735).  One DecodingResult per window, in order;
-        with returnErrors a window that failed yields its WhisperError instead of failing the call (the reference's Result<>, :775-790)."""
+        with returnErrors a window that failed yields its WhisperError instead of failing the call (the reference's Result<>, :775-790).
+
+        audioPath= / audioPaths= (WhisperKit.swift:587-640, 823-860): audio files of any length, sample rate and channel layout, loaded
+        with AudioProcessor.loadAudioAsFloatArray (config.channelMode) on this kit's session and transcribed together by
+        longform.transcribe_audio (decodeOptions: one DecodingOptions).  audioPath returns its TranscriptionResult or raises; audioPaths
+        returns one TranscriptionResult per path, or the WhisperError that path's load raised."""
+        if audioPath is not None or audioPaths is not None:
+            if audioArrays is not None or (audioPath is not None and audioPaths is not None):
+                raise ValueError("pass one of audioArrays, audioPath, audioPaths")
+            res = self._transcribe_paths([audioPath] if audioPath is not None else list(audioPaths), decodeOptions, chunkingStrategy)
+            if audioPath is not None and isinstance(res[0], WhisperError):
+                raise res[0]
+            return res[0] if audioPath is not None else res
         a = audioArrays
         if not hasattr(a, "data_ptr"):
             a = np.ascontiguousarray(a, dtype=np.float32)
@@ -794,6 +809,15 @@ class WhisperKit:
         attach_languages(out, *session_languages(self.model.lib, self.textDecoder.handle, n), tokenizer=self.tokenizer)
         attach_no_speech_probs(out, session_no_speech_probs(self.model.lib, self.textDecoder.handle, n))
         return out
+
+    def _transcribe_paths(self, paths: Sequence[str], decodeOptions, chunkingStrategy: Optional[str]):
+        from . import longform
+        from .audio import AudioProcessor
+        loaded = AudioProcessor.loadAudio(at=paths, channelMode=self.config.channelMode, session=self.textDecoder)
+        good = [a for a in loaded if not isinstance(a, WhisperError)]
+        results = iter(longform.transcribe_audio(self, good, decodeOptions, tokenizer=self.tokenizer, chunkingStrategy=chunkingStrategy)
+                       if good else [])
+        return [a if isinstance(a, WhisperError) else next(results) for a in loaded]
 
     def align(self, audioArrays, tokenLists: Sequence[Sequence[int]], samplesPerWindow: Optional[Sequence[int]] = None,
               returnErrors: bool = False):

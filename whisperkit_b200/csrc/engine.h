@@ -129,6 +129,12 @@ wk_status encode_chunk(wk_model* m, EncWorkspace* ws, const void* mel, int B, vo
 GemmDesc plain_gemm(const void* a, int64_t M, int K, const void* w, int N, int dtype, int mode, void* out, int64_t ld_out,
                     const float* bias, int gelu);
 int choose_splits(int tiles, int total_kb, int num_sms);
+// audio.cu: a session's audio-loading workspace (pinned staging, device buffers), created on its first wk_audio_* call
+struct AudioWs;
+void audio_ws_free(AudioWs* w);
+AudioWs** session_audio_ws(wk_session* s);   // session.cu
+cudaStream_t session_stream(wk_session* s);
+int session_device(wk_session* s);
 size_t esize(int dtype);
 long long launch_counter_load();
 void launch_counter_sub(long long n);

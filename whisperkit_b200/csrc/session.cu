@@ -83,9 +83,14 @@ struct wk_session {
     int graph_beam = 1;
     std::vector<int> slot_window, slot_try;
     int64_t stats[4] = {0, 0, 0, 0};   // of the last batched call: step launches, sum of live rows over them, admissions, ladder re-admissions
+    AudioWs* audio = nullptr;          // wk_audio_load / wk_audio_convert workspace (audio.cu)
 };
 
 namespace wk {
+
+AudioWs** session_audio_ws(wk_session* s) { return &s->audio; }
+cudaStream_t session_stream(wk_session* s) { return s->stream; }
+int session_device(wk_session* s) { return s->m->device; }
 
 // ---------------------------------------------------------------------------------------------- decoder schedule
 static wk_status dec_gemm(wk_session* s, const void* w, int N, int K, const void* act, int* splits_out) {
@@ -1212,6 +1217,7 @@ void wk_session_free(wk_session* s) {
                      s->h_lang_token, s->h_lang_logprob, s->h_no_speech};
     for (void* p : hptrs) if (p) cudaFreeHost(p);
     enc_ws_free(&s->ws);
+    audio_ws_free(s->audio);
     cudaEventDestroy(s->ev_enc); cudaEventDestroy(s->ev_adm); cudaEventDestroy(s->ev_stage);
     for (auto& e : s->ev_t) cudaEventDestroy(e);
     cudaStreamDestroy(s->stream);

@@ -124,8 +124,9 @@ typedef struct wk_decode_opts {
     /* Beam search (SURVEY 8f row 2).  The reference's BeamSearchTokenSampler is an unimplemented stub (TokenSampler.swift:254-290) and its
      * DecodingOptions has no beam field, so these two are an extension: beam_size > 1 decodes every window with that many beams
      * (openai/whisper BeamSearchDecoder semantics inside the decodeText loop, specified by oracle/beam_ref.py; self-oracle parity only),
-     * maxCandidates = Int(Float(beam_size) * beam_patience) as the stub fixes (:266).  One setting per call; the temperature ladder and
-     * word timestamps do not combine with it. */
+     * maxCandidates = Int(Float(beam_size) * beam_patience) as the stub fixes (:266).  One setting per call.  With wk_batch_opts.best_of
+     * = 0 a beam call skips the temperature ladder; best_of >= 1 runs the ladder with beam search on its temperature-0 rung.  Word
+     * timestamps do not combine with beam_size > 1 (wk_align_tokens aligns beam results). */
     int32_t beam_size;            /* <= 1: greedy / temperature sampling (default) */
     float beam_patience;          /* default 1 */
     /* DecodingOptions.detectLanguage (Configurations.swift:165,222; TranscribeTask.swift:340-365): on a multilingual model with
@@ -316,6 +317,17 @@ typedef struct wk_batch_opts {
     int32_t progress_every;             /* decoder steps between callbacks / completion polls; <= 0 = 16 */
     wk_status* status;                  /* per-window Result<> (WhisperKit.swift:775-790): WK_OK or that window's error; may be NULL */
     int32_t encoder_chunk;              /* windows per mel+encoder pass; <= 0 = the model's max_batch */
+    /* Best-of-N sampling inside the temperature ladder (openai/whisper best_of with decode_with_fallback's per-rung rule; the reference's
+     * DecodingOptions has no bestOf, so this is an extension like wk_decode_opts.beam_size).  One value per call: it sizes the rows every
+     * window holds.  0 = off (the zeroed struct; the field sits in what was tail padding): every call decodes as before, and a beam call
+     * skips the ladder.  1..8: on every rung of the ladder (which now runs for beam calls too), temperature 0 decodes with beam_size beams
+     * if beam_size > 1, else one row; temperature > 0 draws best_of independent samples if best_of > 1 (row j of the group: Philox
+     * subsequence = its decode row), else one row.  The kept sample maximises the sum of its token log-probs / max(sampled tokens, 1),
+     * ties to the lowest row, and then goes through DecodingFallback as usual.  Each window takes G = max(beam_size, best_of) decode rows
+     * for the whole call, so a session holds max_batch / G windows in flight; a rung that uses fewer rows (the greedy rung of
+     * beam_size 1, best_of 5 uses one of five) leaves the others idle.  G must fit the session's rows.  Word timestamps work with
+     * beam_size <= 1: the kept sample's alignment rows are returned. */
+    int32_t best_of;
 } wk_batch_opts;
 
 /* ---- whole hot path: host PCM in, token IDs out (TranscribeTask.run body, batched) ----
@@ -395,6 +407,11 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
                                 const wk_special_tokens* st, const wk_decode_opts* opts, const int32_t* prompt, int32_t n_prompt,
                                 const float* clip_timestamps, int32_t n_clip_timestamps, float window_clip_time, int64_t max_window_seek,
                                 int32_t chunking_vad, const wk_tokenizer_hooks* hooks, wk_transcription** out);
+/* The same with wk_batch_opts.best_of for every window of the call (0 = wk_transcribe_streams). */
+wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* const* audio, const int64_t* n_samples, int32_t n_streams,
+                                   const wk_special_tokens* st, const wk_decode_opts* opts, const int32_t* prompt, int32_t n_prompt,
+                                   const float* clip_timestamps, int32_t n_clip_timestamps, float window_clip_time, int64_t max_window_seek,
+                                   int32_t chunking_vad, const wk_tokenizer_hooks* hooks, int32_t best_of, wk_transcription** out);
 int32_t wk_transcription_segment_count(const wk_transcription* t);
 int32_t wk_transcription_window_count(const wk_transcription* t);
 int64_t wk_transcription_token_count(const wk_transcription* t);

@@ -90,7 +90,7 @@ class wk_batch_opts(C.Structure):
                 ("prompts", C.POINTER(C.POINTER(C.c_int32))), ("prompt_lens", C.POINTER(C.c_int32)),
                 ("prompt", C.POINTER(C.c_int32)), ("n_prompt", C.c_int32),
                 ("progress", PROGRESS_FN), ("progress_user", C.c_void_p), ("progress_every", C.c_int32),
-                ("status", C.POINTER(C.c_int32)), ("encoder_chunk", C.c_int32)]
+                ("status", C.POINTER(C.c_int32)), ("encoder_chunk", C.c_int32), ("best_of", C.c_int32)]
 
 
 class wk_segment(C.Structure):
@@ -189,6 +189,8 @@ SYMBOLS = [
     ("wk_vad_chunk_all", I32, [P, I64, I64, PF32, I32, I64, I32, I32, F32, PI64, I32, PI32]),
     ("wk_transcribe_streams", I32, [P, P, C.POINTER(P), PI64, I32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts), PI32, I32,
                                     PF32, I32, F32, I64, I32, C.POINTER(wk_tokenizer_hooks), C.POINTER(P)]),
+    ("wk_transcribe_streams_ex", I32, [P, P, C.POINTER(P), PI64, I32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts), PI32, I32,
+                                       PF32, I32, F32, I64, I32, C.POINTER(wk_tokenizer_hooks), I32, C.POINTER(P)]),
     ("wk_transcription_segment_count", I32, [P]),
     ("wk_transcription_window_count", I32, [P]),
     ("wk_transcription_token_count", I64, [P]),

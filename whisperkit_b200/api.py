@@ -23,7 +23,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import (PROGRESS_FN, WK_DTYPE_BF16, WK_DTYPE_F16, WK_DTYPE_F32, WhisperError, check, wk_batch_opts, wk_decode_opts,
+from ._lib import (PROGRESS_FN, WK_DTYPE_BF16, WK_DTYPE_F16, WK_DTYPE_F32, WK_ERR_INVALID_ARGUMENT, WhisperError, check, wk_batch_opts, wk_decode_opts,
                    wk_decode_result, wk_model_config, wk_model_info, wk_special_tokens)
 
 MAX_TOKEN_CONTEXT = 224  # Constants.maxTokenContext (Models.swift:1334)
@@ -115,6 +115,11 @@ class DecodingOptions:
     # compute DecodingResult.noSpeechProb in the decode loop (openai/whisper's rule; the reference leaves it 0), so that noSpeechThreshold
     # marks silent windows (fallback reason "silence") and the long-form loop skips them
     computeNoSpeechProb: bool = False
+    # best-of-N sampling inside the temperature ladder (openai/whisper's best_of; the reference's DecodingOptions has none): None = off,
+    # as before (a beam call skips the ladder); >= 1 = openai's decode_with_fallback - beam search at temperature 0 when beamSize > 1,
+    # bestOf samples (the most likely kept) at temperature > 0, on every rung of the ladder, beam calls included.  One value per call
+    # (C: wk_batch_opts.best_of, wk_transcribe_streams_ex)
+    bestOf: Optional[int] = None
 
     @property
     def detectsLanguage(self) -> bool:
@@ -629,6 +634,10 @@ def make_batch_opts(n: int, options, prompt, callback=None, callbackEvery: int =
         keep.append(k)
     keep.append(arr)
     bo.opts, bo.n_opts = arr, len(opt_list)
+    best_of = {int(o.bestOf or 0) for o in opt_list}
+    if len(best_of) != 1:
+        raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"bestOf must be the same for every window of a call (got {sorted(best_of)})")
+    bo.best_of = best_of.pop()
     if prompt is not None and len(prompt) > 0 and isinstance(prompt[0], (list, tuple, np.ndarray)):
         if len(prompt) != n:
             raise ValueError(f"{len(prompt)} prompts for {n} windows")

@@ -106,7 +106,12 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
     const int r0 = win * NQ;                 // first decode row of the window
     const int dm = H * 64;
     pdl_launch_dependents();
-    const int ended = done != nullptr ? done[r0] : 0;   // the beams of a window end together
+    // the group is skipped once all its rows have ended (beams end together; best-of samples one by one, and the rows a rung leaves
+    // unused start ended)
+    int ended = done != nullptr;
+    if (done != nullptr)
+#pragma unroll
+        for (int j = 0; j < NQ; ++j) ended &= done[r0 + j] != 0;
     if (tid == 0) {
         tma_prefetch_desc(&tm_k);
         tma_prefetch_desc(&tm_v);

@@ -50,6 +50,9 @@ __global__ void decode_slots_init_kernel(DecodeState st, RowParams* __restrict__
     for (int t = threadIdx.x; t < kMaxCtx; t += blockDim.x) {
         st.tokens[b * kMaxCtx + t] = t < n_prompt ? prompts[i * kMaxCtx + t] : 0;
         st.logprobs[b * kMaxCtx + t] = 0.f;
+        // the call has beam rows, so the self-attention reads every row through the cache ancestry: a row that never reorders (single or
+        // sample rung) must read its own cache rows.  beam_update_kernel rewrites the entries of beam rows before they are read
+        if (bs.beam > 1) bs.anc[b * kMaxCtx + t] = b;
     }
     if (threadIdx.x == 0) {
         rp_dev[b] = R;
@@ -66,7 +69,7 @@ __global__ void decode_slots_init_kernel(DecodeState st, RowParams* __restrict__
         st.no_speech[b] = __int_as_float(0x7fc00000);   // NaN: not computed (yet)
         if (bs.beam > 1) {
             bs.sum_lp[b] = 0.f;
-            if (b % bs.beam == 0) bs.n_fin[b / bs.beam] = 0;
+            if (b % bs.group == 0) bs.n_fin[b / bs.group] = 0;
         }
     }
 }
@@ -835,7 +838,7 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         R.prompt_len = -1; R.sample_begin_ts = p.sample_begin_ts; R.sample_begin_blank = p.sample_begin_blank; R.max_steps = 0;
         R.temperature = p.temperature; R.top_k = p.top_k; R.has_first_thr = 0; R.first_thr = 0.f; R.seed = p.seed;
         R.suppress_off = 0; R.n_suppress = p.n_suppress;
-        R.detect = 0; R.lang_pos = -1; R.n_lang = 0; R.lead_token = 0; R.no_speech_pos = -1;
+        R.detect = 0; R.lang_pos = -1; R.n_lang = 0; R.lead_token = 0; R.no_speech_pos = -1; R.mode = kRowSingle;
     }
     const int32_t* toks = loop_mode ? st.tokens + b * kMaxCtx : tokens_in + (long long)b * ld_tokens;
     const wk_special_tokens& S = p.st;
@@ -864,7 +867,10 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
                 if (x != -INFINITY) sm += __expf(x - mx);
             }
             sm = block_sum(sm, scratch);
-            const ArgMax d = sample_row(srow, 0, V, mx, mx + logf(sm), R.temperature, R.top_k, R.seed, kDetectSubsequence + (unsigned long long)b, 0ull,
+            // every row of a group draws with the group's first row's subsequence: the group's rows are copies of one window, so its
+            // best-of candidates (and beams) share one detected language
+            const int g0 = p.beam.group > 1 ? b - b % p.beam.group : b;
+            const ArgMax d = sample_row(srow, 0, V, mx, mx + logf(sm), R.temperature, R.top_k, R.seed, kDetectSubsequence + (unsigned long long)g0, 0ull,
                                         scratch, sarg);
             if (tid == 0) {
                 const bool ok = d.i >= 0 && d.i < V;
@@ -1007,7 +1013,7 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         for (int i = tid; i < V; i += kSamplerThreads) filtered_out[(long long)b * V + i] = srow[i];
         __syncthreads();
     }
-    if (loop_mode && p.beam.beam > 1) {
+    if (loop_mode && R.mode == kRowBeam) {
         // beam search: rank the row's (beam + 1) best tokens of the filtered log-softmax, best first (whisper BeamSearchDecoder.update step 1);
         // the per-window merge and every state update happen in beam_update_kernel
         const int k = p.beam.beam + 1;
@@ -1075,12 +1081,13 @@ beam_update_kernel(DecodeState st, BeamState bs, wk_special_tokens S, int max_ct
     __shared__ float n_lp[kMaxBeam], n_score[kMaxBeam];
     __shared__ int f_src[kMaxCand]; __shared__ float f_score[kMaxCand];
     __shared__ int sh[4];   // 0: mode (0 prefill/plain advance, 1 ranked, 2 ended without ranking)  1: new finished count  2: window done  3: finished before
-    const int g = blockIdx.x, tid = threadIdx.x, beam = bs.beam, r0 = g * beam;
+    const int g = blockIdx.x, tid = threadIdx.x, beam = bs.beam, r0 = g * bs.group;   // a beam group uses the first `beam` of its rows
     pdl_launch_dependents();
     pdl_wait();
     if (st.done[r0]) return;
     if (st.lang_state[r0] == kLangLeadRan) return;   // the leading language-detection step ranked nothing: no beam bookkeeping
     const RowParams R = st.rp[r0];
+    if (R.mode != kRowBeam) return;                  // a single / best-of rung: the sampler did the rows' bookkeeping
     const int step = st.steps[r0], n_tok = st.n_tokens[r0], P = R.prompt_len;
     const int C1 = kMaxBeam + 1;
     if (tid == 0) {
@@ -1177,8 +1184,10 @@ beam_update_kernel(DecodeState st, BeamState bs, wk_special_tokens S, int max_ct
 }
 
 wk_status beam_update(DecodeState st, BeamState beam, wk_special_tokens sp, int max_ctx, int groups, cudaStream_t stream) {
-    if (beam.beam < 2 || beam.beam > kMaxBeam || beam.max_candidates < 1 || beam.max_candidates > kMaxCand) {
-        set_error("beam_update: beam %d / candidates %d outside [2, %d] / [1, %d]", beam.beam, beam.max_candidates, kMaxBeam, kMaxCand);
+    if (beam.beam < 2 || beam.beam > kMaxBeam || beam.max_candidates < 1 || beam.max_candidates > kMaxCand || beam.group < beam.beam ||
+        beam.group > kMaxBeam) {
+        set_error("beam_update: beam %d / candidates %d / group %d outside [2, %d] / [1, %d] / [beam, %d]", beam.beam, beam.max_candidates,
+                  beam.group, kMaxBeam, kMaxCand, kMaxBeam);
         return WK_ERR_INVALID_ARGUMENT;
     }
     launch_k(beam_update_kernel, dim3(groups), dim3(kBeamThreads), 0, stream, 8, st, beam, sp, max_ctx);

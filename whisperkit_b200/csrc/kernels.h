@@ -114,7 +114,11 @@ struct RowParams {
     int32_t lead_token;          // <|startoftranscript|>: what the leading detection step feeds at position 0
     // DecodingResult.noSpeechProb: the step (= index of the prompt's first SOT) whose raw logits give it, <0 = off
     int32_t no_speech_pos;
+    int32_t mode;                // kRowSingle / kRowBeam / kRowSample: how the row's rung decodes (one step mixes groups at different rungs)
 };
+// RowParams.mode.  Single and sample rows run the per-row sampler and bookkeeping (a sample row is one of best_of independent draws of its
+// group); beam rows only rank candidates, and beam_update_kernel does their bookkeeping per group
+constexpr int kRowSingle = 0, kRowBeam = 1, kRowSample = 2;
 
 struct DecodeState {
     // all device pointers; one entry per decode row (slot).  A slot with done != 0 is skipped by every kernel of the step.
@@ -136,12 +140,14 @@ struct DecodeState {
 constexpr int kLangLead = 2, kLangLeadRan = 3;
 
 // Beam search (SURVEY 8f row 2; semantics restated from openai/whisper BeamSearchDecoder in oracle/beam_ref.py - the reference's
-// BeamSearchTokenSampler is a fatalError stub, TokenSampler.swift:254-290).  Decode rows come in groups of `beam` consecutive rows per window.
+// BeamSearchTokenSampler is a fatalError stub, TokenSampler.swift:254-290).  Decode rows come in groups of `group` consecutive rows per
+// window (G = max(beam_size, best_of)); a beam-mode group uses its first `beam` rows, a best-of group its first best_of rows.
 constexpr int kMaxBeam = 8;
 constexpr int kMaxCand = 8;        // maxCandidates = Int(Float(beamSize) * patience) (TokenSampler.swift:266)
 struct BeamState {
-    int beam;                      // rows per window; <= 1 = greedy / sampling, every field below unused
+    int beam;                      // beams of a beam-mode group; <= 1 = the call has no beam rows, every pointer below unused
     int max_candidates;
+    int group;                     // decode rows per window (<= 1: one)
     float* sum_lp;                 // [rows] cumulative log-prob of the sampled tokens of the beam
     int32_t* cand_tok; float* cand_lp;   // [rows][kMaxBeam + 1] best tokens of the step's filtered log-softmax, best first (-1 = none)
     int32_t* anc;                  // [rows][224] physical cache row that holds position t of this beam's self K/V
@@ -159,7 +165,7 @@ struct SamplerParams {
     const int32_t* language_tokens; int n_language_tokens; int language_sample_begin;
     int max_ctx;             // 224
     const int32_t* detect_tokens;   // loop mode: allLanguageTokens of the rows with RowParams.detect (in-loop language detection)
-    BeamState beam;         // loop mode with beam.beam > 1: the kernel only ranks candidates; beam_update() does the bookkeeping
+    BeamState beam;         // loop mode: rows with RowParams.mode == kRowBeam only rank candidates; beam_update() does their bookkeeping
     // stateless mode only
     int sample_begin_ts, sample_begin_blank, n_suppress;
     float temperature; int top_k; uint64_t seed;
@@ -208,7 +214,8 @@ wk_status sampler_filter_sample(const float* logits, int64_t ld_logits, SamplerP
 wk_status decode_slots_init(DecodeState st, RowParams* rp_dev, const int32_t* slot_ids, const int32_t* prompts, const RowParams* rp_new,
                             int n, cudaStream_t stream, BeamState beam = BeamState());
 // the beam-search step after the sampler ranked every row's candidates: per window, merge the beams' candidates, move finished sequences
-// to the finished list, permute token / log-prob histories and cache ancestry to the surviving beams, advance the loop state
+// to the finished list, permute token / log-prob histories and cache ancestry to the surviving beams, advance the loop state.  One CTA per
+// group of beam.group rows; groups whose rung is not in beam mode return at once
 wk_status beam_update(DecodeState st, BeamState beam, wk_special_tokens sp, int max_ctx, int groups, cudaStream_t stream);
 
 // ---- teacher-forced alignment pass (align_pass.cu): rows are (window, position) pairs, 224 rows per window, row w * 224 + t = position t.

@@ -321,6 +321,14 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
                                 const wk_special_tokens* st, const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt,
                                 const float* cts, int32_t n_cts, float window_clip_time, int64_t max_window_seek, int32_t chunking_vad,
                                 const wk_tokenizer_hooks* hooks, wk_transcription** out) {
+    return wk_transcribe_streams_ex(m, s, audio, n_samples, n_streams, st, o, prompt, n_prompt, cts, n_cts, window_clip_time, max_window_seek,
+                                    chunking_vad, hooks, 0, out);
+}
+
+wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* const* audio, const int64_t* n_samples, int32_t n_streams,
+                                   const wk_special_tokens* st, const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt,
+                                   const float* cts, int32_t n_cts, float window_clip_time, int64_t max_window_seek, int32_t chunking_vad,
+                                   const wk_tokenizer_hooks* hooks, int32_t best_of, wk_transcription** out) {
     if (!m || !s || !audio || !n_samples || n_streams < 1 || !st || !o || !prompt || !out) { set_error("wk_transcribe_streams: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (o->word_timestamps && (!hooks || !hooks->split_to_word_tokens)) { set_error("wk_transcribe_streams: wordTimestamps needs the tokenizer's split_to_word_tokens hook"); return WK_ERR_INVALID_ARGUMENT; }
     wk_model_info info;
@@ -391,7 +399,10 @@ wk_status wk_transcribe_streams(wk_model* m, wk_session* s, const float* const* 
             memcpy(batch + (size_t)k * kWindow, u.audio + u.seek, (size_t)sz * sizeof(float));   // padOrTrim (zero fill happens in the mel kernel via `valid`)
             return WK_OK;
         }, nullptr);
-        rc = wk_transcribe_windows(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, o, prompt, n_prompt, res.data());
+        wk_batch_opts bo;
+        memset(&bo, 0, sizeof(bo));
+        bo.opts = o; bo.n_opts = 1; bo.prompt = prompt; bo.n_prompt = n_prompt; bo.best_of = best_of;
+        rc = wk_transcribe_windows_ex(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data());
         if (rc != WK_OK) { delete T; return rc; }
         T->windows += (int)active.size();
         if (o->detect_language) {   // TranscriptionResult.language: the stream keeps the language of its last detecting window

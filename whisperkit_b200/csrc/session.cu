@@ -27,7 +27,7 @@ using namespace wk;
 struct wk_session {
     wk_model* m = nullptr;
     int max_batch = 0;        // decode slots
-    int batch = 0;            // rows the step runs over: slots [0, batch) (x beam rows per slot with beam search)
+    int batch = 0;            // rows the step runs over: slots [0, batch / G), G = max(beam, best_of) rows per slot
     int bound_windows = 0;    // windows bound by wk_session_set_encoder_output (cross K/V blocks 0 .. bound_windows - 1)
     int bp = 16;              // batch padded to a multiple of 16 (the GEMM tile N granule)
     cudaStream_t stream = nullptr;      // decode stream
@@ -141,7 +141,9 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
     // ended rows are skipped by the attention kernels; a burst that starts with every slot live runs the variant without the checks (a
     // row that ends inside it just keeps computing until the next poll, as harmlessly as before it ended)
     const int32_t* done = (explicit_pos || !check_done) ? nullptr : s->st.done;
-    const bool beam_rows = !explicit_pos && s->bs.beam > 1;   // rows are beams: cache ancestry + one cross K/V block per `beam` rows
+    // loop mode: the window's G rows share one cross K/V block; a call with beam rows reads the self K/V through the cache ancestry
+    const bool beam_rows = !explicit_pos && s->bs.beam > 1;
+    const int kv_div = explicit_pos ? 1 : std::max(1, s->bs.group);
     const int n_layers = c.dec_layers;
     int sp = 1;
     WK_CHECK(decoder_embed_ln(m->emb, m->dec_pos, m->dec[0].ln1.g, m->dec[0].ln1.b, s->st, c.vocab, ts_begin, s->x, s->xn, B, d, dt, explicit_pos, st));
@@ -154,7 +156,7 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
         return decoder_cross_attention(s->partial, sp, Bp, l.bcq, (char*)s->cross_kv + (size_t)(2 * li) * cross_block,
                                        (char*)s->cross_kv + (size_t)(2 * li + 1) * cross_block, s->attn, B, H, T, dt, st, done,
                                        align ? s->align_scratch + (size_t)m->align_base[li] * B * T : nullptr, align ? m->align_mask[li] : 0u,
-                                       beam_rows ? s->bs.beam : 1, s->ckv_fp8 ? s->cross_scale + (2 * li) * cross_rows : nullptr,
+                                       kv_div, s->ckv_fp8 ? s->cross_scale + (2 * li) * cross_rows : nullptr,
                                        s->ckv_fp8 ? s->cross_scale + (2 * li + 1) * cross_rows : nullptr);
     };
     if (fused) {
@@ -338,7 +340,7 @@ static wk_status enqueue_step(wk_session* s, const wk_special_tokens* st, bool f
     wk_model* m = s->m;
     WK_CHECK(decoder_forward(s, st->time_token_begin, nullptr, fused, check_done));
     WK_CHECK(sampler_filter_sample(s->logits, m->cfg.vocab, loop_sampler_params(s, st), s->st, nullptr, 0, nullptr, nullptr, nullptr, nullptr, s->batch, s->stream));
-    if (s->bs.beam > 1) WK_CHECK(beam_update(s->st, s->bs, *st, kKvMaxLen, s->batch / s->bs.beam, s->stream));
+    if (s->bs.beam > 1) WK_CHECK(beam_update(s->st, s->bs, *st, kKvMaxLen, s->batch / s->bs.group, s->stream));
     if (s->align_on)
         WK_CHECK(decoder_align_mean(s->align_scratch, m->n_align_slots, s->st.steps, s->st.done, s->st.lang_state, s->align_w, s->batch, m->cfg.n_audio_ctx,
                                     kKvMaxLen, s->stream));
@@ -357,7 +359,8 @@ static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bo
         s->warmed = true;
     }
     if (done >= n) return WK_OK;
-    const int beam_key = std::max(1, s->bs.beam) * 16 + s->bs.max_candidates;
+    // the step's shape depends on the rows per window (cross K/V sharing) and on whether the call has beam rows (ancestry, beam_update)
+    const int beam_key = (std::max(1, s->bs.group) * 16 + std::max(1, s->bs.beam)) * 16 + s->bs.max_candidates;
     const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_fused != fused || s->graph_beam != beam_key ||
                        memcmp(&s->graph_st, st, sizeof(*st)) != 0;
     if (stale) {
@@ -469,12 +472,20 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     const int64_t n = a.n;
     const int d = c.d_model, T = c.n_audio_ctx;
     const int poll = bo->progress_every > 0 ? bo->progress_every : 16;
-    // beam search: every window takes `beam` consecutive decode rows; one setting per call (it shapes the step graph)
+    // beam search / best-of: every window takes G = max(beam, best_of) consecutive decode rows; one setting per call (it shapes the step
+    // graph).  best_of == 0 keeps the plain rule: beam search (no ladder) or one row; best_of >= 1 picks the rows per ladder rung
     const int beam = bo->opts[0].beam_size > 1 ? bo->opts[0].beam_size : 1;
+    const int best_of = bo->best_of;
     for (int i = 0; i < bo->n_opts; ++i)
         if ((bo->opts[i].beam_size > 1 ? bo->opts[i].beam_size : 1) != beam || (beam > 1 && bo->opts[i].beam_patience != bo->opts[0].beam_patience)) {
             set_error("beam size / patience must be the same for every window of a call"); return WK_ERR_INVALID_ARGUMENT;
         }
+    if (best_of < 0 || best_of > kMaxBeam) { set_error("best_of %d outside [0, %d]", best_of, kMaxBeam); return WK_ERR_INVALID_ARGUMENT; }
+    const int G = std::max(beam, std::max(best_of, 1));
+    if (G > s->max_batch) {
+        set_error("%d rows per window (beam size %d, best_of %d) exceed the session's %d rows", G, beam, best_of, s->max_batch);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
     int max_cand = 0;
     if (beam > 1) {
         const float patience = bo->opts[0].beam_patience > 0.f ? bo->opts[0].beam_patience : 1.f;
@@ -487,9 +498,9 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             if (bo->opts[i].word_timestamps) { set_error("wordTimestamps with beam search is not supported"); return WK_ERR_INVALID_ARGUMENT; }
         WK_CHECK(ensure_beam(s));
     }
-    s->bs.beam = beam; s->bs.max_candidates = max_cand;
-    const int S = s->max_batch / beam;     // decode slots (windows in flight)
-    if (bound && n > S) { set_error("wk_decode_text: %lld bound windows x beam %d exceed the session's %d rows", (long long)n, beam, s->max_batch); return WK_ERR_PREPARE_DECODER_INPUTS; }
+    s->bs.beam = beam; s->bs.max_candidates = max_cand; s->bs.group = G;
+    const int S = s->max_batch / G;        // decode slots (windows in flight)
+    if (bound && n > S) { set_error("wk_decode_text: %lld bound windows x %d rows exceed the session's %d rows", (long long)n, G, s->max_batch); return WK_ERR_PREPARE_DECODER_INPUTS; }
     std::vector<wk_status> st_local((size_t)n, WK_OK);
     wk_status* status = bo->status ? bo->status : st_local.data();
     for (int64_t w = 0; w < n; ++w) status[w] = WK_OK;
@@ -606,8 +617,8 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     if (any_words) WK_CHECK(ensure_align(s, n));
 
     // ---- slots
-    const int Brun = (int)std::min<int64_t>(S, n);     // slots in use; the step covers Brun * beam rows
-    s->batch = Brun * beam;
+    const int Brun = (int)std::min<int64_t>(S, n);     // slots in use; the step covers Brun * G rows
+    s->batch = Brun * G;
     s->bp = round_up(s->batch, 16);
     const int rows = s->batch;
     s->slot_window.assign(S, -1);
@@ -623,6 +634,15 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         const float f16_t = __half2float(__float2half(o.temperature));
         const float f16_step = __half2float(__float2half(__half2float(__float2half((float)i)) * __half2float(__float2half(o.temperature_increment_on_fallback))));
         return __half2float(__float2half(f16_t + f16_step));
+    };
+    // the rows a rung decodes with (openai/whisper decode_with_fallback): best_of == 0 - beam search on every row of a beam call, else one
+    // row; best_of >= 1 - beam search at temperature 0 when beam > 1, best_of independent samples at temperature > 0 when best_of > 1,
+    // else one row.  The group's other rows stay ended
+    auto rung_mode = [&](float temperature, int* active) -> int {
+        if (beam > 1 && (best_of == 0 || temperature == 0.f)) { *active = beam; return kRowBeam; }
+        if (best_of > 1 && temperature > 0.f) { *active = best_of; return kRowSample; }
+        *active = 1;
+        return kRowSingle;
     };
     int n_adm = 0;
     auto stage_admission = [&](int slot, int64_t w, int rung) {
@@ -656,9 +676,11 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 if (i < np && std::binary_search(lang_sorted.begin(), lang_sorted.end(), p[i])) R.lang_pos = i;
             }
         }
+        int active = 1;
+        R.mode = rung_mode(R.temperature, &active);
         if (n_adm == 0) cudaEventSynchronize(s->ev_stage);   // the previous round's copies out of the pinned staging have landed
-        for (int j = 0; j < beam; ++j) {                     // beam search: `beam` identical rows start the window
-            s->h_adm_slots[n_adm] = slot * beam + j;
+        for (int j = 0; j < active; ++j) {                   // beam search / best-of: `active` identical rows start the window
+            s->h_adm_slots[n_adm] = slot * G + j;
             memset(s->h_adm_prompts + (size_t)n_adm * kKvMaxLen, 0, kKvMaxLen * 4);
             memcpy(s->h_adm_prompts + (size_t)n_adm * kKvMaxLen, p, (size_t)np * 4);
             s->h_adm_rp[n_adm] = R;
@@ -831,17 +853,18 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         for (int q = 0; q < Brun; ++q) {
             const int w = s->slot_window[q];
             if (w < 0) continue;
-            const int r0 = q * beam;                  // first decode row of the slot (the only one without beam search)
+            const int r0 = q * G;                     // first decode row of the slot (the only one of a single-row rung)
             const wk_decode_opts& o = opts_of(bo, w);
-            bool ended = s->h_done[r0] != 0, stopped = false;
+            bool ended = true, stopped = false;       // a group has ended when all its rows have (best-of samples end one by one)
+            for (int j = 0; j < G; ++j) ended &= s->h_done[r0 + j] != 0;
             if (!ended && bo->progress) {
                 const int nt = s->h_n_tokens[r0];
                 float sum = 0.f;
                 for (int i = 0; i < nt; ++i) sum += s->h_logprobs[(size_t)r0 * kKvMaxLen + i];
                 if (!bo->progress(bo->progress_user, w, s->h_tokens + (size_t)r0 * kKvMaxLen, nt, nt > 0 ? sum / nt : 0.f)) {
                     // callback -> false: the reference's early-stop flag ends the loop at the next token (TextDecoder.swift:733-762)
-                    std::vector<int32_t> ones(beam, 1);
-                    WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done + r0, ones.data(), beam * 4, cudaMemcpyHostToDevice, s->stream));
+                    std::vector<int32_t> ones(G, 1);
+                    WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done + r0, ones.data(), G * 4, cudaMemcpyHostToDevice, s->stream));
                     WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
                     stopped = true;              // an early-stopped window does not walk the ladder
                     ended = true;
@@ -853,8 +876,27 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             const int32_t* seq_tok = s->h_tokens + (size_t)r0 * kKvMaxLen;
             const float* seq_lp = s->h_logprobs + (size_t)r0 * kKvMaxLen;
             int seq_n = s->h_n_tokens[r0];
+            int rc = r0;                              // the row whose result the window returns
             std::vector<int32_t> btok; std::vector<float> blp;
-            if (beam > 1) {
+            int active = 1;
+            const int rmode = rung_mode(rung_temperature(o, rung), &active);
+            if (rmode == kRowSample) {
+                // best-of: MaximumLikelihoodRanker without length penalty over the samples (oracle/best_of_ref.py rank_best_of) - the sum of
+                // the row's recorded log-probs over max(sampled tokens, 1); ties go to the lowest row
+                const int P = prompt_len_of(w);
+                float best_rank = -INFINITY;
+                for (int j = 0; j < best_of; ++j) {
+                    const int rr = r0 + j;
+                    const float* lp = s->h_logprobs + (size_t)rr * kKvMaxLen;
+                    float sum = 0.f;
+                    for (int i = 0; i < s->h_n_tokens[rr]; ++i) sum += lp[i];
+                    const float rk = sum / (float)std::max(s->h_n_tokens[rr] - P, 1);
+                    if (j == 0 || rk > best_rank) { rc = rr; best_rank = rk; }
+                }
+                seq_tok = s->h_tokens + (size_t)rc * kKvMaxLen;
+                seq_lp = s->h_logprobs + (size_t)rc * kKvMaxLen;
+                seq_n = s->h_n_tokens[rc];
+            } else if (rmode == kRowBeam) {
                 // BeamSearchDecoder.finalize + MaximumLikelihoodRanker (oracle/beam_ref.py): the finished list, topped up with the live beams
                 // (best sum first) to `beam` entries; the winner maximises sum_logprob / sampled tokens
                 struct Cand { const int32_t* tok; const float* lp; int len; float score; bool live; };
@@ -887,12 +929,14 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             }
             // beam search: every beam of the window is the same forced copy through the prefill, so row r0 holds the value
             const float nsp = o.compute_no_speech_prob ? s->h_no_speech[r0] : NAN;
-            finalize_result(r, seq_tok, seq_lp, seq_n, s->h_steps[r0], s->h_first_low[r0], st, &o, rung_temperature(o, rung),
+            finalize_result(r, seq_tok, seq_lp, seq_n, s->h_steps[rc], s->h_first_low[rc], st, &o, rung_temperature(o, rung),
                             isnan(nsp) ? 0.f : nsp);
-            if (s->h_error[r0]) {
-                set_error("window %d: no finite logit at decoder step %d", w, s->h_steps[r0] - 1);
+            int err_row = -1;                         // a row of the rung without a finite logit fails the window
+            for (int j = 0; j < active && err_row < 0; ++j) if (s->h_error[r0 + j]) err_row = r0 + j;
+            if (err_row >= 0) {
+                set_error("window %d: no finite logit at decoder step %d", w, s->h_steps[err_row] - 1);
                 fail_window(w, WK_ERR_DECODING_LOGITS_FAILED);
-            } else if (a.ladder && beam == 1 && !stopped && r.needs_fallback && s->slot_try[q] < o.temperature_fallback_count) {
+            } else if (a.ladder && (beam == 1 || best_of >= 1) && !stopped && r.needs_fallback && s->slot_try[q] < o.temperature_fallback_count) {
                 // decodeWithFallback (TranscribeTask.swift:316-411): same encoder output (the slot keeps its cross K/V), next temperature
                 stage_admission(q, w, s->slot_try[q] + 1);
                 ++s->stats[3];
@@ -903,7 +947,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 s->win_no_speech[w] = nsp;
             }
             if (s->align_on && status[w] == WK_OK)
-                WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)q * kKvMaxLen * T * 2,
+                WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)rc * kKvMaxLen * T * 2,
                                               (size_t)kKvMaxLen * T * 2, cudaMemcpyDeviceToDevice, s->stream));
             s->slot_window[q] = -1;
             --live;
@@ -1243,7 +1287,7 @@ wk_status wk_session_set_encoder_output(wk_session* s, const wk_tensor* enc) {
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     s->batch = (int)enc->batch;
     s->bound_windows = s->batch;
-    s->bs.beam = 1;
+    s->bs.beam = 1; s->bs.group = 1;
     s->bp = round_up(s->batch, 16);
     // the encoder ran on the model stream; the projection reads its output on the session stream and the tensor remembers the reader
     std::lock_guard<std::mutex> lock(m->api_mu);

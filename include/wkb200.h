@@ -424,6 +424,56 @@ wk_status wk_transcription_word(const wk_transcription* t, int32_t i, wk_word* o
 wk_status wk_transcription_language(const wk_transcription* t, int32_t stream, int32_t* token, float* logprob);
 void wk_transcription_free(wk_transcription* t);
 
+/* ---- live transcription of many streams (AudioStreamTranscriber, Sources/WhisperKit/Core/Audio/AudioStreamTranscriber.swift) ----
+ * The caller pushes 16 kHz mono f32 audio per stream.  A round takes every stream whose new audio since its lastBufferSize passes
+ * transcribeCurrentBuffer's gates (:126-158: more than 1 s, and AudioProcessor.isVoiceDetected when use_vad) and runs all of them in ONE
+ * batched pass of the seek loop (TranscribeTask.run with clipTimestamps = [lastConfirmedSegmentEndSeconds], :195-206), with
+ * shouldStopEarly (:208-227) applied deterministically inside the window scheduler: a window ends at its first appended token whose
+ * history meets the rule, is finalized there and walks the temperature fallback ladder as usual.  Each stream then applies the
+ * segment confirmation of :164-192.  A stream holds its audio from the current clip start on (its unconfirmed plus untranscribed
+ * audio; all of it while nothing confirms, as in the reference). */
+typedef struct wk_streamer wk_streamer;
+typedef struct wk_stream_config {
+    int32_t required_segments_for_confirmation;   /* requiredSegmentsForConfirmation (default 2) */
+    float silence_threshold;                      /* silenceThreshold (default 0.3) */
+    int32_t compression_check_window;             /* compressionCheckWindow (default 60, >= 1) */
+    int32_t use_vad;                              /* useVAD (default 1) */
+} wk_stream_config;
+typedef struct wk_stream_state {                  /* AudioStreamTranscriber.State, the fields a server reads */
+    int64_t last_buffer_size;                     /* samples the last transcription of this stream covered */
+    float last_confirmed_segment_end_seconds;
+    int32_t n_confirmed_segments, n_unconfirmed_segments;
+    int32_t transcribed;                          /* the last round transcribed this stream */
+    int64_t pushed_samples;                       /* samples pushed so far */
+    int64_t held_samples;                         /* samples held: absolute [held_from, pushed_samples) */
+    int64_t held_from;
+    int64_t duplicate_confirmations;              /* rounds of this stream whose candidates were already confirmed (:178) */
+} wk_stream_state;
+/* One streamer per option set: opts (copied; beam_size > 1 is refused), the decoder prompt (prefillDecoderInputs), cfg.  hooks (copied;
+ * the functions and user pointer must outlive the streamer) are required with opts->word_timestamps.  Rounds run on session s, which
+ * must not be used by anything else while a round runs. */
+wk_status wk_streamer_create(wk_model* m, wk_session* s, const wk_special_tokens* st, const wk_decode_opts* opts, const int32_t* prompt,
+                             int32_t n_prompt, const wk_stream_config* cfg, const wk_tokenizer_hooks* hooks, wk_streamer** out);
+wk_status wk_streamer_add_stream(wk_streamer* t, int32_t* id);
+wk_status wk_streamer_remove_stream(wk_streamer* t, int32_t id);
+/* AudioProcessor.processBuffer (AudioProcessor.swift:907-917): appends samples; one relative energy per complete 1600-sample block
+ * counted from the start of the stream, whatever the push sizes.  Safe against a running round and against other pushes; a round holds
+ * the lock a push takes only to read its streams' sizes and energies, and copies their audio after releasing it. */
+wk_status wk_streamer_push(wk_streamer* t, int32_t id, const float* pcm, int64_t n);
+/* One round over all streams; ids[0..*n) = the streams it transcribed (cap >= number of streams is always enough).  No ready stream:
+ * no GPU work.  A failing round returns its error and changes no stream's state. */
+wk_status wk_streamer_round(wk_streamer* t, int32_t* ids, int32_t cap, int32_t* n);
+wk_status wk_streamer_state(wk_streamer* t, int32_t id, wk_stream_state* out);
+/* confirmedSegments then unconfirmedSegments of one stream, read with the wk_transcription_* accessors (words included; stream 0 for
+ * wk_transcription_language).  Free with wk_transcription_free. */
+wk_status wk_streamer_result(wk_streamer* t, int32_t id, wk_transcription** out);
+void wk_streamer_free(wk_streamer* t);
+/* AudioProcessor's public helpers as the streams use them: relative energies of the complete 1600-sample blocks of pcm
+ * (calculateRelativeEnergy against the lowest RMS of the previous <= 20 blocks, AudioProcessor.swift:724-741,907-917; the first block
+ * has no reference and is 0), and isVoiceDetected (:636-655). */
+wk_status wk_stream_relative_energy(const float* pcm, int64_t n, float* out, int64_t cap, int64_t* n_blocks);
+wk_status wk_stream_voice_detected(const float* energies, int64_t n, float next_buffer_seconds, float silence_threshold, int32_t* out);
+
 /* ---- word timestamps (SURVEY section 8f row 1) ----
  * Device side: with wk_decode_opts.word_timestamps set, every decode step also writes the mean cross-attention softmax row of the
  * model's alignment heads into row tokenIndex + 1 of a [224][1500] Float16 tensor per window - the decoder model's

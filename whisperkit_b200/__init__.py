@@ -10,7 +10,8 @@ from .api import (AudioEncoder, DecodingFallback, DecodingOptions, DecodingResul
                   FeatureExtractor, Model, SpecialTokens, TextDecoder, WhisperKit, WhisperKitConfig,
                   filter_and_sample)
 from .audio import AudioProcessor, ChannelMode  # noqa: F401
+from .streaming import AudioStreamTranscriber  # noqa: F401
 
 __all__ = ["WhisperKit", "WhisperKitConfig", "DecodingOptions", "DecodingResult", "DecodingFallback", "SpecialTokens",
            "FeatureExtractor", "AudioEncoder", "TextDecoder", "Model", "DeviceTensor", "filter_and_sample",
-           "WhisperError", "load", "AudioProcessor", "ChannelMode"]
+           "WhisperError", "load", "AudioProcessor", "ChannelMode", "AudioStreamTranscriber"]

@@ -115,6 +115,17 @@ class wk_audio_load_opts(C.Structure):
                 ("max_read_frame_size", C.c_int64), ("piece_seconds", C.c_double), ("segment_samples", C.c_int64)]
 
 
+class wk_stream_config(C.Structure):
+    _fields_ = [("required_segments_for_confirmation", C.c_int32), ("silence_threshold", C.c_float), ("compression_check_window", C.c_int32),
+                ("use_vad", C.c_int32)]
+
+
+class wk_stream_state(C.Structure):
+    _fields_ = [("last_buffer_size", C.c_int64), ("last_confirmed_segment_end_seconds", C.c_float), ("n_confirmed_segments", C.c_int32),
+                ("n_unconfirmed_segments", C.c_int32), ("transcribed", C.c_int32), ("pushed_samples", C.c_int64), ("held_samples", C.c_int64),
+                ("held_from", C.c_int64), ("duplicate_confirmations", C.c_int64)]
+
+
 SPLIT_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_char), C.c_int32, C.POINTER(C.c_int32), C.c_int32)
 DECODE_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_char), C.c_int32)
 
@@ -200,6 +211,17 @@ SYMBOLS = [
     ("wk_transcription_word", I32, [P, I32, C.POINTER(wk_word)]),
     ("wk_transcription_language", I32, [P, I32, PI32, PF32]),
     ("wk_transcription_free", None, [P]),
+    ("wk_streamer_create", I32, [P, P, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts), PI32, I32, C.POINTER(wk_stream_config),
+                                 C.POINTER(wk_tokenizer_hooks), C.POINTER(P)]),
+    ("wk_streamer_add_stream", I32, [P, PI32]),
+    ("wk_streamer_remove_stream", I32, [P, I32]),
+    ("wk_streamer_push", I32, [P, I32, P, I64]),
+    ("wk_streamer_round", I32, [P, PI32, I32, PI32]),
+    ("wk_streamer_state", I32, [P, I32, C.POINTER(wk_stream_state)]),
+    ("wk_streamer_result", I32, [P, I32, C.POINTER(P)]),
+    ("wk_streamer_free", None, [P]),
+    ("wk_stream_relative_energy", I32, [P, I64, P, I64, PI64]),
+    ("wk_stream_voice_detected", I32, [P, I64, F32, F32, PI32]),
     ("wk_model_set_alignment_heads", I32, [P, PI32, I32]),
     ("wk_session_alignment_weights", I32, [P, I32, I32, P]),
     ("wk_session_alignment_weights_f16", I32, [P, I32, I32, P, I32]),

@@ -263,4 +263,22 @@ struct ChainDesc {
 };
 wk_status decoder_chain(const ChainDesc& c, int num_sms, cudaStream_t stream);
 
+// ---- AudioStreamTranscriber.shouldStopEarly (AudioStreamTranscriber.swift:208-227) as a deterministic window stop (session.cu)
+// A window ends at its first appended, non-prefill token t whose history currentTokens = tokens[0..t] meets either rule:
+//   count > window and compressionRatio(last `window` tokens) > compression_threshold (compressionRatioThreshold ?? 0.0), or
+//   has_logprob and avg(logProbs[0..t]) < logprob_threshold (prompt log-probs are 0).
+// The result is the history cut after t, then finalize and the usual DecodingFallback; unlike a progress-callback stop, the window
+// walks the fallback ladder when its DecodingFallback asks for it.
+struct StopRule {
+    int window;
+    float compression_threshold;
+    int has_logprob;
+    float logprob_threshold;
+};
+// wk_transcribe_windows_ex with the stop rule applied to every window (stop == nullptr: wk_transcribe_windows_ex).  Single-row windows
+// only (no beam search, no best-of).
+wk_status transcribe_windows_stop(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
+                                  const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
+                                  wk_decode_result* results, const StopRule* stop);
+
 }  // namespace wk

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "kernels.h"
+#include "longform.h"
 
 using namespace wk;
 
@@ -226,38 +227,6 @@ wk_status wk_vad_chunk_all(const float* wav, int64_t n, int64_t max_chunk_len, c
 // =====================================================================================================
 // batched seek loop
 // =====================================================================================================
-struct OutWord {
-    std::string word;
-    std::vector<int32_t> tokens;
-    float start, end, probability;
-    int segment;
-};
-
-struct wk_transcription {
-    std::vector<wk_segment> segments;
-    std::vector<OutWord> words;   // .segment indexes `segments`
-    std::vector<int32_t> tokens;
-    std::vector<float> logprobs;
-    int windows = 0;
-    // per stream: the detected language of its latest window (in stream time) that detected one, and where that window started
-    std::vector<int32_t> lang; std::vector<float> lang_logprob; std::vector<int64_t> lang_at;
-};
-
-namespace {
-struct Unit {                 // one independently advancing cursor: a stream, or one VAD chunk of a stream
-    int stream;
-    const float* audio;       // start of the unit's samples
-    int64_t n;                // samples in the unit
-    int64_t offset;           // unit start inside the stream (seekOffsetIndex)
-    std::vector<int64_t> clips;
-    int clip = 0;
-    int64_t seek = 0;
-    bool done = false;
-    std::vector<wk_segment> segs;
-    std::vector<OutWord> words;   // word timings; .segment indexes `segs`
-};
-}  // namespace
-
 namespace {
 constexpr int kRoundCap = 256;   // windows per round of the stream loop (host staging: 256 x 1.92 MB pinned)
 
@@ -331,11 +300,7 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
                                    const wk_tokenizer_hooks* hooks, int32_t best_of, wk_transcription** out) {
     if (!m || !s || !audio || !n_samples || n_streams < 1 || !st || !o || !prompt || !out) { set_error("wk_transcribe_streams: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (o->word_timestamps && (!hooks || !hooks->split_to_word_tokens)) { set_error("wk_transcribe_streams: wordTimestamps needs the tokenizer's split_to_word_tokens hook"); return WK_ERR_INVALID_ARGUMENT; }
-    wk_model_info info;
-    wk_status rc = wk_model_info_get(m, &info);
-    if (rc != WK_OK) return rc;
-    const int max_batch = info.max_batch;
-    const int64_t window_padding = (int64_t)(window_clip_time * (float)kSampleRate);
+    wk_status rc;
     std::vector<Unit> units;
     for (int i = 0; i < n_streams; ++i) {
         if (n_samples[i] < 0 || (n_samples[i] > 0 && !audio[i])) { set_error("wk_transcribe_streams: stream %d invalid", i); return WK_ERR_AUDIO_PROCESSING_FAILED; }
@@ -359,13 +324,32 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
             rc = wk_prepare_seek_clips(vad_stream ? nullptr : cts, vad_stream ? 0 : n_cts, u.n, u.clips.data(), (int)u.clips.size() / 2, &nc);
             if (rc != WK_OK) return rc;
             u.clips.resize(2 * nc);
-            // a clip is live while seek < clipEnd - windowPadding (TranscribeTask.swift:118) and, as a guard the reference lacks (it would
-            // pad a negative-length window), while the seek is still inside the audio
-            u.seek = u.clips[0];
-            u.done = !(u.seek < u.clips[1] - window_padding && u.seek < u.n);
-            while (u.done && u.clip + 1 < nc) { ++u.clip; u.seek = u.clips[2 * u.clip]; u.done = !(u.seek < u.clips[2 * u.clip + 1] - window_padding && u.seek < u.n); }
             units.push_back(std::move(u));
         }
+    }
+    return seek_loop_units(m, s, units, n_streams, st, o, prompt, n_prompt, window_clip_time, max_window_seek, hooks, best_of, nullptr, true, out);
+}
+
+}  // extern "C"
+
+wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& units, int n_streams, const wk_special_tokens* st,
+                              const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt, float window_clip_time, int64_t max_window_seek,
+                              const wk_tokenizer_hooks* hooks, int32_t best_of, const StopRule* stop, bool renumber_ids, wk_transcription** out) {
+    if (o->word_timestamps && (!hooks || !hooks->split_to_word_tokens)) { set_error("wordTimestamps needs the tokenizer's split_to_word_tokens hook"); return WK_ERR_INVALID_ARGUMENT; }
+    wk_model_info info;
+    wk_status rc = wk_model_info_get(m, &info);
+    if (rc != WK_OK) return rc;
+    const int max_batch = info.max_batch;
+    const int64_t window_padding = (int64_t)(window_clip_time * (float)kSampleRate);
+    for (Unit& u : units) {
+        // a clip is live while seek < clipEnd - windowPadding (TranscribeTask.swift:118) and, as a guard the reference lacks (it would
+        // pad a negative-length window), while the seek is still inside the audio
+        const int nc = (int)u.clips.size() / 2;
+        u.clip = 0;
+        u.seek = u.clips[0];
+        u.done = !(u.seek < u.clips[1] - window_padding && u.seek < u.n);
+        while (u.done && u.clip + 1 < nc) { ++u.clip; u.seek = u.clips[2 * u.clip]; u.done = !(u.seek < u.clips[2 * u.clip + 1] - window_padding && u.seek < u.n); }
+        if (!u.done && u.seek < u.base) { set_error("seek loop: stream %d seeks to sample %lld before its first held sample %lld", u.stream, (long long)u.seek, (long long)u.base); return WK_ERR_INVALID_ARGUMENT; }
     }
     wk_transcription* T = new wk_transcription();
     T->lang.assign(n_streams, -1); T->lang_logprob.assign(n_streams, 0.f); T->lang_at.assign(n_streams, -1);
@@ -396,13 +380,13 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
             const int64_t sz = std::min<int64_t>({kWindow, u.n - u.seek, clip_end - u.seek});   // TranscribeTask.swift:121
             seg_size[k] = sz;
             valid[k] = (int32_t)sz;
-            memcpy(batch + (size_t)k * kWindow, u.audio + u.seek, (size_t)sz * sizeof(float));   // padOrTrim (zero fill happens in the mel kernel via `valid`)
+            memcpy(batch + (size_t)k * kWindow, u.audio + (u.seek - u.base), (size_t)sz * sizeof(float));   // padOrTrim (zero fill happens in the mel kernel via `valid`)
             return WK_OK;
         }, nullptr);
         wk_batch_opts bo;
         memset(&bo, 0, sizeof(bo));
         bo.opts = o; bo.n_opts = 1; bo.prompt = prompt; bo.n_prompt = n_prompt; bo.best_of = best_of;
-        rc = wk_transcribe_windows_ex(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data());
+        rc = transcribe_windows_stop(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data(), stop);
         if (rc != WK_OK) { delete T; return rc; }
         T->windows += (int)active.size();
         if (o->detect_language) {   // TranscriptionResult.language: the stream keeps the language of its last detecting window
@@ -518,7 +502,7 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
             T->words.push_back(std::move(w));
         }
         for (wk_segment sg : u.segs) {
-            sg.id = next_id[u.stream]++;
+            if (renumber_ids) sg.id = next_id[u.stream]++;
             sg.seek += u.offset;
             sg.start += seek_time;
             sg.end += seek_time;
@@ -529,6 +513,8 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
     *out = T;
     return WK_OK;
 }
+
+extern "C" {
 
 int32_t wk_transcription_segment_count(const wk_transcription* t) { return t ? (int32_t)t->segments.size() : 0; }
 int32_t wk_transcription_window_count(const wk_transcription* t) { return t ? t->windows : 0; }

@@ -16,6 +16,7 @@
 #include <zlib.h>
 
 #include <algorithm>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -267,6 +268,45 @@ static float compression_ratio(const std::vector<int32_t>& toks) {
     return (float)n / (float)clen;
 }
 
+// the same ratio on one deflate state kept across calls (deflateReset instead of a fresh deflateInit2: same output, no allocation) -
+// the stream stop rule evaluates it once per decoded token
+namespace {
+struct Deflater {
+    z_stream zs;
+    bool ok = false;
+    std::vector<unsigned char> out;
+    Deflater() { memset(&zs, 0, sizeof(zs)); ok = deflateInit2(&zs, 5, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) == Z_OK; }
+    ~Deflater() { if (ok) deflateEnd(&zs); }
+    Deflater(const Deflater&) = delete;
+    Deflater& operator=(const Deflater&) = delete;
+    float ratio(const int32_t* toks, int n) {
+        if (n <= 0 || !ok || deflateReset(&zs) != Z_OK) return INFINITY;
+        const uLong bytes = (uLong)n * 4;
+        out.resize(deflateBound(&zs, bytes) + 64);
+        zs.next_in = (Bytef*)toks; zs.avail_in = (uInt)bytes;
+        zs.next_out = out.data(); zs.avail_out = (uInt)out.size();
+        const int r = deflate(&zs, Z_FINISH);
+        const uLong clen = zs.total_out;
+        if (r != Z_STREAM_END || clen == 0) return INFINITY;
+        return (float)bytes / (float)clen;
+    }
+};
+}  // namespace
+
+// AudioStreamTranscriber.shouldStopEarly (AudioStreamTranscriber.swift:208-227) over history entries [from, n): the first index t >= P
+// (a token the loop appended, so a callback that may stop, TextDecoder.swift:732-751) whose history tokens[0..t] meets the rule, else -1.
+// *sum carries logProbs.reduce(0, +) over [0, from) and is advanced in the same order
+static int stop_rule_index(const StopRule& rule, Deflater& z, const int32_t* tok, const float* lp, int from, int n, int P, float* sum) {
+    for (int i = from; i < n; ++i) {
+        *sum += lp[i];
+        if (i < P) continue;
+        const int count = i + 1;
+        if (count > rule.window && z.ratio(tok + count - rule.window, rule.window) > rule.compression_threshold) return i;
+        if (rule.has_logprob && *sum / (float)count < rule.logprob_threshold) return i;
+    }
+    return -1;
+}
+
 // finalisation of one window on the host: finalize + slicing + averages (TextDecoder.swift:776-853)
 static void finalize_result(wk_decode_result& r, const int32_t* tokens, const float* lps, int n_tok, int steps, int first_low,
                             const wk_special_tokens* st, const wk_decode_opts* o, float temperature, float no_speech_prob) {
@@ -405,6 +445,7 @@ struct CoreArgs {
     const float* pcm; int64_t n; int64_t stride; const int32_t* spw;   // pcm == nullptr: windows are the session's bound rows (decodeText)
     const wk_special_tokens* st; const wk_batch_opts* bo; wk_decode_result* results;
     bool ladder;
+    const StopRule* stop = nullptr;   // stream stop rule (transcribe_windows_stop); nullptr: windows end on their own or by callback
 };
 
 static const wk_decode_opts& opts_of(const wk_batch_opts* bo, int64_t w) { return bo->n_opts == 1 ? bo->opts[0] : bo->opts[w]; }
@@ -486,6 +527,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         set_error("%d rows per window (beam size %d, best_of %d) exceed the session's %d rows", G, beam, best_of, s->max_batch);
         return WK_ERR_INVALID_ARGUMENT;
     }
+    if (a.stop && (G != 1 || a.stop->window < 1)) { set_error("the stream stop rule needs single-row windows and a check window >= 1"); return WK_ERR_INVALID_ARGUMENT; }
     int max_cand = 0;
     if (beam > 1) {
         const float patience = bo->opts[0].beam_patience > 0.f ? bo->opts[0].beam_patience : 1.f;
@@ -623,6 +665,10 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     const int rows = s->batch;
     s->slot_window.assign(S, -1);
     s->slot_try.assign(S, 0);
+    // stream stop rule: per slot, the history entries already checked and the running log-prob sum over them
+    std::vector<int> stop_checked(a.stop ? S : 0, 0);
+    std::vector<float> stop_sum(a.stop ? S : 0, 0.f);
+    std::unique_ptr<Deflater> stop_deflater(a.stop ? new Deflater() : nullptr);   // zlib state only when the rule is on
     {   // every slot starts free: done = 1 keeps its rows out of the step until a window is admitted
         std::vector<int32_t> ones(s->max_batch, 1);
         WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done, ones.data(), s->max_batch * 4, cudaMemcpyHostToDevice, s->stream));
@@ -688,6 +734,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         }
         s->slot_window[slot] = (int)w;
         s->slot_try[slot] = rung;
+        if (a.stop) { stop_checked[slot] = 0; stop_sum[slot] = 0.f; }
     };
     auto prompt_len_of = [&](int64_t w) -> int { const int32_t* p; int np; prompt_of(w, &p, &np); return np; };
     auto flush_admissions = [&]() -> wk_status {
@@ -857,6 +904,20 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             const wk_decode_opts& o = opts_of(bo, w);
             bool ended = true, stopped = false;       // a group has ended when all its rows have (best-of samples end one by one)
             for (int j = 0; j < G; ++j) ended &= s->h_done[r0 + j] != 0;
+            int stop_at = -1;                         // stream stop rule: history index of the token the window stops at
+            if (a.stop) {
+                // every history entry since the last check (the history is causal: steps run past the stopping token are only lost time)
+                const int nt = s->h_n_tokens[r0];
+                stop_at = stop_rule_index(*a.stop, *stop_deflater, s->h_tokens + (size_t)r0 * kKvMaxLen, s->h_logprobs + (size_t)r0 * kKvMaxLen,
+                                          stop_checked[q], nt, prompt_len_of(w), &stop_sum[q]);
+                stop_checked[q] = nt;
+                if (stop_at >= 0 && !ended) {
+                    const int32_t one = 1;
+                    WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done + r0, &one, 4, cudaMemcpyHostToDevice, s->stream));
+                    WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
+                    ended = true;
+                }
+            }
             if (!ended && bo->progress) {
                 const int nt = s->h_n_tokens[r0];
                 float sum = 0.f;
@@ -927,9 +988,11 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 btok.assign(cd.tok, cd.tok + body); blp.assign(cd.lp, cd.lp + body);
                 seq_tok = btok.data(); seq_lp = blp.data(); seq_n = body;
             }
+            // stream stop rule: the history cut after the stopping token (appended at step stop_at - 1), then the usual finalize
+            if (stop_at >= 0) seq_n = stop_at + 1;
             // beam search: every beam of the window is the same forced copy through the prefill, so row r0 holds the value
             const float nsp = o.compute_no_speech_prob ? s->h_no_speech[r0] : NAN;
-            finalize_result(r, seq_tok, seq_lp, seq_n, s->h_steps[rc], s->h_first_low[rc], st, &o, rung_temperature(o, rung),
+            finalize_result(r, seq_tok, seq_lp, seq_n, stop_at >= 0 ? stop_at : s->h_steps[rc], s->h_first_low[rc], st, &o, rung_temperature(o, rung),
                             isnan(nsp) ? 0.f : nsp);
             int err_row = -1;                         // a row of the rung without a finite logit fails the window
             for (int j = 0; j < active && err_row < 0; ++j) if (s->h_error[r0 + j]) err_row = r0 + j;
@@ -946,6 +1009,9 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 if (any_detect) { s->win_lang[w] = s->h_lang_token[r0]; s->win_lang_logprob[w] = s->h_lang_logprob[r0]; }   // the returned rung's
                 s->win_no_speech[w] = nsp;
             }
+            if (s->align_on && status[w] == WK_OK && stop_at >= 0)   // rows of the steps run past the stopping token: the reference never ran them
+                WK_CUDA_CHECK(cudaMemsetAsync((char*)s->align_w + ((size_t)rc * kKvMaxLen + stop_at + 1) * T * 2, 0,
+                                              (size_t)(kKvMaxLen - stop_at - 1) * T * 2, s->stream));
             if (s->align_on && status[w] == WK_OK)
                 WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)rc * kKvMaxLen * T * 2,
                                               (size_t)kKvMaxLen * T * 2, cudaMemcpyDeviceToDevice, s->stream));
@@ -1395,15 +1461,25 @@ wk_status wk_decode_text(wk_session* s, const wk_special_tokens* st, const wk_de
 wk_status wk_transcribe_windows_ex(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
                                    const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
                                    wk_decode_result* results) {
+    return wk::transcribe_windows_stop(m, s, pcm_host, n_windows, stride, samples_per_window, st, bo, results, nullptr);
+}
+
+}  // extern "C"
+
+wk_status wk::transcribe_windows_stop(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
+                                      const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
+                                      wk_decode_result* results, const StopRule* stop) {
     if (!m || !s || !pcm_host || !st || !bo || !bo->opts || bo->n_opts < 1 || !results || n_windows < 1) { set_error("wk_transcribe_windows: null argument"); return WK_ERR_INVALID_ARGUMENT; }
     if (s->m != m) { set_error("wk_transcribe_windows: session belongs to another model"); return WK_ERR_INVALID_ARGUMENT; }
     if (bo->n_opts != 1 && bo->n_opts != n_windows) { set_error("wk_transcribe_windows: %d option sets for %lld windows", bo->n_opts, (long long)n_windows); return WK_ERR_INVALID_ARGUMENT; }
     if (bo->prompts && !bo->prompt_lens) { set_error("wk_transcribe_windows: prompts without prompt_lens"); return WK_ERR_INVALID_ARGUMENT; }
     if (!m->finalized) { set_error("wk_transcribe_windows: model weights not finalized"); return WK_ERR_MODELS_UNAVAILABLE; }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
-    CoreArgs a{pcm_host, n_windows, stride, samples_per_window, st, bo, results, true};
+    CoreArgs a{pcm_host, n_windows, stride, samples_per_window, st, bo, results, true, stop};
     return transcribe_core(s, a);
 }
+
+extern "C" {
 
 wk_status wk_transcribe_windows(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
                                 const int32_t* samples_per_window, const wk_special_tokens* st, const wk_decode_opts* opts,

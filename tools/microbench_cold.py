@@ -1,5 +1,5 @@
 """HBM-cold timings (weights rotating over the 32 layers, CUDA-graph replay) of the decoder's latency-bound pieces at the benchmarked
-shape: the swap-AB GEMMs one launch at a time, the split-K reduce, self-attention, and the fused phase chains that replace them.
+shape: the swap-AB GEMMs one launch at a time, the split-K reduce, self-attention and cross-attention.
 
     python tools/microbench_cold.py [batch]
 """
@@ -17,11 +17,9 @@ if __name__ == "__main__":
     m.init_random(1)
     dec = wk.TextDecoder(m, B)
     names = {14: "d x d GEMM (out / cross-Q / cross-out)", 17: "QKV GEMM", 15: "FC1 GEMM", 16: "FC2 GEMM", 8: "split-K reduce + LN",
-             9: "self-attention @ pos 100", 0: "cross-attention", 18: "chain B (out-proj > LN > cross-Q)",
-             19: "chain C (cross-out > LN > FC1 > GELU > FC2 > LN > QKV)"}
+             9: "self-attention @ pos 100", 0: "cross-attention"}
     f, w = C.c_float(), C.c_double()
     for k, n in names.items():
         check(m.lib.wk_bench_kernel(m.handle, dec.handle, k, B, 192, C.byref(f), C.byref(w)))
         gbs = w.value / (f.value * 1e-3) / 1e9 if w.value else 0.0
         print(f"{n:58s} {f.value * 1000:8.2f} us   {gbs:8.0f} GB/s of algorithmic bytes", flush=True)
-    # per-layer sums: 6 GEMMs + 3 reduce+LN + 1 reduce+GELU (~ reduce+LN) launched one by one, against the two chains

@@ -16,7 +16,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 BUILD = os.path.join(PKG, "_build")
 LIB = os.path.join(PKG, "libwkb200.so")
-SOURCES = ["gemm_wgmma.cu", "attention_wgmma.cu", "mel.cu", "encoder_ops.cu", "decoder_ops.cu", "cross_attention_mq.cu", "align_pass.cu", "engine.cu", "session.cu", "longform.cu", "wordtiming.cu", "tokenizer.cu", "fused_chain.cu", "writers.cu", "comm.cu", "audio.cu", "streaming.cu"]
+SOURCES = ["gemm_wgmma.cu", "attention_wgmma.cu", "mel.cu", "encoder_ops.cu", "decoder_ops.cu", "cross_attention_mq.cu", "align_pass.cu", "engine.cu", "session.cu", "longform.cu", "wordtiming.cu", "tokenizer.cu", "writers.cu", "comm.cu", "audio.cu", "streaming.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--use_fast_math=false",

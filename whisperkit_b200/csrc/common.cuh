@@ -155,8 +155,8 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
-// Bounded wait for kernels whose CTAs wait on each other (grid-wide barriers): a protocol bug must end as a trapped launch that the
-// host reports, never as a GPU that spins until something kills the process.  2 s is >1000x the longest legitimate wait.
+// Bounded mbarrier wait: a protocol bug must end as a trapped launch that the host reports, never as a GPU that spins until something
+// kills the process.  2 s is >1000x the longest legitimate wait.
 constexpr unsigned long long kSpinLimitNs = 2000000000ull;
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
@@ -173,12 +173,6 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1,
                                             int c2) {

@@ -4,7 +4,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <atomic>
 #include <mutex>
 #include <vector>
 
@@ -110,7 +109,6 @@ struct wk_model {
     std::vector<uint32_t> align_mask; std::vector<int> align_base; int n_align_slots = 0; int has_alignment_heads = 0;
     float timings[6] = {0, 0, 0, 0, 0, 0};
     cudaEvent_t ev[8];
-    std::atomic<int> live_sessions{0};
     // cross-attention K/V cache storage: the model dtype, or FP8 E4M3 with per-row scales (wk_model_set_cross_kv_dtype); fixed once the
     // first session exists.  Both fields are read and written under api_mu.
     bool cross_kv_fp8 = false;

@@ -486,14 +486,6 @@ static wk_status make_tmap(CUtensorMap* tm, const void* base, int dtype, int ndi
     return WK_OK;
 }
 
-// 2-D, 128-byte-swizzled, 16-bit tensor map over a row-major [rows][ld] matrix with a [box_rows][box_cols] box (used by fused_chain.cu)
-wk_status make_tmap_2d(void* tm, const void* base, int dtype, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_cols, uint32_t box_rows) {
-    uint64_t dims[2] = {cols, rows};
-    uint64_t str[1] = {ld_elems * 2};
-    uint32_t box[2] = {box_cols, box_rows};
-    return make_tmap(reinterpret_cast<CUtensorMap*>(tm), base, dtype, 2, dims, str, box);
-}
-
 int wgmma_tile_n(int bn) {
     int t = 16;
     while (t < bn) t <<= 1;

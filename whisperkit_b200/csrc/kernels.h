@@ -237,32 +237,6 @@ wk_status align_rows_f16(const float* acc, const int32_t* seq_len, int n_slots, 
 wk_status align_token_logprobs(const float* logits, int64_t ld, int64_t r0, int64_t rows, const int32_t* row_tok, const int32_t* seq_len, int eot,
                                float* out, cudaStream_t stream);
 
-// ---- a chain of decoder GEMM / split-K reduce phases in ONE persistent kernel with grid-wide barriers between the phases instead of
-// kernel boundaries (fused_chain.cu)
-wk_status make_tmap_2d(void* tm, const void* base, int dtype, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_cols, uint32_t box_rows);
-constexpr int kChainMaxPhases = 7;
-constexpr int kChainMaxGemms = 4;
-struct ChainPhaseDesc {
-    int kind;                  // 0 swap-AB split-K GEMM -> partials; 1 reduce + bias + residual + LayerNorm; 2 reduce + bias + GELU
-    // kind 0
-    const void* w; int n, k;   // weights [n][k]
-    const void* act;           // activations [Bp][k], 16-bit
-    int splits;
-    // kind 1 / 2 (reduce the partials of the GEMM phase before it)
-    const float* bias; const float* gamma; const float* beta;
-    void* out16;               // LN output / GELU output, 16-bit [B][row length]
-};
-struct ChainDesc {
-    int n_phases;
-    ChainPhaseDesc ph[kChainMaxPhases];
-    float* partial; float* x;  // split-K workspace, f32 residual stream [Bp][d]
-    int B, Bp, d, dtype;
-    unsigned int* counters;    // 8 words, zero before the launch: one per phase boundary
-    unsigned int* reset_counters;  // 8 words of the sibling chain (already completed): zeroed by this launch; may be nullptr
-    int pdl;
-};
-wk_status decoder_chain(const ChainDesc& c, int num_sms, cudaStream_t stream);
-
 // ---- AudioStreamTranscriber.shouldStopEarly (AudioStreamTranscriber.swift:208-227) as a deterministic window stop (session.cu)
 // A window ends at its first appended, non-prefill token t whose history currentTokens = tokens[0..t] meets either rule:
 //   count > window and compressionRatio(last `window` tokens) > compression_threshold (compressionRatioThreshold ?? 0.0), or

@@ -61,7 +61,7 @@ struct wk_session {
     // step graph, cached across calls: the step depends on the call only through the rows it covers, the alignment export and the
     // special-token ids baked into the sampler's parameters
     cudaGraphExec_t graph_exec = nullptr, graph_exec_live = nullptr;   // the step with / without the ended-row checks in the attention kernels
-    int graph_batch = 0; bool graph_align = false, graph_fused = false; wk_special_tokens graph_st; long long launches_per_step = 0;
+    int graph_batch = 0; bool graph_align = false; wk_special_tokens graph_st; long long launches_per_step = 0;
     bool warmed = false;
     // word timestamps: per-head softmax rows of the current step, the [S][224][T] Float16 alignmentWeights of the slots, and the per-window
     // copies handed out by wk_session_alignment_weights
@@ -75,9 +75,7 @@ struct wk_session {
     float *al_acc = nullptr, *al_stats = nullptr, *al_lp = nullptr, *al_bqkv = nullptr;
     int32_t *al_tok = nullptr, *al_seq = nullptr;
     std::vector<float> win_align_lp;
-    unsigned int* chain_counters = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_adm = nullptr, ev_stage = nullptr, ev_t[10];
-    bool knob_fused = false, knob_graph = true;
     // beam search (allocated on the first call that asks for it)
     BeamState bs = BeamState(); int bs_cap_rows = 0;
     int32_t *h_n_fin = nullptr, *h_fin_len = nullptr, *h_fin_tokens = nullptr; float *h_fin_score = nullptr, *h_fin_lps = nullptr, *h_sum_lp = nullptr;
@@ -125,12 +123,8 @@ static GemmDesc cross_kv_gemm(const wk_session* s, const void* src, int cnt, int
     return g;
 }
 
-// The fused phase chains hold every SM with a CTA that waits on grid-wide barriers.  Two such grids from different sessions could each
-// take half of the machine and wait for the other half forever, so a session only uses them while it is the model's sole live session.
-static bool use_fused(const wk_session* s) { return s->knob_fused && s->m->live_sessions.load(std::memory_order_relaxed) == 1; }
-
 // one decoder forward for every row of the step.  explicit_pos == nullptr: loop mode (token / position from DecodeState, ended rows skipped)
-static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* explicit_pos, bool fused, bool check_done = true) {
+static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* explicit_pos, bool check_done = true) {
     wk_model* m = s->m;
     const wk_model_config& c = m->cfg;
     const int d = c.d_model, H = c.n_heads, dt = c.dtype, B = s->batch, Bp = s->bp, T = c.n_audio_ctx;
@@ -160,68 +154,21 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
                                        kv_div, s->ckv_fp8 ? s->cross_scale + (2 * li) * cross_rows : nullptr,
                                        s->ckv_fp8 ? s->cross_scale + (2 * li + 1) * cross_rows : nullptr);
     };
-    if (fused) {
-        // per layer: self-attention -> chain B (out-proj, reduce+LN, cross-Q) -> cross-attention -> chain C (cross-out, reduce+LN, FC1,
-        // reduce+GELU, FC2, reduce+LN, next layer's QKV): phases of one persistent kernel separated by grid barriers (fused_chain.cu)
-        const int kWords = 8;
-        auto gemm_phase = [&](const void* w, int N, int K, const void* act) {
-            ChainPhaseDesc ph; memset(&ph, 0, sizeof(ph));
-            ph.kind = 0; ph.w = w; ph.n = N; ph.k = K; ph.act = act; ph.splits = choose_splits((N + 127) / 128, K / 64, m->num_sms);
-            return ph;
-        };
-        auto ln_phase = [&](const float* bias, const LayerNormW& ln) {
-            ChainPhaseDesc ph; memset(&ph, 0, sizeof(ph));
-            ph.kind = 1; ph.bias = bias; ph.gamma = ln.g; ph.beta = ln.b; ph.out16 = s->xn;
-            return ph;
-        };
-        auto chain_base = [&](int li, int which) {
-            ChainDesc cd; memset(&cd, 0, sizeof(cd));
-            cd.partial = s->partial; cd.x = s->x; cd.B = B; cd.Bp = Bp; cd.d = d; cd.dtype = dt; cd.pdl = 1;
-            cd.counters = s->chain_counters + ((size_t)li * 2 + which) * kWords;
-            cd.reset_counters = s->chain_counters + ((size_t)li * 2 + (which ^ 1)) * kWords;   // the sibling chain re-arms this one's words
-            return cd;
-        };
-        WK_CHECK(dec_gemm(s, m->dec[0].wqkv, 3 * d, d, s->xn, &sp));
-        for (int li = 0; li < n_layers; ++li) {
-            DecLayer& l = m->dec[li];
-            WK_CHECK(self_attn(li, l));
-            ChainDesc cb = chain_base(li, 0);
-            cb.ph[0] = gemm_phase(l.wo, d, d, s->attn);
-            cb.ph[1] = ln_phase(l.bo, l.lnx);
-            cb.ph[2] = gemm_phase(l.wcq, d, d, s->xn);
-            cb.n_phases = 3;
-            WK_CHECK(decoder_chain(cb, m->num_sms, st));
-            sp = cb.ph[2].splits;
-            WK_CHECK(cross_attn(li, l));
-            ChainDesc cc = chain_base(li, 1);
-            const LayerNormW& nxt = (li + 1 < n_layers) ? m->dec[li + 1].ln1 : m->dec_ln;
-            cc.ph[0] = gemm_phase(l.wco, d, d, s->attn);
-            cc.ph[1] = ln_phase(l.bco, l.ln3);
-            cc.ph[2] = gemm_phase(l.w1, 4 * d, d, s->xn);
-            cc.ph[3].kind = 2; cc.ph[3].bias = l.b1; cc.ph[3].out16 = s->ffn;
-            cc.ph[4] = gemm_phase(l.w2, d, 4 * d, s->ffn);
-            cc.ph[5] = ln_phase(l.b2, nxt);
-            cc.n_phases = 6;
-            if (li + 1 < n_layers) { cc.ph[6] = gemm_phase(m->dec[li + 1].wqkv, 3 * d, d, s->xn); cc.n_phases = 7; sp = cc.ph[6].splits; }
-            WK_CHECK(decoder_chain(cc, m->num_sms, st));
-        }
-    } else {
-        for (int li = 0; li < n_layers; ++li) {
-            DecLayer& l = m->dec[li];
-            WK_CHECK(dec_gemm(s, l.wqkv, 3 * d, d, s->xn, &sp));
-            WK_CHECK(self_attn(li, l));
-            WK_CHECK(dec_gemm(s, l.wo, d, d, s->attn, &sp));
-            WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.bo, l.lnx.g, l.lnx.b, s->x, s->xn, B, d, dt, st));
-            WK_CHECK(dec_gemm(s, l.wcq, d, d, s->xn, &sp));
-            WK_CHECK(cross_attn(li, l));
-            WK_CHECK(dec_gemm(s, l.wco, d, d, s->attn, &sp));
-            WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.bco, l.ln3.g, l.ln3.b, s->x, s->xn, B, d, dt, st));
-            WK_CHECK(dec_gemm(s, l.w1, 4 * d, d, s->xn, &sp));
-            WK_CHECK(decoder_reduce_bias_gelu(s->partial, sp, Bp, l.b1, s->ffn, B, 4 * d, dt, st));
-            WK_CHECK(dec_gemm(s, l.w2, d, 4 * d, s->ffn, &sp));
-            const LayerNormW& nxt = (li + 1 < n_layers) ? m->dec[li + 1].ln1 : m->dec_ln;
-            WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.b2, nxt.g, nxt.b, s->x, s->xn, B, d, dt, st));
-        }
+    for (int li = 0; li < n_layers; ++li) {
+        DecLayer& l = m->dec[li];
+        WK_CHECK(dec_gemm(s, l.wqkv, 3 * d, d, s->xn, &sp));
+        WK_CHECK(self_attn(li, l));
+        WK_CHECK(dec_gemm(s, l.wo, d, d, s->attn, &sp));
+        WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.bo, l.lnx.g, l.lnx.b, s->x, s->xn, B, d, dt, st));
+        WK_CHECK(dec_gemm(s, l.wcq, d, d, s->xn, &sp));
+        WK_CHECK(cross_attn(li, l));
+        WK_CHECK(dec_gemm(s, l.wco, d, d, s->attn, &sp));
+        WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.bco, l.ln3.g, l.ln3.b, s->x, s->xn, B, d, dt, st));
+        WK_CHECK(dec_gemm(s, l.w1, 4 * d, d, s->xn, &sp));
+        WK_CHECK(decoder_reduce_bias_gelu(s->partial, sp, Bp, l.b1, s->ffn, B, 4 * d, dt, st));
+        WK_CHECK(dec_gemm(s, l.w2, d, 4 * d, s->ffn, &sp));
+        const LayerNormW& nxt = (li + 1 < n_layers) ? m->dec[li + 1].ln1 : m->dec_ln;
+        WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.b2, nxt.g, nxt.b, s->x, s->xn, B, d, dt, st));
     }
     // logits = xn . E^T  (tied embedding), written [B][V] f32 by the transposed-store epilogue (splits = 1)
     {
@@ -376,9 +323,9 @@ static wk_status build_prompt(const wk_model* m, const wk_special_tokens* st, co
 }
 
 // ---------------------------------------------------------------------------------------------- the step and its graph
-static wk_status enqueue_step(wk_session* s, const wk_special_tokens* st, bool fused, bool check_done) {
+static wk_status enqueue_step(wk_session* s, const wk_special_tokens* st, bool check_done) {
     wk_model* m = s->m;
-    WK_CHECK(decoder_forward(s, st->time_token_begin, nullptr, fused, check_done));
+    WK_CHECK(decoder_forward(s, st->time_token_begin, nullptr, check_done));
     WK_CHECK(sampler_filter_sample(s->logits, m->cfg.vocab, loop_sampler_params(s, st), s->st, nullptr, 0, nullptr, nullptr, nullptr, nullptr, s->batch, s->stream));
     if (s->bs.beam > 1) WK_CHECK(beam_update(s->st, s->bs, *st, kKvMaxLen, s->batch / s->bs.group, s->stream));
     if (s->align_on)
@@ -390,23 +337,22 @@ static wk_status enqueue_step(wk_session* s, const wk_special_tokens* st, bool f
 // runs `n` decode steps on the session stream (CUDA graph replay; the first step of a session runs eagerly so that lazily loaded
 // kernels and function attributes exist before a capture)
 static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bool all_live) {
-    const bool fused = use_fused(s);
     const bool check_done = !all_live;
     int done = 0;
-    if (!s->knob_graph || !s->warmed) {
-        const int eager = s->knob_graph ? 1 : n;
-        for (; done < eager && done < n; ++done) WK_CHECK(enqueue_step(s, st, fused, check_done));
+    if (!s->warmed) {
+        WK_CHECK(enqueue_step(s, st, check_done));
+        ++done;
         s->warmed = true;
     }
     if (done >= n) return WK_OK;
     // the step's shape depends on the rows per window (cross K/V sharing) and on whether the call has beam rows (ancestry, beam_update)
     const int beam_key = (std::max(1, s->bs.group) * 16 + std::max(1, s->bs.beam)) * 16 + s->bs.max_candidates;
-    const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_fused != fused || s->graph_beam != beam_key ||
+    const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_beam != beam_key ||
                        memcmp(&s->graph_st, st, sizeof(*st)) != 0;
     if (stale) {
         if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }
         if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
-        s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_fused = fused; s->graph_st = *st; s->graph_beam = beam_key;
+        s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_st = *st; s->graph_beam = beam_key;
     }
     cudaGraphExec_t& exec = check_done ? s->graph_exec : s->graph_exec_live;
     if (!exec) {
@@ -414,7 +360,7 @@ static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bo
             cudaGraph_t graph = nullptr;
             const long long before = launch_counter_load();
             WK_CUDA_CHECK(cudaStreamBeginCapture(s->stream, cudaStreamCaptureModeThreadLocal));
-            wk_status r = enqueue_step(s, st, fused, check_done);
+            wk_status r = enqueue_step(s, st, check_done);
             cudaError_t e = cudaStreamEndCapture(s->stream, &graph);
             s->launches_per_step = launch_counter_load() - before;
             launch_counter_sub(s->launches_per_step);  // captured, not executed
@@ -1216,11 +1162,6 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     wk_session* s = new wk_session();
     s->m = m;
     s->max_batch = S;
-    // A/B switches, read once per session (never on the step path).  WKB200_FUSED=1 runs the decoder's GEMM / reduce phases as persistent
-    // chains with grid barriers (fused_chain.cu): bit-identical, but a phase costs dependent L2 round trips
-    // either way and a grid barrier is no cheaper than a programmatic kernel boundary, so it is off by default.  WKB200_NO_GRAPH=1 replays nothing.
-    if (const char* e = getenv("WKB200_FUSED")) s->knob_fused = atoi(e) != 0;
-    s->knob_graph = getenv("WKB200_NO_GRAPH") == nullptr;
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&s->enc_stream, cudaStreamNonBlocking));
     const int bpm = round_up(S, 16);
@@ -1275,7 +1216,6 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CHECK(dmalloc(&s->d_adm_slots, S));
     WK_CHECK(dmalloc(&s->d_adm_prompts, (size_t)S * kKvMaxLen));
     WK_CHECK(dmalloc(&s->d_adm_rp, S));
-    WK_CHECK(dmalloc(&s->chain_counters, (size_t)L * 2 * 8));
     auto pinned = [&](void** p, size_t bytes) -> wk_status {
         cudaError_t e = cudaHostAlloc(p, bytes, cudaHostAllocDefault);
         if (e != cudaSuccess) { set_error("cudaHostAlloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return WK_ERR_CUDA; }
@@ -1304,7 +1244,6 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CUDA_CHECK(cudaEventRecord(s->ev_stage, s->stream));
     s->slot_window.assign(S, -1);
     s->slot_try.assign(S, 0);
-    m->live_sessions.fetch_add(1);
     *out = s;
     return WK_OK;
 }
@@ -1314,14 +1253,13 @@ void wk_session_free(wk_session* s) {
     cudaSetDevice(s->m->device);
     cudaStreamSynchronize(s->stream);
     cudaStreamSynchronize(s->enc_stream);
-    s->m->live_sessions.fetch_sub(1);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     if (s->graph_exec_live) cudaGraphExecDestroy(s->graph_exec_live);
     void* ptrs[] = {s->cross_kv, s->cross_scale, s->self_k, s->self_v, s->partial, s->x, s->xn, s->attn, s->ffn, s->logits, s->st.tokens, s->st.n_tokens,
                     s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error,
                     s->st.lang_token, s->st.lang_logprob, s->st.lang_state, s->st.no_speech, s->rp_dev,
                     s->pos_dev, s->lang_dev, s->suppress_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, s->align_scratch, s->align_w,
-                    s->align_store, s->chain_counters, s->al_acc, s->al_stats, s->al_lp, s->al_bqkv, s->al_tok, s->al_seq};
+                    s->align_store, s->al_acc, s->al_stats, s->al_lp, s->al_bqkv, s->al_tok, s->al_seq};
     for (void* p : ptrs) if (p) cudaFree(p);
     void* hptrs[] = {s->h_adm_slots, s->h_adm_prompts, s->h_adm_rp, s->h_tokens, s->h_logprobs, s->h_n_tokens, s->h_done, s->h_first_low, s->h_steps, s->h_error,
                      s->h_lang_token, s->h_lang_logprob, s->h_no_speech};
@@ -1387,7 +1325,7 @@ wk_status wk_decode_step(wk_session* s, const int32_t* input_ids, const int32_t*
     }
     WK_CUDA_CHECK(cudaMemcpyAsync(s->st.input_ids, input_ids, s->batch * 4, cudaMemcpyHostToDevice, s->stream));
     WK_CUDA_CHECK(cudaMemcpyAsync(s->pos_dev, cache_length, s->batch * 4, cudaMemcpyHostToDevice, s->stream));
-    WK_CHECK(decoder_forward(s, 0, s->pos_dev, use_fused(s)));
+    WK_CHECK(decoder_forward(s, 0, s->pos_dev));
     if (logits_out)
         WK_CUDA_CHECK(cudaMemcpyAsync(logits_out, s->logits, (size_t)s->batch * m->cfg.vocab * 4, cudaMemcpyDeviceToHost, s->stream));
     cudaError_t e = cudaStreamSynchronize(s->stream);
@@ -1418,7 +1356,7 @@ wk_status wk_detect_language(wk_session* s, const wk_special_tokens* st, const i
     std::vector<int32_t> ids(B, st->start_of_transcript_token), zeros(B, 0), ones(B, 1);
     WK_CUDA_CHECK(cudaMemcpyAsync(s->st.input_ids, ids.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
     WK_CUDA_CHECK(cudaMemcpyAsync(s->pos_dev, zeros.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
-    WK_CHECK(decoder_forward(s, 0, s->pos_dev, use_fused(s)));
+    WK_CHECK(decoder_forward(s, 0, s->pos_dev));
     // currentTokens = [SOT] for every window: reuse the decode-state arrays as the stateless token history
     WK_CUDA_CHECK(cudaMemcpyAsync(s->st.tokens, ids.data(), B * 4, cudaMemcpyHostToDevice, s->stream));   // ld_tokens = 1
     WK_CUDA_CHECK(cudaMemcpyAsync(s->st.n_tokens, ones.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
@@ -1574,7 +1512,6 @@ wk_status wk_session_aligned_logprobs(const wk_session* s, int32_t window, int32
 //   3 encoder attention      4 decoder QKV swap-AB GEMM      5 encoder QKV GEMM      6/7 decoder d x d / FC2 GEMM (L2-warm weights)
 //   8 split-K reduce + LN    9 decoder self-attention at position 100      10 sampler (V-long rows)
 //   14-17 decoder GEMMs with the weights rotating over the layers (HBM-cold: d x d, FC1, FC2, QKV)
-//   18 / 19 the fused phase chains B / C of one layer, weights rotating over the layers
 // Also returns the algorithmic bytes (HBM-bound kernels) or FLOPs (tensor-bound) of one launch.
 wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t batch, int32_t iters, float* ms_out, double* work_out) {
     if (!m || !s || s->m != m || !ms_out || !work_out || iters < 1) return WK_ERR_INVALID_ARGUMENT;
@@ -1596,22 +1533,6 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
     static int32_t* pos100 = nullptr;
     if (which == 9 && !pos100) { std::vector<int32_t> h(256, 100); cudaMalloc(&pos100, 256 * 4); cudaMemcpy(pos100, h.data(), 256 * 4, cudaMemcpyHostToDevice); }
     int rot = 0;
-    auto chain_desc = [&](int li, int which_chain, ChainDesc* cd) {
-        memset(cd, 0, sizeof(*cd));
-        const DecLayer& l = m->dec[li];
-        cd->partial = s->partial; cd->x = s->x; cd->B = B; cd->Bp = s->bp; cd->d = d; cd->dtype = dt; cd->pdl = 0;
-        const int set = rot & 1;   // alternate two word sets: each launch re-arms the other one
-        cd->counters = s->chain_counters + set * 8; cd->reset_counters = s->chain_counters + (set ^ 1) * 8;
-        auto gp = [&](const void* w, int N, int K, const void* act) { ChainPhaseDesc ph; memset(&ph, 0, sizeof(ph)); ph.kind = 0; ph.w = w; ph.n = N; ph.k = K; ph.act = act; ph.splits = choose_splits((N + 127) / 128, K / 64, m->num_sms); return ph; };
-        auto lp = [&](const float* bias, const LayerNormW& ln) { ChainPhaseDesc ph; memset(&ph, 0, sizeof(ph)); ph.kind = 1; ph.bias = bias; ph.gamma = ln.g; ph.beta = ln.b; ph.out16 = s->xn; return ph; };
-        if (which_chain == 0) {
-            cd->ph[0] = gp(l.wo, d, d, s->attn); cd->ph[1] = lp(l.bo, l.lnx); cd->ph[2] = gp(l.wcq, d, d, s->xn); cd->n_phases = 3;
-        } else {
-            cd->ph[0] = gp(l.wco, d, d, s->attn); cd->ph[1] = lp(l.bco, l.ln3); cd->ph[2] = gp(l.w1, 4 * d, d, s->xn);
-            cd->ph[3].kind = 2; cd->ph[3].bias = l.b1; cd->ph[3].out16 = s->ffn;
-            cd->ph[4] = gp(l.w2, d, 4 * d, s->ffn); cd->ph[5] = lp(l.b2, l.ln1); cd->ph[6] = gp(l.wqkv, 3 * d, d, s->xn); cd->n_phases = 7;
-        }
-    };
     auto run = [&]() -> wk_status {
         int sp;
         switch (which) {
@@ -1634,12 +1555,6 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
                 if (which == 16) return dec_gemm(s, l.w2, d, 4 * d, s->ffn, &sp);
                 return dec_gemm(s, l.wqkv, 3 * d, d, s->xn, &sp);
             }
-            case 18: case 19: {
-                ChainDesc cd;
-                chain_desc(rot % c.dec_layers, which - 18, &cd);
-                ++rot;
-                return decoder_chain(cd, m->num_sms, st);
-            }
             default: set_error("wk_bench_kernel: unknown kernel %d", which); return WK_ERR_INVALID_ARGUMENT;
         }
     };
@@ -1653,8 +1568,6 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
         case 6: case 14: *work_out = 1.0 * d * d * 2; break;
         case 7: case 15: case 16: *work_out = 4.0 * d * d * 2; break;
         case 9: *work_out = (double)B * H * 100 * 64 * 2 * 2; break;                       // K + V rows read at position 100
-        case 18: *work_out = 2.0 * d * d * 2; break;                                       // out-proj + cross-Q weights
-        case 19: *work_out = 12.0 * d * d * 2; break;                                      // cross-out + FC1 + FC2 + QKV weights
         default: *work_out = 0; break;
     }
     wk_status rs = WK_OK;

@@ -1,5 +1,5 @@
-// Inline-PTX wrappers of the Hopper warpgroup MMA (wgmma.mma_async, sm_90a) used by the GEMM, the encoder attention and the
-// decoder chain.  D (f32) is held in registers: for m64nNk16 thread t of the warpgroup owns rows 16 * (t / 32) + (t % 32) / 4 (+ 8)
+// Inline-PTX wrappers of the Hopper warpgroup MMA (wgmma.mma_async, sm_90a) used by the GEMM and the encoder attention.
+// D (f32) is held in registers: for m64nNk16 thread t of the warpgroup owns rows 16 * (t / 32) + (t % 32) / 4 (+ 8)
 // and columns 8 * j + 2 * (t % 4) (+ 1), j < N / 8, as d[4 j + {0, 1}] (row) and d[4 j + {2, 3}] (row + 8).
 #pragma once
 #include <stdint.h>

@@ -591,6 +591,9 @@ int32_t wk_write_vtt(const float* starts, const float* ends, const char* const* 
 /* ---- instrumentation ---- */
 /* Number of kernels launched by this library on the calling process since the last reset. */
 int64_t wk_kernel_launch_count(int32_t reset);
+/* Bytes of device and pinned host memory the library holds through its buffer owner (all models, sessions and workspaces of the
+ * process; not wk_tensor data, which is stream-ordered).  Test instrumentation. */
+wk_status wk_debug_live_bytes(int64_t* device_bytes, int64_t* pinned_bytes);
 /* Last-run stage timings in ms, TranscriptionTimings buckets (Models.swift:730-776):
  * [0] logmels [1] encoding [2] crossKV [3] decodingLoop [4] h2d [5] d2h */
 wk_status wk_last_timings(wk_model* m, float* ms6);

@@ -256,6 +256,7 @@ SYMBOLS = [
     ("wk_write_srt", I32, [PF32, PF32, C.POINTER(C.c_char_p), I32, C.POINTER(C.c_char), I32]),
     ("wk_write_vtt", I32, [PF32, PF32, C.POINTER(C.c_char_p), I32, C.POINTER(C.c_char), I32]),
     ("wk_kernel_launch_count", I64, [I32]),
+    ("wk_debug_live_bytes", I32, [PI64, PI64]),
     ("wk_last_timings", I32, [P, PF32]),
     ("wk_model_stream", P, [P]),
     ("wk_test_gemm", I32, [P, P, P, P, P, I32, I32, I32, I32, I32, I32]),

@@ -413,55 +413,30 @@ static wk_status make_mix(int fmt, int channels, const wk_audio_load_opts* o, Mi
 
 // ------------------------------------------------------------------------------------------------ host: workspace and driver
 struct AudioWs {
+    Buffers mem;
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    uint8_t* h_in[2] = {nullptr, nullptr}; size_t h_in_cap = 0;    // pinned input staging (double-buffered: the host fills one while
-    float* h_out[2] = {nullptr, nullptr}; size_t h_out_cap = 0;    // the other is copied); pinned output staging for host outputs
+    uint8_t* h_in[2] = {nullptr, nullptr};    // pinned input staging (double-buffered: the host fills one while
+    float* h_out[2] = {nullptr, nullptr};     // the other is copied); pinned output staging for host outputs
     cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-    uint8_t* d_raw = nullptr; size_t d_raw_cap = 0;
-    float* d_out = nullptr; size_t d_out_cap = 0;
-    float* d_tab = nullptr; size_t d_tab_cap = 0; int tab_rate = 0;
-    int64_t* d_starts = nullptr; size_t d_starts_cap = 0;
-    unsigned* d_peaks = nullptr; size_t d_peaks_cap = 0;
+    uint8_t* d_raw = nullptr;
+    float* d_out = nullptr;
+    float* d_tab = nullptr; int tab_rate = 0;
+    int64_t* d_starts = nullptr;
+    unsigned* d_peaks = nullptr;
+    ~AudioWs() {
+        cudaSetDevice(device);
+        if (stream) cudaStreamSynchronize(stream);
+        for (int i = 0; i < 2; ++i) {
+            if (ev_in[i]) cudaEventDestroy(ev_in[i]);
+            if (ev_out[i]) cudaEventDestroy(ev_out[i]);
+        }
+        if (own_stream && stream) cudaStreamDestroy(stream);
+    }
 };
 
-void audio_ws_free(AudioWs* w) {
-    if (!w) return;
-    cudaSetDevice(w->device);
-    if (w->stream) cudaStreamSynchronize(w->stream);
-    for (int i = 0; i < 2; ++i) {
-        if (w->h_in[i]) cudaFreeHost(w->h_in[i]);
-        if (w->h_out[i]) cudaFreeHost(w->h_out[i]);
-        if (w->ev_in[i]) cudaEventDestroy(w->ev_in[i]);
-        if (w->ev_out[i]) cudaEventDestroy(w->ev_out[i]);
-    }
-    void* d[] = {w->d_raw, w->d_out, w->d_tab, w->d_starts, w->d_peaks};
-    for (void* p : d) if (p) cudaFree(p);
-    if (w->own_stream) cudaStreamDestroy(w->stream);
-    delete w;
-}
-
-static wk_status grow_dev(void** p, size_t* cap, size_t need) {
-    if (need <= *cap) return WK_OK;
-    if (*p) WK_CUDA_CHECK(cudaFree(*p));
-    *p = nullptr; *cap = 0;
-    WK_CUDA_CHECK(cudaMalloc(p, need));
-    *cap = need;
-    return WK_OK;
-}
-static wk_status grow_pinned2(void** p, size_t* cap, size_t need) {
-    if (need <= *cap) return WK_OK;
-    for (int i = 0; i < 2; ++i) {
-        if (p[i]) WK_CUDA_CHECK(cudaFreeHost(p[i]));
-        p[i] = nullptr;
-    }
-    *cap = 0;
-    for (int i = 0; i < 2; ++i)
-        if (cudaHostAlloc(&p[i], need, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_error("pinned audio staging of %zu bytes failed", need); return WK_ERR_CUDA; }
-    *cap = need;
-    return WK_OK;
-}
+void audio_ws_free(AudioWs* w) { delete w; }
 
 // Where the stored frames come from: a WAV file (data chunk at data_offset), host memory, or device memory (read in place).
 struct Source {
@@ -537,7 +512,7 @@ static wk_status run_convert(AudioWs* w, const Source& src, int rate, const MixP
                     const int64_t j = phi + (int64_t)k * up;
                     if (j < (int64_t)h.size()) tab[(size_t)phi * fp.ld + k] = (float)h[j];
                 }
-            WK_CHECK(grow_dev((void**)&w->d_tab, &w->d_tab_cap, tab.size() * 4));
+            WK_CHECK(w->mem.grow(&w->d_tab, tab.size()));
             WK_CUDA_CHECK(cudaMemcpyAsync(w->d_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, w->stream));
             WK_CUDA_CHECK(cudaStreamSynchronize(w->stream));   // `tab` is pageable and goes out of scope
             w->tab_rate = rate;
@@ -561,20 +536,20 @@ static wk_status run_convert(AudioWs* w, const Source& src, int rate, const MixP
     const int n_chunks = (int)plan.starts.size() - 1;
     WK_CUDA_CHECK(cudaSetDevice(w->device));
     if (!src.dev) {
-        WK_CHECK(grow_dev((void**)&w->d_raw, &w->d_raw_cap, (size_t)seg_in_frames * fb));
-        WK_CHECK(grow_pinned2((void**)w->h_in, &w->h_in_cap, (size_t)seg_in_frames * fb));
+        WK_CHECK(w->mem.grow(&w->d_raw, (size_t)seg_in_frames * fb));
+        for (uint8_t*& h : w->h_in) WK_CHECK(w->mem.grow_pinned(&h, (size_t)seg_in_frames * fb));
     }
     const bool out_dev = is_device_ptr(out);
     if (!out_dev) {
-        WK_CHECK(grow_dev((void**)&w->d_out, &w->d_out_cap, (size_t)seg * 4));
-        WK_CHECK(grow_pinned2((void**)w->h_out, &w->h_out_cap, (size_t)seg * 4));
+        WK_CHECK(w->mem.grow(&w->d_out, (size_t)seg));
+        for (float*& h : w->h_out) WK_CHECK(w->mem.grow_pinned(&h, (size_t)seg));
     }
     for (int i = 0; i < 2; ++i) {
         if (!w->ev_in[i]) WK_CUDA_CHECK(cudaEventCreateWithFlags(&w->ev_in[i], cudaEventDisableTiming));
         if (!w->ev_out[i]) WK_CUDA_CHECK(cudaEventCreateWithFlags(&w->ev_out[i], cudaEventDisableTiming));
     }
-    WK_CHECK(grow_dev((void**)&w->d_starts, &w->d_starts_cap, plan.starts.size() * 8));
-    WK_CHECK(grow_dev((void**)&w->d_peaks, &w->d_peaks_cap, (size_t)std::max(n_chunks, 1) * 8));
+    WK_CHECK(w->mem.grow(&w->d_starts, plan.starts.size()));
+    WK_CHECK(w->mem.grow(&w->d_peaks, (size_t)std::max(n_chunks, 1) * 2));   // two peaks per chunk
     WK_CUDA_CHECK(cudaMemcpyAsync(w->d_starts, plan.starts.data(), plan.starts.size() * 8, cudaMemcpyHostToDevice, w->stream));
     WK_CUDA_CHECK(cudaMemsetAsync(w->d_peaks, 0, (size_t)std::max(n_chunks, 1) * 8, w->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(w->stream));   // plan.starts is pageable
@@ -637,7 +612,7 @@ static wk_status run_convert(AudioWs* w, const Source& src, int rate, const MixP
 struct WsHandle {
     AudioWs* w = nullptr;
     bool temp = false;
-    ~WsHandle() { if (temp) audio_ws_free(w); }
+    ~WsHandle() { if (temp) delete w; }
     wk_status open(wk_session* s) {
         if (!wk_device_available()) { set_error("audio: no sm_90 (Hopper) device"); return WK_ERR_MODELS_UNAVAILABLE; }
         if (s) {

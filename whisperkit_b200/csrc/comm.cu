@@ -60,9 +60,10 @@ struct wk_comm {
     ncclComm_t comm = nullptr;
     int rank = 0, world = 1, device = 0;
     cudaStream_t stream = nullptr, copy_stream = nullptr;
-    float* stage[2] = {nullptr, nullptr}; size_t stage_elems = 0;   // root: shards of the other ranks on their way from the host
+    wk::Buffers mem;
+    float* stage[2] = {nullptr, nullptr};   // root: shards of the other ranks on their way from the host
     cudaEvent_t staged[2], sent[2];
-    wk_decode_result* res_dev = nullptr; size_t res_cap = 0;
+    wk_decode_result* res_dev = nullptr;
     float stage_ms[4] = {0, 0, 0, 0};   // last sharded call on this rank: scatter, transcribe, gather, total (host wall clock)
 };
 
@@ -112,8 +113,7 @@ void wk_comm_free(wk_comm* c) {
     cudaStreamSynchronize(c->stream);
     cudaStreamSynchronize(c->copy_stream);
     if (c->comm && nccl()) nccl()->CommDestroy(c->comm);
-    for (int i = 0; i < 2; ++i) { if (c->stage[i]) cudaFree(c->stage[i]); cudaEventDestroy(c->staged[i]); cudaEventDestroy(c->sent[i]); }
-    if (c->res_dev) cudaFree(c->res_dev);
+    for (int i = 0; i < 2; ++i) { cudaEventDestroy(c->staged[i]); cudaEventDestroy(c->sent[i]); }
     cudaStreamDestroy(c->stream);
     cudaStreamDestroy(c->copy_stream);
     delete c;
@@ -139,10 +139,8 @@ wk_status wk_comm_scatter_windows(wk_comm* c, const float* all_pcm, int64_t n_wi
     cudaGetLastError();
     int64_t max_shard = 0;
     for (int r = 0; r < c->world; ++r) { int64_t a, b; wk_comm_shard_bounds(n_windows, c->world, r, &a, &b); if (r != root) max_shard = std::max(max_shard, b - a); }
-    if (!on_dev && (size_t)max_shard * stride > c->stage_elems) {
-        for (int i = 0; i < 2; ++i) { if (c->stage[i]) cudaFree(c->stage[i]); WK_CUDA_CHECK(cudaMalloc((void**)&c->stage[i], (size_t)max_shard * stride * 4)); }
-        c->stage_elems = (size_t)max_shard * stride;
-    }
+    if (!on_dev)
+        for (float*& p : c->stage) WK_CHECK(c->mem.grow(&p, (size_t)max_shard * stride));
     int k = 0;
     for (int r = 0; r < c->world; ++r) {
         if (r == root) continue;
@@ -175,12 +173,7 @@ wk_status wk_comm_gather_results(wk_comm* c, const wk_decode_result* local, int6
     NcclApi* n = nccl();
     WK_CUDA_CHECK(cudaSetDevice(c->device));
     const size_t need = (size_t)(c->rank == root ? n_windows : n_local);
-    if (need > c->res_cap) {
-        WK_CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        if (c->res_dev) cudaFree(c->res_dev);
-        WK_CUDA_CHECK(cudaMalloc((void**)&c->res_dev, need * sizeof(wk_decode_result)));
-        c->res_cap = need;
-    }
+    WK_CHECK(c->mem.grow(&c->res_dev, need, c->stream));
     int64_t lo, hi;
     wk_comm_shard_bounds(n_windows, c->world, c->rank, &lo, &hi);
     if (hi - lo != n_local) { wk::set_error("wk_comm_gather_results: rank %d holds %lld results, its shard has %lld windows", c->rank, (long long)n_local, (long long)(hi - lo)); return WK_ERR_INVALID_ARGUMENT; }
@@ -215,8 +208,9 @@ wk_status wk_transcribe_windows_sharded(wk_comm* c, wk_model* m, wk_session* s, 
     wk_comm_shard_bounds(n_windows, c->world, c->rank, &lo, &hi);
     const int64_t nl = hi - lo;
     WK_CUDA_CHECK(cudaSetDevice(c->device));
+    wk::Buffers scratch;
     float* shard = nullptr;
-    WK_CUDA_CHECK(cudaMalloc((void**)&shard, (size_t)std::max<int64_t>(nl, 1) * stride * 4));
+    WK_CHECK(scratch.dmalloc(&shard, (size_t)std::max<int64_t>(nl, 1) * stride, false));
     auto now = []() { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e3 + t.tv_nsec * 1e-6; };
     const double t0 = now();
     wk_status r = wk_comm_scatter_windows(c, all_pcm, n_windows, stride, root, shard, nullptr);
@@ -224,7 +218,6 @@ wk_status wk_transcribe_windows_sharded(wk_comm* c, wk_model* m, wk_session* s, 
     std::vector<wk_decode_result> local((size_t)std::max<int64_t>(nl, 1));
     if (r == WK_OK && nl > 0) r = wk_transcribe_windows_ex(m, s, shard, nl, stride, nullptr, st, bo, local.data());
     const double t2 = now();
-    cudaFree(shard);
     if (r != WK_OK) return r;
     r = wk_comm_gather_results(c, local.data(), nl, n_windows, root, results);
     const double t3 = now();

@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <atomic>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -30,6 +31,7 @@ void set_error(const char* fmt, ...) {
 }
 const char* last_error_cstr() { return g_err; }
 static std::atomic<long long> g_launches{0};
+static std::atomic<int64_t> g_live_bytes[2] = {{0}, {0}};   // held through Buffers: [0] device, [1] pinned host
 static std::atomic<int> g_pdl{-1};
 int pdl_mode() {
     // Programmatic dependent launch along the decode step.  Mask 53 = embed | cross-attention (its K chunks are static and prefetched
@@ -49,6 +51,49 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 long long launch_counter_load() { return g_launches.load(); }
 void launch_counter_sub(long long n) { g_launches.fetch_sub(n); }
 
+// ------------------------------------------------------------------------------------------------ buffer owner
+wk_status Buffers::alloc(void** p, size_t bytes, bool pinned, bool zero) {
+    cudaError_t e = pinned ? cudaHostAlloc(p, bytes, cudaHostAllocDefault) : cudaMalloc(p, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        *p = nullptr;
+        if (pinned) set_error("pinned staging of %zu bytes failed: %s", bytes, cudaGetErrorString(e));
+        else set_error("cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
+        return WK_ERR_CUDA;
+    }
+    live_.push_back({*p, bytes, pinned});
+    g_live_bytes[pinned].fetch_add((int64_t)bytes);
+    if (zero) {
+        if (pinned) memset(*p, 0, bytes);
+        else if ((e = cudaMemset(*p, 0, bytes)) != cudaSuccess) { set_error("cudaMemset failed: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    }
+    return WK_OK;
+}
+
+static void free_buffer(void* p, size_t bytes, bool pinned) {
+    if (pinned) cudaFreeHost(p);
+    else cudaFree(p);
+    g_live_bytes[pinned].fetch_sub((int64_t)bytes);
+}
+
+wk_status Buffers::regrow(void** p, size_t bytes, bool pinned, cudaStream_t drain, bool* moved) {
+    if (moved) *moved = false;
+    auto it = std::find_if(live_.begin(), live_.end(), [&](const Buf& b) { return *p && b.p == *p; });
+    if ((it == live_.end() ? 0 : it->bytes) >= bytes) return WK_OK;
+    if (moved) *moved = true;
+    if (it != live_.end()) {
+        if (drain) WK_CUDA_CHECK(cudaStreamSynchronize(drain));
+        free_buffer(it->p, it->bytes, it->pinned);
+        live_.erase(it);
+    }
+    return alloc(p, bytes, pinned, false);
+}
+
+void Buffers::release_all() {
+    for (const Buf& b : live_) free_buffer(b.p, b.bytes, b.pinned);
+    live_.clear();
+}
+
 int choose_splits(int tiles, int total_kb, int num_sms) {
     // Split-K depth of a decoder swap-AB GEMM: the deepest split that still fits ONE wave of CTAs (tiles * s <= SMs), so every SM that
     // takes part streams its share of the weights exactly once: one SM alone cannot pull HBM bandwidth, so too few CTAs starve, while a
@@ -63,9 +108,9 @@ int choose_splits(int tiles, int total_kb, int num_sms) {
 
 size_t esize(int dtype) { return dtype == WK_DTYPE_F32 || dtype == WK_DTYPE_I32 ? 4 : 2; }
 
-static wk_status alloc_ln(LayerNormW& ln, int d) {
-    WK_CHECK(dmalloc(&ln.g, d));
-    WK_CHECK(dmalloc(&ln.b, d));
+static wk_status alloc_ln(Buffers& b, LayerNormW& ln, int d) {
+    WK_CHECK(b.dmalloc(&ln.g, d));
+    WK_CHECK(b.dmalloc(&ln.b, d));
     return WK_OK;
 }
 
@@ -73,65 +118,61 @@ static wk_status model_alloc(wk_model* m) {
     const wk_model_config& c = m->cfg;
     const int d = c.d_model, L = c.enc_layers, Ld = c.dec_layers;
     const size_t T = c.n_audio_ctx;
-    WK_CHECK(alloc16(&m->conv1_w, (size_t)d * 3 * 128));
-    WK_CHECK(dmalloc(&m->conv1_b, d));
-    WK_CHECK(alloc16(&m->conv2_w, (size_t)d * 3 * d));
-    WK_CHECK(dmalloc(&m->conv2_b, d));
-    WK_CHECK(dmalloc(&m->enc_pos, T * d));
+    Buffers& b = m->mem;
+    WK_CHECK(b.alloc16(&m->conv1_w, (size_t)d * 3 * 128));
+    WK_CHECK(b.dmalloc(&m->conv1_b, d));
+    WK_CHECK(b.alloc16(&m->conv2_w, (size_t)d * 3 * d));
+    WK_CHECK(b.dmalloc(&m->conv2_b, d));
+    WK_CHECK(b.dmalloc(&m->enc_pos, T * d));
     m->enc.resize(L);
     for (auto& l : m->enc) {
-        WK_CHECK(alloc_ln(l.ln1, d)); WK_CHECK(alloc_ln(l.ln2, d));
-        WK_CHECK(alloc16(&l.wqkv, (size_t)3 * d * d)); WK_CHECK(dmalloc(&l.bqkv, 3 * d));
-        WK_CHECK(alloc16(&l.wo, (size_t)d * d)); WK_CHECK(dmalloc(&l.bo, d));
-        WK_CHECK(alloc16(&l.w1, (size_t)4 * d * d)); WK_CHECK(dmalloc(&l.b1, 4 * d));
-        WK_CHECK(alloc16(&l.w2, (size_t)4 * d * d)); WK_CHECK(dmalloc(&l.b2, d));
+        WK_CHECK(alloc_ln(b, l.ln1, d)); WK_CHECK(alloc_ln(b, l.ln2, d));
+        WK_CHECK(b.alloc16(&l.wqkv, (size_t)3 * d * d)); WK_CHECK(b.dmalloc(&l.bqkv, 3 * d));
+        WK_CHECK(b.alloc16(&l.wo, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bo, d));
+        WK_CHECK(b.alloc16(&l.w1, (size_t)4 * d * d)); WK_CHECK(b.dmalloc(&l.b1, 4 * d));
+        WK_CHECK(b.alloc16(&l.w2, (size_t)4 * d * d)); WK_CHECK(b.dmalloc(&l.b2, d));
     }
-    WK_CHECK(alloc_ln(m->enc_ln, d));
+    WK_CHECK(alloc_ln(b, m->enc_ln, d));
     // embedding rows padded to a multiple of 128 so the last TMA tile never leaves the allocation
-    WK_CHECK(alloc16(&m->emb, (size_t)round_up(c.vocab, 128) * d));
-    WK_CHECK(dmalloc(&m->dec_pos, (size_t)c.n_text_ctx * d));
+    WK_CHECK(b.alloc16(&m->emb, (size_t)round_up(c.vocab, 128) * d));
+    WK_CHECK(b.dmalloc(&m->dec_pos, (size_t)c.n_text_ctx * d));
     m->dec.resize(Ld);
     for (auto& l : m->dec) {
-        WK_CHECK(alloc_ln(l.ln1, d)); WK_CHECK(alloc_ln(l.lnx, d)); WK_CHECK(alloc_ln(l.ln3, d));
-        WK_CHECK(alloc16(&l.wqkv, (size_t)3 * d * d)); WK_CHECK(dmalloc(&l.bq, d)); WK_CHECK(dmalloc(&l.bv, d));
-        WK_CHECK(alloc16(&l.wo, (size_t)d * d)); WK_CHECK(dmalloc(&l.bo, d));
-        WK_CHECK(alloc16(&l.wcq, (size_t)d * d)); WK_CHECK(dmalloc(&l.bcq, d));
-        WK_CHECK(alloc16(&l.wco, (size_t)d * d)); WK_CHECK(dmalloc(&l.bco, d));
-        WK_CHECK(alloc16(&l.w1, (size_t)4 * d * d)); WK_CHECK(dmalloc(&l.b1, 4 * d));
-        WK_CHECK(alloc16(&l.w2, (size_t)4 * d * d)); WK_CHECK(dmalloc(&l.b2, d));
+        WK_CHECK(alloc_ln(b, l.ln1, d)); WK_CHECK(alloc_ln(b, l.lnx, d)); WK_CHECK(alloc_ln(b, l.ln3, d));
+        WK_CHECK(b.alloc16(&l.wqkv, (size_t)3 * d * d)); WK_CHECK(b.dmalloc(&l.bq, d)); WK_CHECK(b.dmalloc(&l.bv, d));
+        WK_CHECK(b.alloc16(&l.wo, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bo, d));
+        WK_CHECK(b.alloc16(&l.wcq, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bcq, d));
+        WK_CHECK(b.alloc16(&l.wco, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bco, d));
+        WK_CHECK(b.alloc16(&l.w1, (size_t)4 * d * d)); WK_CHECK(b.dmalloc(&l.b1, 4 * d));
+        WK_CHECK(b.alloc16(&l.w2, (size_t)4 * d * d)); WK_CHECK(b.dmalloc(&l.b2, d));
     }
-    WK_CHECK(alloc_ln(m->dec_ln, d));
-    WK_CHECK(alloc16(&m->wckv, (size_t)2 * Ld * d * d));
-    WK_CHECK(dmalloc(&m->bckv, (size_t)2 * Ld * d));
+    WK_CHECK(alloc_ln(b, m->dec_ln, d));
+    WK_CHECK(b.alloc16(&m->wckv, (size_t)2 * Ld * d * d));
+    WK_CHECK(b.dmalloc(&m->bckv, (size_t)2 * Ld * d));
     return WK_OK;
 }
 
 wk_status enc_ws_ensure(wk_model* m, EncWorkspace* ws, int max_batch) {
     if (ws->max_batch >= max_batch) return WK_OK;
-    enc_ws_free(ws);
+    *ws = EncWorkspace();   // releases a smaller workspace
     const wk_model_config& c = m->cfg;
     const int d = c.d_model, Bm = max_batch;
     const size_t T = c.n_audio_ctx;
-    WK_CHECK(dmalloc(&ws->pcm_dev, (size_t)Bm * kWindowSamples, false));
-    WK_CHECK(dmalloc(&ws->nvalid_dev, Bm));
-    WK_CHECK(dmalloc(&ws->gmax, Bm));
-    WK_CHECK(alloc16(&ws->mel, (size_t)Bm * kMelRows * kMelCols));
-    WK_CHECK(alloc16(&ws->h1, (size_t)Bm * kMelRows * d));
+    Buffers& b = ws->mem;
+    WK_CHECK(b.dmalloc(&ws->pcm_dev, (size_t)Bm * kWindowSamples, false));
+    WK_CHECK(b.dmalloc(&ws->nvalid_dev, Bm));
+    WK_CHECK(b.dmalloc(&ws->gmax, Bm));
+    WK_CHECK(b.alloc16(&ws->mel, (size_t)Bm * kMelRows * kMelCols));
+    WK_CHECK(b.alloc16(&ws->h1, (size_t)Bm * kMelRows * d));
     const size_t M = (size_t)Bm * T;
-    WK_CHECK(dmalloc(&ws->x, M * d, false));
-    WK_CHECK(alloc16(&ws->xn, M * d));
-    WK_CHECK(alloc16(&ws->qkv, M * 3 * d));
-    WK_CHECK(alloc16(&ws->attn, M * d));
-    WK_CHECK(alloc16(&ws->ffn, M * 4 * d));
-    WK_CHECK(alloc16(&ws->enc_out, M * d));
+    WK_CHECK(b.dmalloc(&ws->x, M * d, false));
+    WK_CHECK(b.alloc16(&ws->xn, M * d));
+    WK_CHECK(b.alloc16(&ws->qkv, M * 3 * d));
+    WK_CHECK(b.alloc16(&ws->attn, M * d));
+    WK_CHECK(b.alloc16(&ws->ffn, M * 4 * d));
+    WK_CHECK(b.alloc16(&ws->enc_out, M * d));
     ws->max_batch = Bm;
     return WK_OK;
-}
-
-void enc_ws_free(EncWorkspace* ws) {
-    void* ptrs[] = {ws->pcm_dev, ws->nvalid_dev, ws->gmax, ws->mel, ws->h1, ws->x, ws->xn, ws->qkv, ws->attn, ws->ffn, ws->enc_out};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    *ws = EncWorkspace();
 }
 
 // ---------------------------------------------------------------------------------------------- weight ingestion
@@ -256,7 +297,7 @@ wk_status mel_run(wk_model* m, EncWorkspace* ws, const float* pcm, int64_t n, in
         WK_CUDA_CHECK(cudaMemcpyAsync(ws->nvalid_dev, samples_per_window, n * 4, cudaMemcpyHostToDevice, stream));
         nv = ws->nvalid_dev;
     }
-    return mel_forward(m->mel_tables, src, n, src_stride, nv, mel_out, ws->gmax, stream);
+    return mel_forward(&m->mel_tables, src, n, src_stride, nv, mel_out, ws->gmax, stream);
 }
 
 wk_status encode_chunk(wk_model* m, EncWorkspace* ws, const void* mel, int B, void* enc_out, cudaStream_t s) {
@@ -384,20 +425,19 @@ wk_status wk_model_create(const wk_model_config* cfg, int32_t device, wk_model**
         return WK_ERR_INVALID_ARGUMENT;
     }
     WK_CUDA_CHECK(cudaSetDevice(device));
-    wk_model* m = new wk_model();
+    std::unique_ptr<wk_model> m(new wk_model());   // released on any failure below
     m->cfg = *cfg;
-    wk_model_set_alignment_heads(m, nullptr, 0);
+    wk_model_set_alignment_heads(m.get(), nullptr, 0);
     m->device = device;
     cudaDeviceProp prop;
     WK_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
     m->num_sms = prop.multiProcessorCount;
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
     for (auto& e : m->ev) WK_CUDA_CHECK(cudaEventCreate(&e));
-    wk_status s = model_alloc(m);
-    if (s != WK_OK) return s;
-    WK_CHECK(mel_tables_create(cfg->n_mels, &m->mel_tables));
+    WK_CHECK(model_alloc(m.get()));
+    WK_CHECK(mel_tables_create(cfg->n_mels, m->mem, &m->mel_tables));
     WK_CUDA_CHECK(cudaDeviceSynchronize());  // setup memsets / table uploads ran on the legacy default stream
-    *out = m;
+    *out = m.release();
     return WK_OK;
 }
 
@@ -416,26 +456,25 @@ wk_status wk_model_set_tensor(wk_model* m, const char* name, const void* data, i
         set_error("wk_model_set_tensor: '%s' has %zu elements, expected %zu", name, numel, dst.numel);
         return WK_ERR_INVALID_ARGUMENT;
     }
-    void* tmp = nullptr;
-    WK_CUDA_CHECK(cudaMalloc(&tmp, numel * esize(dtype)));
+    Buffers scratch;
+    uint8_t* tmp = nullptr;
+    WK_CHECK(scratch.dmalloc(&tmp, numel * esize(dtype), false));
     // stream-ordered copy: a pageable-host cudaMemcpy may return before its DMA lands, and the library stream is
     // non-blocking (it does not order against the legacy default stream)
     WK_CUDA_CHECK(cudaMemcpyAsync(tmp, data, numel * esize(dtype), cudaMemcpyDefault, m->stream));
     wk_status st = WK_OK;
     if (dst.special) {
         float* f = nullptr;
-        WK_CUDA_CHECK(cudaMalloc(&f, numel * 4));
+        WK_CHECK(scratch.dmalloc(&f, numel, false));
         st = convert_to_16(tmp, dtype, f, WK_DTYPE_F32, (int64_t)numel, m->stream);
         const int co = m->cfg.d_model, ci = dst.special == 1 ? m->cfg.n_mels : m->cfg.d_model, cip = dst.special == 1 ? kMelCols : m->cfg.d_model;
         const long long n = (long long)co * 3 * cip;
         conv_w_rearrange_kernel<<<(unsigned)((n + 255) / 256), 256, 0, m->stream>>>(f, (__half*)dst.p, co, ci, cip);
         cudaStreamSynchronize(m->stream);
-        cudaFree(f);
     } else {
         st = convert_to_16(tmp, dtype, dst.p, dst.dtype, (int64_t)numel, m->stream);
         cudaStreamSynchronize(m->stream);
     }
-    cudaFree(tmp);
     return st;
 }
 
@@ -721,23 +760,15 @@ wk_status wk_cross_kv_quantize_rows(const float* x, int64_t rows, uint8_t* codes
     return WK_OK;
 }
 
+wk_model::~wk_model() {
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+}
+
 void wk_model_free(wk_model* m) {
     if (!m) return;
     cudaSetDevice(m->device);
     cudaDeviceSynchronize();
-    auto fr = [](void* p) { if (p) cudaFree(p); };
-    fr(m->conv1_w); fr(m->conv1_b); fr(m->conv2_w); fr(m->conv2_b); fr(m->enc_pos);
-    for (auto& l : m->enc) { fr(l.ln1.g); fr(l.ln1.b); fr(l.ln2.g); fr(l.ln2.b); fr(l.wqkv); fr(l.bqkv); fr(l.wo); fr(l.bo); fr(l.w1); fr(l.b1); fr(l.w2); fr(l.b2); }
-    fr(m->enc_ln.g); fr(m->enc_ln.b); fr(m->emb); fr(m->dec_pos);
-    for (auto& l : m->dec) {
-        fr(l.ln1.g); fr(l.ln1.b); fr(l.lnx.g); fr(l.lnx.b); fr(l.ln3.g); fr(l.ln3.b); fr(l.wqkv); fr(l.bq); fr(l.bv); fr(l.wo); fr(l.bo);
-        fr(l.wcq); fr(l.bcq); fr(l.wco); fr(l.bco); fr(l.w1); fr(l.b1); fr(l.w2); fr(l.b2);
-    }
-    fr(m->dec_ln.g); fr(m->dec_ln.b); fr(m->wckv); fr(m->bckv);
-    enc_ws_free(&m->ws);
-    mel_tables_free(m->mel_tables);
-    for (auto& e : m->ev) cudaEventDestroy(e);
-    cudaStreamDestroy(m->stream);
     delete m;
 }
 
@@ -874,14 +905,15 @@ wk_status wk_filter_sample(wk_model* m, const wk_special_tokens* st, const wk_de
     float *dlog = nullptr, *dfil = nullptr, *dlp = nullptr;
     int32_t *dtok = nullptr, *dn = nullptr, *dout = nullptr, *dsup = nullptr, *dlang = nullptr;
     const int ldt = ld_tokens > 0 ? ld_tokens : 1;
-    WK_CUDA_CHECK(cudaMalloc(&dlog, (size_t)batch * vocab * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dfil, (size_t)batch * vocab * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dlp, batch * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dtok, (size_t)batch * ldt * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dn, batch * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dout, batch * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dsup, 4096 * 4));
-    WK_CUDA_CHECK(cudaMalloc(&dlang, 4096 * 4));
+    Buffers scratch;
+    WK_CHECK(scratch.dmalloc(&dlog, (size_t)batch * vocab, false));
+    WK_CHECK(scratch.dmalloc(&dfil, (size_t)batch * vocab, false));
+    WK_CHECK(scratch.dmalloc(&dlp, batch, false));
+    WK_CHECK(scratch.dmalloc(&dtok, (size_t)batch * ldt, false));
+    WK_CHECK(scratch.dmalloc(&dn, batch, false));
+    WK_CHECK(scratch.dmalloc(&dout, batch, false));
+    WK_CHECK(scratch.dmalloc(&dsup, 4096, false));
+    WK_CHECK(scratch.dmalloc(&dlang, 4096, false));
     WK_CUDA_CHECK(cudaMemcpyAsync(dlog, logits, (size_t)batch * vocab * 4, cudaMemcpyDefault, s));
     if (tokens && ld_tokens > 0) WK_CUDA_CHECK(cudaMemcpyAsync(dtok, tokens, (size_t)batch * ldt * 4, cudaMemcpyDefault, s));
     WK_CUDA_CHECK(cudaMemcpyAsync(dn, n_tokens, batch * 4, cudaMemcpyDefault, s));
@@ -912,7 +944,6 @@ wk_status wk_filter_sample(wk_model* m, const wk_special_tokens* st, const wk_de
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         if (e != cudaSuccess) { set_error("wk_filter_sample: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     }
-    cudaFree(dlog); cudaFree(dfil); cudaFree(dlp); cudaFree(dtok); cudaFree(dn); cudaFree(dout); cudaFree(dsup); cudaFree(dlang);
     return r;
 }
 
@@ -952,6 +983,13 @@ int64_t wk_kernel_launch_count(int32_t reset) {
     const long long v = wk::launch_counter_load();
     if (reset) wk::launch_counter_sub(v);
     return v;
+}
+
+wk_status wk_debug_live_bytes(int64_t* device_bytes, int64_t* pinned_bytes) {
+    if (!device_bytes || !pinned_bytes) return WK_ERR_INVALID_ARGUMENT;
+    *device_bytes = g_live_bytes[0].load();
+    *pinned_bytes = g_live_bytes[1].load();
+    return WK_OK;
 }
 
 wk_status wk_last_timings(wk_model* m, float* ms6) {
@@ -998,8 +1036,9 @@ wk_status wk_test_gemm_splitk(wk_model* m, const void* w, const void* x, float* 
     if (rows_x % 16 != 0 || rows_x > 256) { set_error("wk_test_gemm_splitk: rows_x must be a multiple of 16 <= 256"); return WK_ERR_INVALID_ARGUMENT; }
     const int tiles = (N + 127) / 128;
     const int sp = splits > 0 ? splits : choose_splits(tiles, K / 64, m->num_sms);
+    Buffers scratch;
     float* partial = nullptr;
-    WK_CUDA_CHECK(cudaMalloc(&partial, (size_t)sp * rows_x * N * 4));
+    WK_CHECK(scratch.dmalloc(&partial, (size_t)sp * rows_x * N, false));
     GemmDesc g;
     memset(&g, 0, sizeof(g));
     g.a = w; g.a_rows = N; g.a_cols = K; g.a_ld = K; g.a_batches = 1;
@@ -1013,7 +1052,6 @@ wk_status wk_test_gemm_splitk(wk_model* m, const void* w, const void* x, float* 
         cudaError_t e = cudaStreamSynchronize(m->stream);
         if (e != cudaSuccess) { set_error("wk_test_gemm_splitk: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     }
-    cudaFree(partial);
     return r;
 }
 
@@ -1032,11 +1070,11 @@ wk_status wk_test_cross_attention(wk_model* m, const float* q, const void* kcros
     if (!m || !q || !kcross || !vcross || !out || B < 1 || H < 1 || H > 32) { set_error("wk_test_cross_attention: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
+    Buffers scratch;
     float* zero = nullptr;
-    WK_CHECK(dmalloc(&zero, (size_t)H * 64));
+    WK_CHECK(scratch.dmalloc(&zero, (size_t)H * 64));
     wk_status r = decoder_cross_attention(q, 1, B, zero, kcross, vcross, out, B, H, T, dtype, m->stream, done);
     cudaError_t e = cudaStreamSynchronize(m->stream);
-    cudaFree(zero);
     if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     return r;
 }
@@ -1047,11 +1085,11 @@ wk_status wk_test_cross_attention_shared(wk_model* m, const float* q, const void
     if (!m || !q || !kcross || !vcross || !out || B < 1 || H < 1 || H > 32 || kv_div < 1) { set_error("wk_test_cross_attention_shared: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
+    Buffers scratch;
     float* zero = nullptr;
-    WK_CHECK(dmalloc(&zero, (size_t)H * 64));
+    WK_CHECK(scratch.dmalloc(&zero, (size_t)H * 64));
     wk_status r = decoder_cross_attention(q, 1, B, zero, kcross, vcross, out, B, H, T, dtype, m->stream, done, nullptr, 0, kv_div);
     cudaError_t e = cudaStreamSynchronize(m->stream);
-    cudaFree(zero);
     if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention_shared: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     return r;
 }
@@ -1067,13 +1105,13 @@ wk_status wk_test_cross_attention_fp8(wk_model* m, const float* q, const uint8_t
     }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
+    Buffers scratch;
     float* zero = nullptr;
-    WK_CHECK(dmalloc(&zero, (size_t)H * 64));
+    WK_CHECK(scratch.dmalloc(&zero, (size_t)H * 64));
     const uint32_t all_heads = H == 32 ? 0xffffffffu : (1u << H) - 1u;
     wk_status r = decoder_cross_attention(q, 1, B, zero, kcodes, vcodes, out, B, H, T, dtype, m->stream, done, align_out, align_out ? all_heads : 0u,
                                           kv_div, kscale, vscale);
     cudaError_t e = cudaStreamSynchronize(m->stream);
-    cudaFree(zero);
     if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention_fp8: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     return r;
 }
@@ -1085,11 +1123,11 @@ wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, vo
     if (!m || !qkv || !kcache || !vcache || !pos || !out || B < 1 || H < 1) { set_error("wk_test_self_attention: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
+    Buffers scratch;
     float* zero = nullptr;
-    WK_CHECK(dmalloc(&zero, (size_t)H * 64));
+    WK_CHECK(scratch.dmalloc(&zero, (size_t)H * 64));
     wk_status r = decoder_self_attention(qkv, 1, B, zero, zero, kcache, vcache, pos, done, out, B, H, kKvMaxLen, dtype, m->stream);
     cudaError_t e = cudaStreamSynchronize(m->stream);
-    cudaFree(zero);
     if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_self_attention: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     return r;
 }

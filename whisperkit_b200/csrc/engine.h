@@ -16,32 +16,6 @@ constexpr int kWindowSamples = 480000;  // Constants.defaultWindowSamples (Model
 
 static inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
 
-#define WK_CHECK(expr)                    \
-    do {                                  \
-        wk_status _s = (expr);            \
-        if (_s != WK_OK) return _s;       \
-    } while (0)
-
-template <typename T>
-static wk_status dmalloc(T** p, size_t n, bool zero = true) {
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T));
-    if (e != cudaSuccess) {
-        set_error("cudaMalloc(%zu bytes) failed: %s", n * sizeof(T), cudaGetErrorString(e));
-        return WK_ERR_CUDA;
-    }
-    if (zero) {
-        e = cudaMemset(*p, 0, n * sizeof(T));
-        if (e != cudaSuccess) { set_error("cudaMemset failed: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
-    }
-    return WK_OK;
-}
-static inline wk_status alloc16(void** p, size_t n) {
-    uint16_t* q = nullptr;
-    wk_status s = dmalloc(&q, n);
-    *p = q;
-    return s;
-}
-
 struct LayerNormW { float* g = nullptr; float* b = nullptr; };
 struct EncLayer {
     LayerNormW ln1, ln2;
@@ -63,6 +37,7 @@ struct DecLayer {
 // Mel + encoder activations for up to max_batch windows.  The model keeps one for the piecewise API (wk_mel / wk_encode, serialised by
 // wk_model::api_mu); every session allocates its own on first use, so sessions on different host threads encode concurrently.
 struct EncWorkspace {
+    Buffers mem;
     int max_batch = 0;
     float* pcm_dev = nullptr; int32_t* nvalid_dev = nullptr; int32_t* gmax = nullptr;
     void* mel = nullptr;       // f16 [Bm][3002][128]
@@ -85,6 +60,8 @@ struct wk_tensor {
 };
 
 struct wk_model {
+    ~wk_model();   // destroys the stream and events; the caller has made the model's device current and drained it
+    wk::Buffers mem;                 // weights and mel tables
     wk_model_config cfg;
     int device = 0;
     int num_sms = 132;
@@ -103,12 +80,12 @@ struct wk_model {
     std::vector<wk::DecLayer> dec;
     wk::LayerNormW dec_ln;
     void* wckv = nullptr; float* bckv = nullptr;         // [2L*d][d], [2L*d]
-    wk::MelTables* mel_tables = nullptr;
+    wk::MelTables mel_tables = {};
     wk::EncWorkspace ws;                                 // allocated on the first wk_mel / wk_encode
     // alignment heads (word timestamps): per decoder layer a head bit mask and the first scratch slot of the layer
     std::vector<uint32_t> align_mask; std::vector<int> align_base; int n_align_slots = 0; int has_alignment_heads = 0;
     float timings[6] = {0, 0, 0, 0, 0, 0};
-    cudaEvent_t ev[8];
+    cudaEvent_t ev[8] = {};
     // cross-attention K/V cache storage: the model dtype, or FP8 E4M3 with per-row scales (wk_model_set_cross_kv_dtype); fixed once the
     // first session exists.  Both fields are read and written under api_mu.
     bool cross_kv_fp8 = false;
@@ -118,7 +95,6 @@ struct wk_model {
 namespace wk {
 
 wk_status enc_ws_ensure(wk_model* m, EncWorkspace* ws, int max_batch);
-void enc_ws_free(EncWorkspace* ws);
 // PCM rows (host or device) -> staged in ws->pcm_dev when needed -> log-mel into mel_out ([n][3002][128] f16), all on `stream`
 wk_status mel_run(wk_model* m, EncWorkspace* ws, const float* pcm, int64_t n, int64_t stride, const int32_t* samples_per_window_host,
                   void* mel_out, cudaStream_t stream);

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "../../include/wkb200.h"
 
 namespace wk {
@@ -11,6 +13,52 @@ namespace wk {
 void set_error(const char* fmt, ...);
 const char* last_error_cstr();
 void count_launch(int n = 1);
+
+#define WK_CHECK(expr)                    \
+    do {                                  \
+        wk_status _s = (expr);            \
+        if (_s != WK_OK) return _s;       \
+    } while (0)
+
+// Owner of device (cudaMalloc) and pinned host (cudaHostAlloc) buffers: everything allocated through it is released when it is
+// destroyed, so an object that holds one frees its memory on every path, a half-built one included.  Structs handed to kernels keep raw
+// pointers into it.  Releasing does not synchronise: the holder drains the streams that use the buffers first.  Every byte it holds is
+// counted in the process-wide totals of wk_debug_live_bytes.
+class Buffers {
+public:
+    Buffers() = default;
+    Buffers(const Buffers&) = delete;
+    Buffers& operator=(const Buffers&) = delete;
+    Buffers(Buffers&& o) noexcept { live_.swap(o.live_); }
+    Buffers& operator=(Buffers&& o) noexcept {
+        if (this != &o) { release_all(); live_.swap(o.live_); }
+        return *this;
+    }
+    ~Buffers() { release_all(); }
+
+    // n elements of T on the device, zero-filled unless zero == false; alloc16: n elements of a 16-bit dtype, zero-filled
+    template <typename T>
+    wk_status dmalloc(T** p, size_t n, bool zero = true) { return alloc(reinterpret_cast<void**>(p), n * sizeof(T), false, zero); }
+    wk_status alloc16(void** p, size_t n) { return alloc(p, n * 2, false, true); }
+    // n elements of T in pinned host memory, zero-filled
+    template <typename T>
+    wk_status pinned(T** p, size_t n) { return alloc(reinterpret_cast<void**>(p), n * sizeof(T), true, true); }
+    // *p (null or a buffer of this owner) holds at least n elements of T afterwards.  A smaller buffer is released, after `drain` (when not
+    // null) has finished, and replaced by one that is not zero-filled; *moved tells whether that happened.
+    template <typename T>
+    wk_status grow(T** p, size_t n, cudaStream_t drain = nullptr, bool* moved = nullptr) {
+        return regrow(reinterpret_cast<void**>(p), n * sizeof(T), false, drain, moved);
+    }
+    template <typename T>
+    wk_status grow_pinned(T** p, size_t n) { return regrow(reinterpret_cast<void**>(p), n * sizeof(T), true, nullptr, nullptr); }
+
+private:
+    struct Buf { void* p; size_t bytes; bool pinned; };
+    std::vector<Buf> live_;
+    wk_status alloc(void** p, size_t bytes, bool pinned, bool zero);
+    wk_status regrow(void** p, size_t bytes, bool pinned, cudaStream_t drain, bool* moved);
+    void release_all();
+};
 
 // ---------------------------------------------------------------- GEMM (gemm_wgmma.cu)
 enum GemmMode {
@@ -70,9 +118,17 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream);
 int wgmma_tile_n(int bn);
 
 // ---------------------------------------------------------------- mel (mel.cu)
-struct MelTables;  // device tables (window, twiddles, sparse filterbank)
-wk_status mel_tables_create(int n_mels, MelTables** out);
-void mel_tables_free(MelTables* t);
+namespace mel { struct cf; }
+struct MelTables {   // device tables of the log-mel kernel, which takes them by value
+    int n_mels;
+    float* win;        // [400] window
+    mel::cf* tw400;    // [25][9] twiddles
+    mel::cf* tw25;     // [5][5]
+    float* wts;        // [kMaxTaps][128] sparse filterbank
+    int* start;        // [128]
+};
+// uploads the tables for n_mels channels into buffers of `mem`
+wk_status mel_tables_create(int n_mels, Buffers& mem, MelTables* out);
 // pcm [n_windows, stride] f32 device; out [n_windows, 3002, 128] f16 (rows 0 and 3001 are the conv zero pad, mel
 // channels >= n_mels zero); gmax scratch [n_windows] int32
 wk_status mel_forward(const MelTables* t, const float* pcm, int64_t n_windows, int64_t stride, const int32_t* n_valid,

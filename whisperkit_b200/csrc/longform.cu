@@ -10,12 +10,13 @@
 #include <algorithm>
 #include <string>
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
 
-#include "kernels.h"
+#include "engine.h"
 #include "longform.h"
 
 using namespace wk;
@@ -232,24 +233,9 @@ constexpr int kRoundCap = 256;   // windows per round of the stream loop (host s
 
 // pinned host staging, kept for the life of the thread that transcribes (allocation of half a gigabyte of pinned memory costs ~0.1 s)
 struct HostStage {
-    float* pcm = nullptr; size_t pcm_bytes = 0;
-    uint16_t* align = nullptr; size_t align_bytes = 0;
-    wk_status ensure(size_t need_pcm, size_t need_align) {
-        if (need_pcm > pcm_bytes) {
-            if (pcm) cudaFreeHost(pcm);
-            pcm = nullptr; pcm_bytes = 0;
-            if (cudaHostAlloc((void**)&pcm, need_pcm, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_error("pinned staging of %zu bytes failed", need_pcm); return WK_ERR_CUDA; }
-            pcm_bytes = need_pcm;
-        }
-        if (need_align > align_bytes) {
-            if (align) cudaFreeHost(align);
-            align = nullptr; align_bytes = 0;
-            if (cudaHostAlloc((void**)&align, need_align, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_error("pinned staging of %zu bytes failed", need_align); return WK_ERR_CUDA; }
-            align_bytes = need_align;
-        }
-        return WK_OK;
-    }
-    ~HostStage() { if (pcm) cudaFreeHost(pcm); if (align) cudaFreeHost(align); }
+    Buffers mem;
+    float* pcm = nullptr;
+    uint16_t* align = nullptr;
 };
 HostStage& host_stage() { static thread_local HostStage hs; return hs; }
 
@@ -351,7 +337,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         while (u.done && u.clip + 1 < nc) { ++u.clip; u.seek = u.clips[2 * u.clip]; u.done = !(u.seek < u.clips[2 * u.clip + 1] - window_padding && u.seek < u.n); }
         if (!u.done && u.seek < u.base) { set_error("seek loop: stream %d seeks to sample %lld before its first held sample %lld", u.stream, (long long)u.seek, (long long)u.base); return WK_ERR_INVALID_ARGUMENT; }
     }
-    wk_transcription* T = new wk_transcription();
+    std::unique_ptr<wk_transcription> T(new wk_transcription());
     T->lang.assign(n_streams, -1); T->lang_logprob.assign(n_streams, 0.f); T->lang_at.assign(n_streams, -1);
     // One round = the next window of EVERY unfinished unit (up to kRoundCap): the window scheduler behind wk_transcribe_windows keeps the
     // session's decode slots full and runs the mel + encoder pass of the following windows under the running decode, so a round is not
@@ -359,8 +345,8 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
     // search, DTW, word timing) runs on a pool of host threads.
     const int round_cap = std::max(max_batch, kRoundCap);
     HostStage& hs = host_stage();
-    rc = hs.ensure((size_t)round_cap * kWindow * sizeof(float), o->word_timestamps ? (size_t)round_cap * info.kv_max_len * info.n_audio_ctx * 2 : 0);
-    if (rc != WK_OK) { delete T; return rc; }
+    WK_CHECK(hs.mem.grow_pinned(&hs.pcm, (size_t)round_cap * kWindow));
+    if (o->word_timestamps) WK_CHECK(hs.mem.grow_pinned(&hs.align, (size_t)round_cap * info.kv_max_len * info.n_audio_ctx));
     float* batch = hs.pcm;
     std::vector<int32_t> valid(round_cap);
     std::vector<wk_decode_result> res(round_cap);
@@ -387,13 +373,13 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         memset(&bo, 0, sizeof(bo));
         bo.opts = o; bo.n_opts = 1; bo.prompt = prompt; bo.n_prompt = n_prompt; bo.best_of = best_of;
         rc = transcribe_windows_stop(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data(), stop);
-        if (rc != WK_OK) { delete T; return rc; }
+        if (rc != WK_OK) return rc;
         T->windows += (int)active.size();
         if (o->detect_language) {   // TranscriptionResult.language: the stream keeps the language of its last detecting window
             std::vector<int32_t> lt(active.size());
             std::vector<float> ll(active.size());
             rc = wk_session_languages(s, 0, (int32_t)active.size(), lt.data(), ll.data());
-            if (rc != WK_OK) { delete T; return rc; }
+            if (rc != WK_OK) return rc;
             for (size_t k = 0; k < active.size(); ++k) {
                 const Unit& u = units[active[k]];
                 const int64_t at = u.offset + u.seek;
@@ -404,7 +390,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         std::vector<float> nsp(active.size(), 0.f);
         if (o->compute_no_speech_prob) {
             rc = wk_session_no_speech_probs(s, 0, (int32_t)active.size(), nsp.data());
-            if (rc != WK_OK) { delete T; return rc; }
+            if (rc != WK_OK) return rc;
             for (float& v : nsp) if (isnan(v)) v = 0.f;
         }
         const int cols = info.n_audio_ctx;
@@ -412,7 +398,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
             for (size_t k = 0; k < active.size(); ++k) {
                 const int have = std::min(res[k].n_tokens, info.kv_max_len);
                 rc = wk_session_alignment_weights_f16(s, (int32_t)k, have, hs.align + (size_t)k * info.kv_max_len * cols, k + 1 == active.size() ? 1 : 0);
-                if (rc != WK_OK) { delete T; return rc; }
+                if (rc != WK_OK) return rc;
             }
         }
         std::string worker_error;
@@ -486,7 +472,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
             }
             return WK_OK;
         }, &worker_error);
-        if (rc != WK_OK) { set_error("%s", worker_error.c_str()); delete T; return rc; }
+        if (rc != WK_OK) { set_error("%s", worker_error.c_str()); return rc; }
     }
     // flatten: streams in order, units (chunks) in order, chunk offsets applied (updateSegmentTimings, AudioChunker.swift:14-39)
     std::vector<int> next_id(n_streams, 0);
@@ -510,7 +496,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
             T->segments.push_back(sg);
         }
     }
-    *out = T;
+    *out = T.release();
     return WK_OK;
 }
 

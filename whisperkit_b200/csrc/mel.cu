@@ -23,15 +23,6 @@ namespace wk {
 
 using namespace mel;
 
-struct MelTables {
-    int n_mels;
-    float* win;      // [400]
-    cf* tw400;       // [25][9]
-    cf* tw25;        // [5][5]
-    float* wts;      // [kMaxTaps][128]
-    int* start;      // [128]
-};
-
 static constexpr int kPStride = kBins;  // floats per frame in the power buffer
 static constexpr int kRegionA = (kF * kPStride > kSamplesPerCta ? kF * kPStride : kSamplesPerCta);  // samples | power
 
@@ -135,7 +126,7 @@ mel_pass2_kernel(uint16_t* __restrict__ io, const int* __restrict__ gmax, int n_
 }
 
 // ------------------------------------------------------------------------------------------------
-wk_status mel_tables_create(int n_mels, MelTables** out) {
+wk_status mel_tables_create(int n_mels, Buffers& mem, MelTables* t) {
     if (n_mels != 80 && n_mels != 128) {
         set_error("mel: n_mels must be 80 or 128 (got %d)", n_mels);
         return WK_ERR_INVALID_ARGUMENT;
@@ -144,27 +135,19 @@ wk_status mel_tables_create(int n_mels, MelTables** out) {
     std::vector<cf> tw400, tw25;
     std::vector<int> start;
     mel_host_tables(n_mels, win, tw400, tw25, wts, start);
-    MelTables* t = new MelTables();
     t->n_mels = n_mels;
-    WK_CUDA_CHECK(cudaMalloc(&t->win, win.size() * sizeof(float)));
-    WK_CUDA_CHECK(cudaMalloc(&t->tw400, tw400.size() * sizeof(cf)));
-    WK_CUDA_CHECK(cudaMalloc(&t->tw25, tw25.size() * sizeof(cf)));
-    WK_CUDA_CHECK(cudaMalloc(&t->wts, wts.size() * sizeof(float)));
-    WK_CUDA_CHECK(cudaMalloc(&t->start, start.size() * sizeof(int)));
+    WK_CHECK(mem.dmalloc(&t->win, win.size(), false));
+    WK_CHECK(mem.dmalloc(&t->tw400, tw400.size(), false));
+    WK_CHECK(mem.dmalloc(&t->tw25, tw25.size(), false));
+    WK_CHECK(mem.dmalloc(&t->wts, wts.size(), false));
+    WK_CHECK(mem.dmalloc(&t->start, start.size(), false));
     WK_CUDA_CHECK(cudaMemcpy(t->win, win.data(), win.size() * sizeof(float), cudaMemcpyHostToDevice));
     WK_CUDA_CHECK(cudaMemcpy(t->tw400, tw400.data(), tw400.size() * sizeof(cf), cudaMemcpyHostToDevice));
     WK_CUDA_CHECK(cudaMemcpy(t->tw25, tw25.data(), tw25.size() * sizeof(cf), cudaMemcpyHostToDevice));
     WK_CUDA_CHECK(cudaMemcpy(t->wts, wts.data(), wts.size() * sizeof(float), cudaMemcpyHostToDevice));
     WK_CUDA_CHECK(cudaMemcpy(t->start, start.data(), start.size() * sizeof(int), cudaMemcpyHostToDevice));
     WK_CUDA_CHECK(cudaFuncSetAttribute(mel_pass1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MelSmem)));
-    *out = t;
     return WK_OK;
-}
-
-void mel_tables_free(MelTables* t) {
-    if (!t) return;
-    cudaFree(t->win); cudaFree(t->tw400); cudaFree(t->tw25); cudaFree(t->wts); cudaFree(t->start);
-    delete t;
 }
 
 wk_status mel_forward(const MelTables* t, const float* pcm, int64_t n_windows, int64_t stride, const int32_t* n_valid,

@@ -26,6 +26,8 @@
 using namespace wk;
 
 struct wk_session {
+    ~wk_session();   // drains and destroys the streams, events and graphs; the owners release the buffers after it
+    Buffers mem;              // every device and pinned buffer below
     wk_model* m = nullptr;
     int max_batch = 0;        // decode slots
     int batch = 0;            // rows the step runs over: slots [0, batch / G), G = max(beam, best_of) rows per slot
@@ -66,16 +68,15 @@ struct wk_session {
     // word timestamps: per-head softmax rows of the current step, the [S][224][T] Float16 alignmentWeights of the slots, and the per-window
     // copies handed out by wk_session_alignment_weights
     float* align_scratch = nullptr; void* align_w = nullptr; int align_slots = 0; bool align_on = false;
-    // align_store_cap is in bytes; align_store_rows rows per window: 224 after a decode, 225 after an align call (row t + 1 = position t)
-    void* align_store = nullptr; int64_t align_store_cap = 0, align_store_n = 0; int align_store_rows = kKvMaxLen;
-    // teacher-forced alignment pass (wk_align_tokens / wk_align_windows): buffers for `al_cap` windows of 224 rows - the f32 alignment
-    // accumulator [rows][T], per-head softmax (max, sum) [H][rows][2], row tokens, sequence lengths, token log-probs, the QKV biases [L][3d];
-    // and the log-probs of the last call on the host, 224 per window
-    int al_cap = 0;
+    // align_store_rows rows per window: 224 after a decode, 225 after an align call (row t + 1 = position t)
+    uint8_t* align_store = nullptr; int64_t align_store_n = 0; int align_store_rows = kKvMaxLen;
+    // teacher-forced alignment pass (wk_align_tokens / wk_align_windows): buffers for the windows of one chunk, 224 rows each - the f32
+    // alignment accumulator [rows][T], per-head softmax (max, sum) [H][rows][2], row tokens, sequence lengths, token log-probs, the QKV
+    // biases [L][3d]; and the log-probs of the last call on the host, 224 per window
     float *al_acc = nullptr, *al_stats = nullptr, *al_lp = nullptr, *al_bqkv = nullptr;
     int32_t *al_tok = nullptr, *al_seq = nullptr;
     std::vector<float> win_align_lp;
-    cudaEvent_t ev_enc = nullptr, ev_adm = nullptr, ev_stage = nullptr, ev_t[10];
+    cudaEvent_t ev_enc = nullptr, ev_adm = nullptr, ev_stage = nullptr, ev_t[10] = {};
     // beam search (allocated on the first call that asks for it)
     BeamState bs = BeamState(); int bs_cap_rows = 0;
     int32_t *h_n_fin = nullptr, *h_fin_len = nullptr, *h_fin_tokens = nullptr; float *h_fin_score = nullptr, *h_fin_lps = nullptr, *h_sum_lp = nullptr;
@@ -83,7 +84,25 @@ struct wk_session {
     std::vector<int> slot_window, slot_try;
     int64_t stats[4] = {0, 0, 0, 0};   // of the last batched call: step launches, sum of live rows over them, admissions, ladder re-admissions
     AudioWs* audio = nullptr;          // wk_audio_load / wk_audio_convert workspace (audio.cu)
+    int32_t* pos100 = nullptr;         // wk_bench_kernel's self-attention positions (all 100)
 };
+
+// The cached step graphs bake in the call's shape and the session's buffer pointers: dropped, they are captured again on the next step
+static void drop_graphs(wk_session* s) {
+    if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }
+    if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
+}
+
+wk_session::~wk_session() {
+    if (stream) cudaStreamSynchronize(stream);
+    if (enc_stream) cudaStreamSynchronize(enc_stream);
+    drop_graphs(this);
+    audio_ws_free(audio);
+    for (cudaEvent_t e : {ev_enc, ev_adm, ev_stage}) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ev_t) if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+    if (enc_stream) cudaStreamDestroy(enc_stream);
+}
 
 namespace wk {
 
@@ -350,8 +369,7 @@ static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bo
     const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_beam != beam_key ||
                        memcmp(&s->graph_st, st, sizeof(*st)) != 0;
     if (stale) {
-        if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }
-        if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
+        drop_graphs(s);
         s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_st = *st; s->graph_beam = beam_key;
     }
     cudaGraphExec_t& exec = check_done ? s->graph_exec : s->graph_exec_live;
@@ -398,12 +416,7 @@ static const wk_decode_opts& opts_of(const wk_batch_opts* bo, int64_t w) { retur
 
 // the per-window alignmentWeights handed out by wk_session_alignment_weights: n_windows x rows x T Float16
 static wk_status ensure_align_store(wk_session* s, int64_t n_windows, int rows) {
-    const int64_t need = n_windows * rows * s->m->cfg.n_audio_ctx * 2;
-    if (s->align_store_cap < need) {
-        if (s->align_store) { WK_CUDA_CHECK(cudaStreamSynchronize(s->stream)); cudaFree(s->align_store); s->align_store = nullptr; }
-        WK_CUDA_CHECK(cudaMalloc(&s->align_store, (size_t)need));
-        s->align_store_cap = need;
-    }
+    WK_CHECK(s->mem.grow(&s->align_store, (size_t)n_windows * rows * s->m->cfg.n_audio_ctx * 2, s->stream));
     s->align_store_n = n_windows;
     s->align_store_rows = rows;
     return WK_OK;
@@ -412,40 +425,33 @@ static wk_status ensure_align_store(wk_session* s, int64_t n_windows, int rows) 
 static wk_status ensure_align(wk_session* s, int64_t n_windows) {
     wk_model* m = s->m;
     const size_t T = m->cfg.n_audio_ctx;
-    if (!s->align_w) WK_CUDA_CHECK(cudaMalloc(&s->align_w, (size_t)s->max_batch * kKvMaxLen * T * 2));
-    if (!s->align_scratch || s->align_slots != m->n_align_slots) {
-        if (s->align_scratch) { WK_CUDA_CHECK(cudaStreamSynchronize(s->stream)); cudaFree(s->align_scratch); s->align_scratch = nullptr; }
-        WK_CUDA_CHECK(cudaMalloc((void**)&s->align_scratch, (size_t)std::max(1, m->n_align_slots) * s->max_batch * T * 4));
-        s->align_slots = m->n_align_slots;
-        if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }   // the scratch pointer is baked into the graphs
-        if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
-    }
+    if (!s->align_w) WK_CHECK(s->mem.alloc16(&s->align_w, (size_t)s->max_batch * kKvMaxLen * T));
+    bool moved = false;
+    WK_CHECK(s->mem.grow(&s->align_scratch, (size_t)std::max(1, m->n_align_slots) * s->max_batch * T, s->stream, &moved));
+    if (moved || s->align_slots != m->n_align_slots) drop_graphs(s);   // the scratch pointer and the head slots are baked into the graphs
+    s->align_slots = m->n_align_slots;
     return ensure_align_store(s, n_windows, kKvMaxLen);
 }
 
 static wk_status ensure_beam(wk_session* s) {
     if (s->bs_cap_rows >= s->max_batch) return WK_OK;
     const int S = s->max_batch, G = S / 2 + 1;
-    WK_CHECK(dmalloc(&s->bs.sum_lp, S));
-    WK_CHECK(dmalloc(&s->bs.cand_tok, (size_t)S * (kMaxBeam + 1)));
-    WK_CHECK(dmalloc(&s->bs.cand_lp, (size_t)S * (kMaxBeam + 1)));
-    WK_CHECK(dmalloc(&s->bs.anc, (size_t)S * kKvMaxLen));
-    WK_CHECK(dmalloc(&s->bs.fin_tokens, (size_t)G * kMaxCand * kKvMaxLen));
-    WK_CHECK(dmalloc(&s->bs.fin_lps, (size_t)G * kMaxCand * kKvMaxLen));
-    WK_CHECK(dmalloc(&s->bs.fin_len, (size_t)G * kMaxCand));
-    WK_CHECK(dmalloc(&s->bs.fin_score, (size_t)G * kMaxCand));
-    WK_CHECK(dmalloc(&s->bs.n_fin, G));
-    auto pinned = [&](void** p, size_t bytes) -> wk_status {
-        cudaError_t e = cudaHostAlloc(p, bytes, cudaHostAllocDefault);
-        if (e != cudaSuccess) { set_error("cudaHostAlloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return WK_ERR_CUDA; }
-        return WK_OK;
-    };
-    WK_CHECK(pinned((void**)&s->h_n_fin, (size_t)G * 4));
-    WK_CHECK(pinned((void**)&s->h_fin_len, (size_t)G * kMaxCand * 4));
-    WK_CHECK(pinned((void**)&s->h_fin_score, (size_t)G * kMaxCand * 4));
-    WK_CHECK(pinned((void**)&s->h_fin_tokens, (size_t)G * kMaxCand * kKvMaxLen * 4));
-    WK_CHECK(pinned((void**)&s->h_fin_lps, (size_t)G * kMaxCand * kKvMaxLen * 4));
-    WK_CHECK(pinned((void**)&s->h_sum_lp, (size_t)S * 4));
+    Buffers& b = s->mem;
+    WK_CHECK(b.dmalloc(&s->bs.sum_lp, S));
+    WK_CHECK(b.dmalloc(&s->bs.cand_tok, (size_t)S * (kMaxBeam + 1)));
+    WK_CHECK(b.dmalloc(&s->bs.cand_lp, (size_t)S * (kMaxBeam + 1)));
+    WK_CHECK(b.dmalloc(&s->bs.anc, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&s->bs.fin_tokens, (size_t)G * kMaxCand * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&s->bs.fin_lps, (size_t)G * kMaxCand * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&s->bs.fin_len, (size_t)G * kMaxCand));
+    WK_CHECK(b.dmalloc(&s->bs.fin_score, (size_t)G * kMaxCand));
+    WK_CHECK(b.dmalloc(&s->bs.n_fin, G));
+    WK_CHECK(b.pinned(&s->h_n_fin, G));
+    WK_CHECK(b.pinned(&s->h_fin_len, (size_t)G * kMaxCand));
+    WK_CHECK(b.pinned(&s->h_fin_score, (size_t)G * kMaxCand));
+    WK_CHECK(b.pinned(&s->h_fin_tokens, (size_t)G * kMaxCand * kKvMaxLen));
+    WK_CHECK(b.pinned(&s->h_fin_lps, (size_t)G * kMaxCand * kKvMaxLen));
+    WK_CHECK(b.pinned(&s->h_sum_lp, S));
     s->bs_cap_rows = S;
     return WK_OK;
 }
@@ -590,12 +596,10 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     if (!bo->status)
         for (int64_t w = 0; w < n; ++w) if (status[w] != WK_OK) { set_error("%s", first_err.c_str()); return status[w]; }
     if (sup_pool.size() > s->suppress_cap) {
-        WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
-        if (s->suppress_dev) cudaFree(s->suppress_dev);
-        s->suppress_cap = std::max<size_t>(4096, sup_pool.size() * 2);
-        WK_CHECK(dmalloc(&s->suppress_dev, s->suppress_cap));
-        if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }   // pool pointer is baked into the graphs
-        if (s->graph_exec_live) { cudaGraphExecDestroy(s->graph_exec_live); s->graph_exec_live = nullptr; }
+        const size_t cap = std::max<size_t>(4096, sup_pool.size() * 2);
+        WK_CHECK(s->mem.grow(&s->suppress_dev, cap, s->stream));
+        s->suppress_cap = cap;
+        drop_graphs(s);   // pool pointer is baked into the graphs
     }
     if (!sup_pool.empty()) WK_CUDA_CHECK(cudaMemcpyAsync(s->suppress_dev, sup_pool.data(), sup_pool.size() * 4, cudaMemcpyHostToDevice, s->stream));
     if (any_detect) WK_CUDA_CHECK(cudaMemcpyAsync(s->lang_dev, lang_list.data(), lang_list.size() * 4, cudaMemcpyHostToDevice, s->stream));
@@ -986,19 +990,15 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
 static constexpr int kAlignRows = kKvMaxLen + 1;   // alignment rows per window: row t + 1 for input position t, t < 224
 
 static wk_status ensure_align_pass(wk_session* s, int nw) {
-    if (s->al_cap >= nw) return WK_OK;
     const wk_model_config& c = s->m->cfg;
-    WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
-    void* old[] = {s->al_acc, s->al_stats, s->al_lp, s->al_bqkv, s->al_tok, s->al_seq};
-    for (void* p : old) if (p) cudaFree(p);
     const size_t R = (size_t)nw * kKvMaxLen;
-    WK_CHECK(dmalloc(&s->al_acc, R * c.n_audio_ctx, false));
-    WK_CHECK(dmalloc(&s->al_stats, R * c.n_heads * 2, false));
-    WK_CHECK(dmalloc(&s->al_lp, R));
-    WK_CHECK(dmalloc(&s->al_bqkv, (size_t)c.dec_layers * 3 * c.d_model));
-    WK_CHECK(dmalloc(&s->al_tok, R));
-    WK_CHECK(dmalloc(&s->al_seq, (size_t)nw));
-    s->al_cap = nw;
+    Buffers& b = s->mem;
+    WK_CHECK(b.grow(&s->al_acc, R * c.n_audio_ctx, s->stream));
+    WK_CHECK(b.grow(&s->al_stats, R * c.n_heads * 2, s->stream));
+    WK_CHECK(b.grow(&s->al_lp, R, s->stream));
+    WK_CHECK(b.grow(&s->al_bqkv, (size_t)c.dec_layers * 3 * c.d_model, s->stream));
+    WK_CHECK(b.grow(&s->al_tok, R, s->stream));
+    WK_CHECK(b.grow(&s->al_seq, (size_t)nw, s->stream));
     return WK_OK;
 }
 
@@ -1159,7 +1159,7 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     const wk_model_config& c = m->cfg;
     const int d = c.d_model, H = c.n_heads, L = c.dec_layers, T = c.n_audio_ctx, S = max_batch;
-    wk_session* s = new wk_session();
+    std::unique_ptr<wk_session> s(new wk_session());   // released on any failure below
     s->m = m;
     s->max_batch = S;
     WK_CUDA_CHECK(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
@@ -1170,16 +1170,17 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
         m->session_created = true;
         s->ckv_fp8 = m->cross_kv_fp8;
     }
+    Buffers& b = s->mem;
     if (s->ckv_fp8) {
         uint8_t* codes = nullptr;
-        WK_CHECK(dmalloc(&codes, (size_t)2 * L * S * H * T * 64));
+        WK_CHECK(b.dmalloc(&codes, (size_t)2 * L * S * H * T * 64));
         s->cross_kv = codes;
-        WK_CHECK(dmalloc(&s->cross_scale, (size_t)2 * L * S * H * T));
+        WK_CHECK(b.dmalloc(&s->cross_scale, (size_t)2 * L * S * H * T));
     } else {
-        WK_CHECK(alloc16(&s->cross_kv, (size_t)2 * L * S * H * T * 64));
+        WK_CHECK(b.alloc16(&s->cross_kv, (size_t)2 * L * S * H * T * 64));
     }
-    WK_CHECK(alloc16(&s->self_k, (size_t)L * S * H * kKvMaxLen * 64));
-    WK_CHECK(alloc16(&s->self_v, (size_t)L * S * H * kKvMaxLen * 64));
+    WK_CHECK(b.alloc16(&s->self_k, (size_t)L * S * H * kKvMaxLen * 64));
+    WK_CHECK(b.alloc16(&s->self_v, (size_t)L * S * H * kKvMaxLen * 64));
     // split-K partial workspace: max over the decoder GEMM shapes of splits * N
     size_t pe = 0;
     const int shapes[4][2] = {{3 * d, d}, {d, d}, {4 * d, d}, {d, 4 * d}};
@@ -1188,53 +1189,47 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
         pe = std::max(pe, (size_t)sp * sh[0]);
     }
     s->partial_elems = pe * bpm;
-    WK_CHECK(dmalloc(&s->partial, s->partial_elems));
-    WK_CHECK(dmalloc(&s->x, (size_t)bpm * d));
-    WK_CHECK(alloc16(&s->xn, (size_t)bpm * d));
-    WK_CHECK(alloc16(&s->attn, (size_t)bpm * d));
-    WK_CHECK(alloc16(&s->ffn, (size_t)bpm * 4 * d));
-    WK_CHECK(dmalloc(&s->logits, (size_t)S * c.vocab));
-    WK_CHECK(dmalloc(&s->st.tokens, (size_t)S * kKvMaxLen));
-    WK_CHECK(dmalloc(&s->st.n_tokens, S));
-    WK_CHECK(dmalloc(&s->st.logprobs, (size_t)S * kKvMaxLen));
-    WK_CHECK(dmalloc(&s->st.next_token, S));
-    WK_CHECK(dmalloc(&s->st.done, S));
-    WK_CHECK(dmalloc(&s->st.first_low, S));
-    WK_CHECK(dmalloc(&s->st.steps, S));
-    WK_CHECK(dmalloc(&s->st.input_ids, S));
-    WK_CHECK(dmalloc(&s->st.error, S));
-    WK_CHECK(dmalloc(&s->st.lang_token, S));
-    WK_CHECK(dmalloc(&s->st.lang_logprob, S));
-    WK_CHECK(dmalloc(&s->st.lang_state, S));
-    WK_CHECK(dmalloc(&s->st.no_speech, S));
-    WK_CHECK(dmalloc(&s->rp_dev, S));
+    WK_CHECK(b.dmalloc(&s->partial, s->partial_elems));
+    WK_CHECK(b.dmalloc(&s->x, (size_t)bpm * d));
+    WK_CHECK(b.alloc16(&s->xn, (size_t)bpm * d));
+    WK_CHECK(b.alloc16(&s->attn, (size_t)bpm * d));
+    WK_CHECK(b.alloc16(&s->ffn, (size_t)bpm * 4 * d));
+    WK_CHECK(b.dmalloc(&s->logits, (size_t)S * c.vocab));
+    WK_CHECK(b.dmalloc(&s->st.tokens, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&s->st.n_tokens, S));
+    WK_CHECK(b.dmalloc(&s->st.logprobs, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&s->st.next_token, S));
+    WK_CHECK(b.dmalloc(&s->st.done, S));
+    WK_CHECK(b.dmalloc(&s->st.first_low, S));
+    WK_CHECK(b.dmalloc(&s->st.steps, S));
+    WK_CHECK(b.dmalloc(&s->st.input_ids, S));
+    WK_CHECK(b.dmalloc(&s->st.error, S));
+    WK_CHECK(b.dmalloc(&s->st.lang_token, S));
+    WK_CHECK(b.dmalloc(&s->st.lang_logprob, S));
+    WK_CHECK(b.dmalloc(&s->st.lang_state, S));
+    WK_CHECK(b.dmalloc(&s->st.no_speech, S));
+    WK_CHECK(b.dmalloc(&s->rp_dev, S));
     s->st.rp = s->rp_dev;
-    WK_CHECK(dmalloc(&s->pos_dev, S));
-    WK_CHECK(dmalloc(&s->lang_dev, 4096));
+    WK_CHECK(b.dmalloc(&s->pos_dev, S));
+    WK_CHECK(b.dmalloc(&s->lang_dev, 4096));
     s->suppress_cap = 4096;
-    WK_CHECK(dmalloc(&s->suppress_dev, s->suppress_cap));
-    WK_CHECK(dmalloc(&s->d_adm_slots, S));
-    WK_CHECK(dmalloc(&s->d_adm_prompts, (size_t)S * kKvMaxLen));
-    WK_CHECK(dmalloc(&s->d_adm_rp, S));
-    auto pinned = [&](void** p, size_t bytes) -> wk_status {
-        cudaError_t e = cudaHostAlloc(p, bytes, cudaHostAllocDefault);
-        if (e != cudaSuccess) { set_error("cudaHostAlloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return WK_ERR_CUDA; }
-        memset(*p, 0, bytes);
-        return WK_OK;
-    };
-    WK_CHECK(pinned((void**)&s->h_adm_slots, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_adm_prompts, (size_t)S * kKvMaxLen * 4));
-    WK_CHECK(pinned((void**)&s->h_adm_rp, (size_t)S * sizeof(RowParams)));
-    WK_CHECK(pinned((void**)&s->h_tokens, (size_t)S * kKvMaxLen * 4));
-    WK_CHECK(pinned((void**)&s->h_logprobs, (size_t)S * kKvMaxLen * 4));
-    WK_CHECK(pinned((void**)&s->h_n_tokens, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_done, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_first_low, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_steps, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_error, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_lang_token, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_lang_logprob, (size_t)S * 4));
-    WK_CHECK(pinned((void**)&s->h_no_speech, (size_t)S * 4));
+    WK_CHECK(b.dmalloc(&s->suppress_dev, s->suppress_cap));
+    WK_CHECK(b.dmalloc(&s->d_adm_slots, S));
+    WK_CHECK(b.dmalloc(&s->d_adm_prompts, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&s->d_adm_rp, S));
+    WK_CHECK(b.pinned(&s->h_adm_slots, S));
+    WK_CHECK(b.pinned(&s->h_adm_prompts, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.pinned(&s->h_adm_rp, S));
+    WK_CHECK(b.pinned(&s->h_tokens, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.pinned(&s->h_logprobs, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.pinned(&s->h_n_tokens, S));
+    WK_CHECK(b.pinned(&s->h_done, S));
+    WK_CHECK(b.pinned(&s->h_first_low, S));
+    WK_CHECK(b.pinned(&s->h_steps, S));
+    WK_CHECK(b.pinned(&s->h_error, S));
+    WK_CHECK(b.pinned(&s->h_lang_token, S));
+    WK_CHECK(b.pinned(&s->h_lang_logprob, S));
+    WK_CHECK(b.pinned(&s->h_no_speech, S));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_enc, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_adm, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_stage, cudaEventDisableTiming));
@@ -1244,32 +1239,13 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CUDA_CHECK(cudaEventRecord(s->ev_stage, s->stream));
     s->slot_window.assign(S, -1);
     s->slot_try.assign(S, 0);
-    *out = s;
+    *out = s.release();
     return WK_OK;
 }
 
 void wk_session_free(wk_session* s) {
     if (!s) return;
     cudaSetDevice(s->m->device);
-    cudaStreamSynchronize(s->stream);
-    cudaStreamSynchronize(s->enc_stream);
-    if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-    if (s->graph_exec_live) cudaGraphExecDestroy(s->graph_exec_live);
-    void* ptrs[] = {s->cross_kv, s->cross_scale, s->self_k, s->self_v, s->partial, s->x, s->xn, s->attn, s->ffn, s->logits, s->st.tokens, s->st.n_tokens,
-                    s->st.logprobs, s->st.next_token, s->st.done, s->st.first_low, s->st.steps, s->st.input_ids, s->st.error,
-                    s->st.lang_token, s->st.lang_logprob, s->st.lang_state, s->st.no_speech, s->rp_dev,
-                    s->pos_dev, s->lang_dev, s->suppress_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, s->align_scratch, s->align_w,
-                    s->align_store, s->al_acc, s->al_stats, s->al_lp, s->al_bqkv, s->al_tok, s->al_seq};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    void* hptrs[] = {s->h_adm_slots, s->h_adm_prompts, s->h_adm_rp, s->h_tokens, s->h_logprobs, s->h_n_tokens, s->h_done, s->h_first_low, s->h_steps, s->h_error,
-                     s->h_lang_token, s->h_lang_logprob, s->h_no_speech};
-    for (void* p : hptrs) if (p) cudaFreeHost(p);
-    enc_ws_free(&s->ws);
-    audio_ws_free(s->audio);
-    cudaEventDestroy(s->ev_enc); cudaEventDestroy(s->ev_adm); cudaEventDestroy(s->ev_stage);
-    for (auto& e : s->ev_t) cudaEventDestroy(e);
-    cudaStreamDestroy(s->stream);
-    cudaStreamDestroy(s->enc_stream);
     delete s;
 }
 
@@ -1530,8 +1506,11 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
     const size_t cross_block = cross_rows * 64 * ckv_esize(s);
     const float* ksc = s->ckv_fp8 ? s->cross_scale : nullptr;
     const float* vsc = s->ckv_fp8 ? s->cross_scale + cross_rows : nullptr;
-    static int32_t* pos100 = nullptr;
-    if (which == 9 && !pos100) { std::vector<int32_t> h(256, 100); cudaMalloc(&pos100, 256 * 4); cudaMemcpy(pos100, h.data(), 256 * 4, cudaMemcpyHostToDevice); }
+    if (which == 9 && !s->pos100) {
+        std::vector<int32_t> h(256, 100);
+        WK_CHECK(s->mem.dmalloc(&s->pos100, 256, false));
+        WK_CUDA_CHECK(cudaMemcpy(s->pos100, h.data(), 256 * 4, cudaMemcpyHostToDevice));
+    }
     int rot = 0;
     auto run = [&]() -> wk_status {
         int sp;
@@ -1539,14 +1518,14 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
             case 0: return decoder_cross_attention(s->partial, 1, s->bp, m->dec[0].bcq, s->cross_kv, (char*)s->cross_kv + cross_block, s->attn, B, H, T, dt, st,
                                                    nullptr, nullptr, 0, 1, ksc, vsc);
             case 1: return gemm_wgmma(plain_gemm(s->ws.xn, M, d, m->enc[0].w1, 4 * d, dt, GEMM_OUT_T16, s->ws.ffn, 4 * d, m->enc[0].b1, 1), m->num_sms, st);
-            case 2: return mel_forward(m->mel_tables, s->ws.pcm_dev, B, kWindowSamples, nullptr, s->ws.mel, s->ws.gmax, st);
+            case 2: return mel_forward(&m->mel_tables, s->ws.pcm_dev, B, kWindowSamples, nullptr, s->ws.mel, s->ws.gmax, st);
             case 3: return encoder_attention(s->ws.qkv, s->ws.attn, B, T, H, dt, st);
             case 4: return dec_gemm(s, m->dec[0].wqkv, 3 * d, d, s->xn, &sp);
             case 5: return gemm_wgmma(plain_gemm(s->ws.xn, M, d, m->enc[0].wqkv, 3 * d, dt, GEMM_OUT_T16, s->ws.qkv, 3 * d, m->enc[0].bqkv, 0), m->num_sms, st);
             case 6: return dec_gemm(s, m->dec[0].wo, d, d, s->attn, &sp);
             case 7: return dec_gemm(s, m->dec[0].w2, d, 4 * d, s->ffn, &sp);
             case 8: return decoder_reduce_resid_ln(s->partial, choose_splits((d + 127) / 128, d / 64, m->num_sms), s->bp, m->dec[0].bo, m->dec[0].lnx.g, m->dec[0].lnx.b, s->x, s->xn, B, d, dt, st);
-            case 9: return decoder_self_attention(s->partial, 1, s->bp, m->dec[0].bq, m->dec[0].bv, s->self_k, s->self_v, pos100, nullptr, s->attn, B, H, kKvMaxLen, dt, st);
+            case 9: return decoder_self_attention(s->partial, 1, s->bp, m->dec[0].bq, m->dec[0].bv, s->self_k, s->self_v, s->pos100, nullptr, s->attn, B, H, kKvMaxLen, dt, st);
             case 14: case 15: case 16: case 17: {
                 const int r = rot++;
                 const DecLayer& l = m->dec[r % c.dec_layers];
@@ -1651,8 +1630,9 @@ wk_status wk_debug_read(wk_model* m, wk_session* s, int32_t which, int64_t offse
         for (int64_t i = 0; i < n; ++i) dst[i] = fp8_decode(codes[i]) * sc[(offset_elems + i) / 64 - r0];
         return WK_OK;
     }
+    Buffers scratch;
     float* tmp = nullptr;
-    WK_CUDA_CHECK(cudaMalloc(&tmp, n * 4));
+    WK_CHECK(scratch.dmalloc(&tmp, n, false));
     WK_CUDA_CHECK(cudaDeviceSynchronize());
     wk_status r = convert_to_16((const char*)src + offset_elems * esize(dt), dt, tmp, WK_DTYPE_F32, n, m->stream);
     if (r == WK_OK) {
@@ -1660,7 +1640,6 @@ wk_status wk_debug_read(wk_model* m, wk_session* s, int32_t which, int64_t offse
         if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
         if (e != cudaSuccess) { set_error("wk_debug_read: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     }
-    cudaFree(tmp);
     return r;
 }
 

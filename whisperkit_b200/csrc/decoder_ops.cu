@@ -431,9 +431,9 @@ wk_status decoder_self_attention(const float* partial, int splits, int Bp, const
 // cross attention for one query per (b, h) over T encoder positions.  HBM-streaming kernel: each CTA pulls its
 // contiguous K block then V block through a ring of 16000-byte bulk-copy stages (cp.async.bulk + mbarrier), a dedicated producer warp
 // keeps the ring full while 4 consumer warps compute.  K/V layout [B][H][T][64] (written head-major by the cross-KV GEMM epilogue).
-//   16-bit cache: 128-byte rows, 125 rows per stage, 4 stages; a lane takes 8 values (16 bytes) of a row.
+//   16-bit cache: 128-byte rows, 125 rows per stage, 2 stages (5 CTAs per SM); a lane takes 8 values (16 bytes) of a row.
 //   FP8 cache (FP8 = true): 64-byte rows of E4M3 codes with one f32 scale per row ([B][H][T], see fp8_row_scale), 250 rows per stage,
-//   3 stages (3 CTAs per SM, as the 16-bit kernel has); the producer first bulk-loads the block's two scale vectors, a lane widens 16
+//   2 stages (4 CTAs per SM); the producer first bulk-loads the block's two scale vectors, a lane widens 16
 //   codes exactly to f32, the K scale multiplies each key's dot product before the softmax and the V scale is folded into p for the P.V
 //   phase - the alignment export stays the normalised softmax row.
 // =====================================================================================================
@@ -441,7 +441,9 @@ template <bool FP8> struct CrossCfg {
     static constexpr int kRowBytes = FP8 ? 64 : 128;
     static constexpr int kRows = FP8 ? 250 : 125;             // rows per stage: kRows * kRowBytes = 16000 B (multiple of 16)
     static constexpr int kStageBytes = kRows * kRowBytes;
-    static constexpr int kStages = FP8 ? 3 : 4;
+    // 2 stages: 38.6 KB of shared memory per 16-bit CTA (5 per SM), 50.3 KB per FP8 CTA (4 per SM).  More, smaller CTAs per SM keep
+    // more K/V streams in flight and shorten the last wave: a deeper ring (4 stages, 3 CTAs per SM) moved the same bytes more slowly
+    static constexpr int kStages = 2;
     static constexpr int kLanesPerRow = kRowBytes / 16;       // a lane reads 16 bytes of a row
     static constexpr int kRowsPerWarp = 32 / kLanesPerRow;    // rows per warp instruction
     static constexpr int kDims = 64 / kLanesPerRow;           // values per lane

@@ -61,7 +61,8 @@ typedef struct wk_session wk_session;
 typedef struct wk_tensor wk_tensor;
 
 enum { WK_DTYPE_F32 = 0, WK_DTYPE_F16 = 1, WK_DTYPE_BF16 = 2, WK_DTYPE_I32 = 3,
-       WK_DTYPE_FP8_E4M3 = 4 /* cross-attention K/V cache only: E4M3 codes + one f32 scale per 64-value row */ };
+       WK_DTYPE_FP8_E4M3 = 4 /* storage policies only: the cross-attention K/V cache (E4M3 codes + one f32 scale per 64-value row) and the
+                                encoder's QKV / FC1 / FC2 GEMM operands (wk_model_set_encoder_dtype) */ };
 
 /* Model dimensions.  The reference reads these off the CoreML model descriptions at run time
  * (TextDecoder.swift:313-331, AudioEncoder.swift:24-38, FeatureExtractor.swift:24-38). */
@@ -191,6 +192,23 @@ wk_status wk_model_info_get(const wk_model* m, wk_model_info* out);
 wk_status wk_model_set_cross_kv_dtype(wk_model* m, int32_t dtype);
 /* The FP8 row quantizer above on the host (the code the GPU projection epilogue runs): x [rows][64] f32 -> codes [rows][64], scales [rows]. */
 wk_status wk_cross_kv_quantize_rows(const float* x, int64_t rows, uint8_t* codes, float* scales);
+/* Precision of the encoder's QKV, FC1 and FC2 GEMMs (default: the model's dtype).  WK_DTYPE_FP8_E4M3 runs them on the FP8 tensor cores
+ * (wgmma e4m3 x e4m3, f32 accumulation): activations as E4M3 codes with one f32 scale s = amax / 448 per (row, 128-column block) -
+ * the LayerNorm outputs, and FC1's GELU output quantized in its epilogue from f32 - and weights as E4M3 copies with one scale per
+ * output channel, quantized on the device from the 16-bit weights now and again whenever wk_model_set_tensor / wk_model_init_random
+ * changes one of them (about 0.63 GB more for large-v3).  Each k-block's products are promoted into the f32 accumulator with their row
+ * scale; the weight scale is applied once in the epilogue.  The conv stem, attention, the out-projection, LayerNorm statistics, the f32
+ * residual stream, the final LayerNorm and the 16-bit encoder output are unchanged, so the decoder and the cross-K/V policy see a 16-bit
+ * encoder output as before.  Every scale comes from its own row: a window's result does not depend on its batch.  Applies to every
+ * encoder call of the model (wk_encode, sessions, the window scheduler, long-form, streams, alignment).  Accepts WK_DTYPE_FP8_E4M3 or
+ * the model's own dtype; WK_ERR_INVALID_ARGUMENT once a session exists or wk_encode has run. */
+wk_status wk_model_set_encoder_dtype(wk_model* m, int32_t dtype);
+/* The encoder precision policy: WK_DTYPE_FP8_E4M3 or the model's dtype. */
+wk_status wk_model_encoder_dtype(const wk_model* m, int32_t* dtype);
+/* The FP8 quantizer on the host (the code the GPU LayerNorm, FC1 epilogue and weight quantizer run): x [rows][cols] f32 in groups of
+ * `block` columns (cols a multiple of block) -> codes [rows][cols], scales [rows][cols / block].  block = 128 is the activation rule,
+ * block = cols the weight rule (one scale per row). */
+wk_status wk_fp8_quantize_blocks(const float* x, int64_t rows, int64_t cols, int64_t block, uint8_t* codes, float* scales);
 void wk_model_free(wk_model* m);
 
 /* ---- tensors (opaque device buffers passed mel -> encoder -> decoder without touching the host) ---- */
@@ -606,6 +624,13 @@ wk_status wk_test_gemm(wk_model* m, const void* a, const void* w, const float* b
                        int32_t in_dtype, int32_t out_dtype, int32_t gelu);
 /* out[M,N] (f32, in place) += A[M,K] * W[N,K]^T + bias: the residual-update epilogue of the encoder's out-proj / FC2. */
 wk_status wk_test_gemm_residual(wk_model* m, const void* a, const void* w, const float* bias, float* out, int32_t M, int32_t N, int32_t K, int32_t in_dtype);
+/* The FP8 encoder GEMM (wk_model_set_encoder_dtype) alone: a [M][K] E4M3 codes with block scales a_scale [K / 128][round_up(M, 128)]
+ * (one per row and 128-column block), w [N][K] E4M3 with one scale per row w_scale [N]; N, K multiples of 128.  kind 0 (QKV):
+ * out [M][N] dtype = (sum_kb (a w^T)[kb] * a_scale[kb][row]) * w_scale[col] + bias; kind 1 (FC1): the same value through exact GELU,
+ * quantized per (row, 128-column block) into out [M][N] E4M3 and out_scale [N / 128][round_up(M, 128)]; kind 2 (FC2): out [M][N] f32
+ * += the value. */
+wk_status wk_test_gemm_fp8(wk_model* m, int32_t kind, const uint8_t* a, const float* a_scale, const uint8_t* w, const float* w_scale,
+                           const float* bias, void* out, float* out_scale, int32_t M, int32_t N, int32_t K, int32_t dtype);
 /* Same product through the decoder's swap-AB split-K path: out f32 [rows_x, N]. */
 wk_status wk_test_gemm_splitk(wk_model* m, const void* w, const void* x, float* out, int32_t N, int32_t rows_x, int32_t K, int32_t in_dtype, int32_t splits);
 /* Encoder attention on packed qkv [B*T, 3*d] -> out [B*T, d]. */

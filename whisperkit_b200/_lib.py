@@ -12,7 +12,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libwkb200.so")
 
 WK_DTYPE_F32, WK_DTYPE_F16, WK_DTYPE_BF16, WK_DTYPE_I32 = 0, 1, 2, 3
-WK_DTYPE_FP8_E4M3 = 4   # cross-attention K/V cache storage only
+WK_DTYPE_FP8_E4M3 = 4   # storage policies only: the cross-attention K/V cache, the encoder's QKV / FC1 / FC2 GEMM operands
 
 STATUS_NAMES = {
     0: "ok", -1: "invalidArgument", -2: "modelsUnavailable", -3: "audioProcessingFailed",
@@ -151,6 +151,9 @@ SYMBOLS = [
     ("wk_model_info_get", I32, [P, C.POINTER(wk_model_info)]),
     ("wk_model_set_cross_kv_dtype", I32, [P, I32]),
     ("wk_cross_kv_quantize_rows", I32, [P, I64, P, P]),
+    ("wk_model_set_encoder_dtype", I32, [P, I32]),
+    ("wk_model_encoder_dtype", I32, [P, P]),
+    ("wk_fp8_quantize_blocks", I32, [P, I64, I64, I64, P, P]),
     ("wk_model_free", None, [P]),
     ("wk_tensor_shape", I32, [P, PI64, PI32, PI32]),
     ("wk_tensor_to_host", I32, [P, P, I64]),
@@ -265,6 +268,7 @@ SYMBOLS = [
     ("wk_test_cross_attention_fp8", I32, [P, P, P, P, P, P, P, I32, I32, I32, I32, P, I32, P]),
     ("wk_test_self_attention", I32, [P, P, P, P, P, P, I32, I32, I32, P]),
     ("wk_test_gemm_residual", I32, [P, P, P, P, P, I32, I32, I32, I32]),
+    ("wk_test_gemm_fp8", I32, [P, I32, P, P, P, P, P, P, P, I32, I32, I32, I32]),
     ("wk_test_gemm_splitk", I32, [P, P, P, P, I32, I32, I32, I32, I32]),
     ("wk_test_attention", I32, [P, P, P, I32, I32, I32, I32]),
     ("wk_test_gemm_partial", I32, [P, P, P, P, I32, I32, I32, I32, I32, I32]),

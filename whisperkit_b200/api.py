@@ -246,21 +246,27 @@ _DT = {"f32": WK_DTYPE_F32, "f16": WK_DTYPE_F16, "bf16": WK_DTYPE_BF16}
 _CKV_DT = {"fp8": _lib.WK_DTYPE_FP8_E4M3, "f16": WK_DTYPE_F16, "bf16": WK_DTYPE_BF16}
 
 
-def _check_cross_kv_dtype(crossKVDtype: Optional[str]) -> None:
+def _check_storage_dtypes(crossKVDtype: Optional[str], encoderDtype: Optional[str] = None) -> None:
     if crossKVDtype is not None and crossKVDtype not in _CKV_DT:
         raise ValueError(f"crossKVDtype must be one of {sorted(_CKV_DT)} or None, not {crossKVDtype!r}")
+    if encoderDtype is not None and encoderDtype not in _CKV_DT:
+        raise ValueError(f"encoderDtype must be one of {sorted(_CKV_DT)} or None, not {encoderDtype!r}")
 
 
 class Model:
     """Owns a wk_model (weights + encoder workspaces on one GPU).
 
     crossKVDtype="fp8" stores the decoder's cross-attention K/V cache as E4M3 codes with one f32 scale per 64-value row
-    (wk_model_set_cross_kv_dtype): about half the cache memory and the bytes the decode loop streams; None keeps `dtype`."""
+    (wk_model_set_cross_kv_dtype): about half the cache memory and the bytes the decode loop streams; None keeps `dtype`.
+
+    encoderDtype="fp8" runs the encoder's QKV, FC1 and FC2 GEMMs on the FP8 tensor cores (wk_model_set_encoder_dtype): E4M3
+    activations with one f32 scale per (row, 128-column block), E4M3 weight copies with one scale per output channel; the encoder output
+    stays `dtype`.  None keeps `dtype`."""
 
     def __init__(self, variant: str = "large-v3", device: int = 0, max_batch: int = 16, dtype: str = "bf16",
-                 config: Optional[dict] = None, crossKVDtype: Optional[str] = None):
+                 config: Optional[dict] = None, crossKVDtype: Optional[str] = None, encoderDtype: Optional[str] = None):
         self.lib = _lib.load()
-        _check_cross_kv_dtype(crossKVDtype)
+        _check_storage_dtypes(crossKVDtype, encoderDtype)
         cfg = wk_model_config()
         self.lib.wk_default_config(variant.encode(), C.byref(cfg))
         if config:
@@ -273,15 +279,15 @@ class Model:
         check(self.lib.wk_model_create(C.byref(cfg), device, C.byref(self.handle)))
         self.variant = variant
         self.device = device
-        self._set_cross_kv_dtype(crossKVDtype)
+        self._set_storage_dtypes(crossKVDtype, encoderDtype)
 
     @classmethod
     def from_pretrained(cls, weights_dir: str, device: int = 0, max_batch: int = 16, dtype: str = "bf16",
-                        crossKVDtype: Optional[str] = None) -> "Model":
+                        crossKVDtype: Optional[str] = None, encoderDtype: Optional[str] = None) -> "Model":
         """HuggingFace checkpoint directory (config.json + *.safetensors)."""
         self = cls.__new__(cls)
         self.lib = _lib.load()
-        _check_cross_kv_dtype(crossKVDtype)
+        _check_storage_dtypes(crossKVDtype, encoderDtype)
         self.handle = C.c_void_p()
         check(self.lib.wk_model_load(weights_dir.encode(), device, max_batch, _DT[dtype], C.byref(self.handle)))
         info = wk_model_info()
@@ -290,14 +296,15 @@ class Model:
         for f in ("n_mels", "d_model", "n_heads", "enc_layers", "dec_layers", "vocab", "n_audio_ctx", "dtype", "max_batch"):
             setattr(cfg, f, getattr(info, f))
         self.cfg, self.variant, self.device = cfg, os.path.basename(weights_dir.rstrip("/")), device
-        self._set_cross_kv_dtype(crossKVDtype)
+        self._set_storage_dtypes(crossKVDtype, encoderDtype)
         return self
 
-    def _set_cross_kv_dtype(self, crossKVDtype: Optional[str]) -> None:
-        if crossKVDtype is None:
-            return
+    def _set_storage_dtypes(self, crossKVDtype: Optional[str], encoderDtype: Optional[str] = None) -> None:
         try:
-            check(self.lib.wk_model_set_cross_kv_dtype(self.handle, _CKV_DT[crossKVDtype]))
+            if crossKVDtype is not None:
+                check(self.lib.wk_model_set_cross_kv_dtype(self.handle, _CKV_DT[crossKVDtype]))
+            if encoderDtype is not None:
+                check(self.lib.wk_model_set_encoder_dtype(self.handle, _CKV_DT[encoderDtype]))
         except WhisperError:
             self.close()   # the model was created for this call: do not leak it
             raise
@@ -708,6 +715,7 @@ class WhisperKitConfig:
     seed: int = 0
     modelFolder: Optional[str] = None            # HuggingFace checkpoint directory: config.json + *.safetensors (+ tokenizer.json / vocab.json)
     crossKVDtype: Optional[str] = None           # "fp8": E4M3 cross-attention K/V cache (Model); None = dtype
+    encoderDtype: Optional[str] = None           # "fp8": encoder QKV / FC1 / FC2 GEMMs on E4M3 operands (Model); None = dtype
     # audioInputConfig.channelMode: how transcribe(audioPath=...) mixes multi-channel files, ("sum", None | [indices]) or ("channel", i)
     channelMode: tuple = ("sum", None)
 
@@ -722,12 +730,14 @@ class WhisperKit:
         if config.modelFolder is not None:
             # loadModels + loadTokenizer from a local folder (WhisperKit.swift:358-470): weights through the safetensors loader, the
             # decode-side tokenizer when the folder carries tokenizer.json or vocab.json
-            self.model = Model.from_pretrained(config.modelFolder, config.device, config.maxBatch, config.dtype, config.crossKVDtype)
+            self.model = Model.from_pretrained(config.modelFolder, config.device, config.maxBatch, config.dtype, config.crossKVDtype,
+                                               config.encoderDtype)
             if any(os.path.exists(os.path.join(config.modelFolder, f)) for f in ("tokenizer.json", "vocab.json")):
                 from .tokenizer import WhisperTokenizer
                 self.tokenizer = WhisperTokenizer(config.modelFolder)
         else:
-            self.model = Model(config.model, config.device, config.maxBatch, config.dtype, crossKVDtype=config.crossKVDtype)
+            self.model = Model(config.model, config.device, config.maxBatch, config.dtype, crossKVDtype=config.crossKVDtype,
+                               encoderDtype=config.encoderDtype)
             if config.weights is not None:
                 self.model.load_state_dict(config.weights)
             else:

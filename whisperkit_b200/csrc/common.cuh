@@ -38,11 +38,14 @@ template <> struct T16<__half> {
     }
 };
 
-// ------------------------------------------------------------------ FP8 (E4M3) cross-attention K/V rows
-// A row of 64 values is stored as 64 E4M3 codes plus one f32 scale s = amax(|row|) / 448; code = cvt.rn.satfinite.e4m3(x / s) and the
-// stored value is code * s.  A row whose amax is 0 gets s = 0 and all-zero codes.  The GEMM epilogue (gemm_wgmma.cu) and the host test
-// entry (wk_cross_kv_quantize_rows) both go through these two functions, so the CPU tests pin the rounding the GPU does.
+// ------------------------------------------------------------------ FP8 (E4M3) quantization
+// A group of values (a 64-value cross-attention K/V row; under the FP8 encoder policy a 128-column block of an activation row, or a
+// whole weight row) is stored as E4M3 codes plus one f32 scale s = amax(|group|) / 448; code = cvt.rn.satfinite.e4m3(x / s) and the
+// stored value is code * s.  A group whose amax is 0 gets s = 0 and all-zero codes.  The GEMM epilogues (gemm_wgmma.cu), the FP8
+// LayerNorm and weight quantizer (encoder_ops.cu) and the host test entries (wk_cross_kv_quantize_rows, wk_fp8_quantize_blocks) all go
+// through these two functions, so the CPU tests pin the rounding the GPU does.
 constexpr float kFp8E4M3Max = 448.f;
+constexpr int kFp8Block = 128;   // columns per activation scale of the FP8 encoder GEMMs (one 128-byte swizzle row, one k-block)
 __host__ __device__ __forceinline__ float fp8_row_scale(float amax) { return amax / kFp8E4M3Max; }
 __host__ __device__ __forceinline__ uint8_t fp8_encode(float x, float s) {
     return s > 0.f ? (uint8_t)__nv_cvt_float_to_fp8(x / s, __NV_SATFINITE, __NV_E4M3) : (uint8_t)0;
@@ -198,6 +201,14 @@ __device__ __forceinline__ void tma_load_3d_elect(void* smem_dst, const void* tm
         "elect.sync _|q, 0xffffffff;\n\t"
         "@q cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n\t}"
         ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+__device__ __forceinline__ void bulk_load_1d_elect(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+    asm volatile(
+        "{\n\t.reg .pred q;\n\t"
+        "elect.sync _|q, 0xffffffff;\n\t"
+        "@q cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}"
+        ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
         : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx_elect(uint64_t* bar, uint32_t bytes) {

@@ -13,6 +13,22 @@ namespace wk {
 // =====================================================================================================
 // LayerNorm: one warp per row, row kept in registers (two-pass mean / variance in fp32, eps 1e-5)
 // =====================================================================================================
+// the row's (mean, rstd) from its NV float4 per lane
+template <int NV>
+__device__ __forceinline__ float2 ln_stats(const float4 (&v)[NV], int d) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) s += v[i].x + v[i].y + v[i].z + v[i].w;
+    const float mean = warp_sum(s) / d;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, e = v[i].w - mean;
+        q += a * a + b * b + c * c + e * e;
+    }
+    return make_float2(mean, rsqrtf(warp_sum(q) / d + 1e-5f));
+}
+
 template <int NV, typename OutT>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -22,20 +38,10 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, c
     if (row >= rows) return;
     const float4* xr = reinterpret_cast<const float4*>(x + row * d);
     float4 v[NV];
-    float s = 0.f;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        v[i] = xr[lane + 32 * i];
-        s += v[i].x + v[i].y + v[i].z + v[i].w;
-    }
-    const float mean = warp_sum(s) / d;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, e = v[i].w - mean;
-        q += a * a + b * b + c * c + e * e;
-    }
-    const float rstd = rsqrtf(warp_sum(q) / d + 1e-5f);
+    for (int i = 0; i < NV; ++i) v[i] = xr[lane + 32 * i];
+    const float2 st = ln_stats<NV>(v, d);
+    const float mean = st.x, rstd = st.y;
     const float4* g4 = reinterpret_cast<const float4*>(gamma);
     const float4* b4 = reinterpret_cast<const float4*>(beta);
 #pragma unroll
@@ -51,6 +57,36 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, c
             pk.y = T16<OutT>::pack2(o2, o3);
             reinterpret_cast<uint2*>(out + row * d)[lane + 32 * i] = pk;
         }
+    }
+}
+
+// The FP8 encoder policy's LayerNorm: the same f32 output, quantized without a 16-bit rounding.  The warp's v[i] is the row's 128-column
+// block i, so the block's amax is one warp reduction; every lane stores its 4 codes, lane 0 the block scale to scales[i][row].
+template <int NV>
+__global__ void __launch_bounds__(256)
+layernorm_fp8_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     uint8_t* __restrict__ codes, float* __restrict__ scales, long long scale_ld, long long rows, int d) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long row = (long long)blockIdx.x * 8 + warp;
+    if (row >= rows) return;
+    const float4* xr = reinterpret_cast<const float4*>(x + row * d);
+    float4 v[NV];
+#pragma unroll
+    for (int i = 0; i < NV; ++i) v[i] = xr[lane + 32 * i];
+    const float2 st = ln_stats<NV>(v, d);
+    const float mean = st.x, rstd = st.y;
+    const float4* g4 = reinterpret_cast<const float4*>(gamma);
+    const float4* b4 = reinterpret_cast<const float4*>(beta);
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        const float4 g = __ldg(g4 + lane + 32 * i), bb = __ldg(b4 + lane + 32 * i);
+        const float o0 = (v[i].x - mean) * rstd * g.x + bb.x, o1 = (v[i].y - mean) * rstd * g.y + bb.y;
+        const float o2 = (v[i].z - mean) * rstd * g.z + bb.z, o3 = (v[i].w - mean) * rstd * g.w + bb.w;
+        const float s = fp8_row_scale(warp_max(fmaxf(fmaxf(fabsf(o0), fabsf(o1)), fmaxf(fabsf(o2), fabsf(o3)))));
+        reinterpret_cast<uint32_t*>(codes + row * d)[lane + 32 * i] =
+            (uint32_t)fp8_encode(o0, s) | ((uint32_t)fp8_encode(o1, s) << 8) | ((uint32_t)fp8_encode(o2, s) << 16) |
+            ((uint32_t)fp8_encode(o3, s) << 24);
+        if (lane == 0) scales[(long long)i * scale_ld + row] = s;
     }
 }
 
@@ -83,6 +119,52 @@ wk_status layernorm_f32_to_f32(const float* x, const float* gamma, const float* 
                                cudaStream_t stream) {
     if (d % 128 != 0) { set_error("layernorm: d_model %d not a multiple of 128", d); return WK_ERR_INVALID_ARGUMENT; }
     return launch_ln<float>(x, gamma, beta, out, rows, d, stream);
+}
+
+wk_status layernorm_f32_to_fp8(const float* x, const float* gamma, const float* beta, uint8_t* codes, float* scales, int64_t scale_ld,
+                               int64_t rows, int d, cudaStream_t st) {
+    const unsigned grid = (unsigned)((rows + 7) / 8);
+    switch (d / 128) {
+        case 1: layernorm_fp8_kernel<1><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        case 2: layernorm_fp8_kernel<2><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        case 3: layernorm_fp8_kernel<3><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        case 4: layernorm_fp8_kernel<4><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        case 6: layernorm_fp8_kernel<6><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        case 8: layernorm_fp8_kernel<8><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        case 10: layernorm_fp8_kernel<10><<<grid, 256, 0, st>>>(x, gamma, beta, codes, scales, scale_ld, rows, d); break;
+        default: set_error("layernorm: unsupported d_model %d", d); return WK_ERR_INVALID_ARGUMENT;
+    }
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("layernorm launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
+}
+
+// One output channel (weight row) per block: s = amax(|row|) / 448 over the whole row, then the row's codes
+template <typename T>
+__global__ void __launch_bounds__(256)
+quantize_weight_rows_kernel(const T* __restrict__ w, uint8_t* __restrict__ codes, float* __restrict__ scales, int k) {
+    __shared__ float red[8];
+    const T* wr = w + (long long)blockIdx.x * k;
+    float amax = 0.f;
+    for (int i = threadIdx.x; i < k; i += 256) amax = fmaxf(amax, fabsf(T16<T>::to_f(wr[i])));
+    amax = warp_max(amax);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = amax;
+    __syncthreads();
+    amax = red[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) amax = fmaxf(amax, red[i]);
+    const float s = fp8_row_scale(amax);
+    for (int i = threadIdx.x; i < k; i += 256) codes[(long long)blockIdx.x * k + i] = fp8_encode(T16<T>::to_f(wr[i]), s);
+    if (threadIdx.x == 0) scales[blockIdx.x] = s;
+}
+
+wk_status quantize_weight_rows_fp8(const void* w, int dtype, uint8_t* codes, float* scales, int64_t rows, int k, cudaStream_t stream) {
+    if (dtype == WK_DTYPE_F16) quantize_weight_rows_kernel<__half><<<(unsigned)rows, 256, 0, stream>>>((const __half*)w, codes, scales, k);
+    else quantize_weight_rows_kernel<__nv_bfloat16><<<(unsigned)rows, 256, 0, stream>>>((const __nv_bfloat16*)w, codes, scales, k);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("quantize_weight_rows_fp8 launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
 }
 
 // Encoder attention lives in attention_wgmma.cu (TMA + wgmma); this is only its entry point.

@@ -300,6 +300,62 @@ wk_status mel_run(wk_model* m, EncWorkspace* ws, const float* pcm, int64_t n, in
     return mel_forward(&m->mel_tables, src, n, src_stride, nv, mel_out, ws->gmax, stream);
 }
 
+// an FP8 GEMM of the encoder: A = E4M3 codes [M][K] with block scales a_scale [K / 128][ld], W = E4M3 [N][K] with channel scales
+static GemmDesc fp8_gemm(const uint8_t* a, const float* a_scale, int64_t ld, int64_t M, int K, const uint8_t* w, const float* w_scale, int N,
+                         int dtype, int mode, void* out, float* out_scale, const float* bias, int gelu) {
+    GemmDesc g = plain_gemm(a, M, K, w, N, dtype, mode, out, N, bias, gelu);
+    g.a_ld = K; g.b_ld = K;   // bytes: one per code
+    g.a_scale = a_scale; g.a_scale_ld = ld; g.w_scale = w_scale; g.out_scale = out_scale;
+    return g;
+}
+
+// The encoder layers under the FP8 policy: LayerNorms write E4M3 codes + block scales into xn, the QKV / FC1 / FC2 GEMMs run on the FP8
+// tensor cores (FC1 quantizes its GELU output into ffn for FC2); attention, the out-projection and the residual stream are as in the
+// 16-bit schedule.  Every scale comes from its own row, so a window's result does not depend on the batch it is encoded in.
+static wk_status encode_layers_fp8(wk_model* m, EncWorkspace* ws, int B, void* enc_out, cudaStream_t s) {
+    const wk_model_config& c = m->cfg;
+    const int d = c.d_model, T = c.n_audio_ctx, dt = c.dtype;
+    const int64_t M = (int64_t)B * T;
+    const int64_t ld = round_up(ws->max_batch * T, 128);
+    if (!ws->xn_scale) {
+        WK_CHECK(ws->mem.dmalloc(&ws->xn_scale, (size_t)(d / kFp8Block) * ld));
+        WK_CHECK(ws->mem.dmalloc(&ws->ffn_scale, (size_t)(4 * d / kFp8Block) * ld));
+    }
+    uint8_t* xn8 = static_cast<uint8_t*>(ws->xn);
+    uint8_t* ffn8 = static_cast<uint8_t*>(ws->ffn);
+    for (int li = 0; li < c.enc_layers; ++li) {
+        EncLayer& l = m->enc[li];
+        WK_CHECK(layernorm_f32_to_fp8(ws->x, l.ln1.g, l.ln1.b, xn8, ws->xn_scale, ld, M, d, s));
+        WK_CHECK(gemm_wgmma_fp8(fp8_gemm(xn8, ws->xn_scale, ld, M, d, l.wqkv8, l.sqkv, 3 * d, dt, GEMM_OUT_T16, ws->qkv, nullptr, l.bqkv, 0),
+                                m->num_sms, s));
+        WK_CHECK(encoder_attention(ws->qkv, ws->attn, B, T, c.n_heads, dt, s));
+        WK_CHECK(gemm_wgmma(plain_gemm(ws->attn, M, d, l.wo, d, dt, GEMM_OUT_F32_ADD, ws->x, d, l.bo, 0), m->num_sms, s));
+        WK_CHECK(layernorm_f32_to_fp8(ws->x, l.ln2.g, l.ln2.b, xn8, ws->xn_scale, ld, M, d, s));
+        WK_CHECK(gemm_wgmma_fp8(fp8_gemm(xn8, ws->xn_scale, ld, M, d, l.w18, l.s1, 4 * d, dt, GEMM_OUT_FP8_BLOCKS, ffn8, ws->ffn_scale, l.b1, 1),
+                                m->num_sms, s));
+        WK_CHECK(gemm_wgmma_fp8(fp8_gemm(ffn8, ws->ffn_scale, ld, M, 4 * d, l.w28, l.s2, d, dt, GEMM_OUT_F32_ADD, ws->x, nullptr, l.b2, 0),
+                                m->num_sms, s));
+    }
+    WK_CHECK(layernorm_f32_to_16(ws->x, m->enc_ln.g, m->enc_ln.b, enc_out, M, d, dt, s));
+    return WK_OK;
+}
+
+// E4M3 copies of encoder layer li's QKV / FC1 / FC2 weights (the FP8 policy), from the 16-bit weights, on the model stream
+static wk_status quantize_enc_layer(wk_model* m, int li) {
+    const int d = m->cfg.d_model, dt = m->cfg.dtype;
+    EncLayer& l = m->enc[li];
+    WK_CHECK(quantize_weight_rows_fp8(l.wqkv, dt, l.wqkv8, l.sqkv, 3 * d, d, m->stream));
+    WK_CHECK(quantize_weight_rows_fp8(l.w1, dt, l.w18, l.s1, 4 * d, d, m->stream));
+    WK_CHECK(quantize_weight_rows_fp8(l.w2, dt, l.w28, l.s2, d, 4 * d, m->stream));
+    return WK_OK;
+}
+
+static wk_status quantize_enc_weights(wk_model* m) {
+    for (size_t li = 0; li < m->enc.size(); ++li) WK_CHECK(quantize_enc_layer(m, (int)li));
+    WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return WK_OK;
+}
+
 wk_status encode_chunk(wk_model* m, EncWorkspace* ws, const void* mel, int B, void* enc_out, cudaStream_t s) {
     const wk_model_config& c = m->cfg;
     const int d = c.d_model, T = c.n_audio_ctx, dt = c.dtype;
@@ -336,6 +392,7 @@ wk_status encode_chunk(wk_model* m, EncWorkspace* ws, const void* mel, int B, vo
         g.out = ws->x; g.ld_out = d; g.out_rows_per_batch = T; g.bias = m->conv2_b; g.pos = m->enc_pos; g.ld_pos = d;
         WK_CHECK(gemm_wgmma(g, m->num_sms, s));
     }
+    if (m->enc_fp8) return encode_layers_fp8(m, ws, B, enc_out, s);
     for (int li = 0; li < c.enc_layers; ++li) {
         EncLayer& l = m->enc[li];
         WK_CHECK(layernorm_f32_to_16(ws->x, l.ln1.g, l.ln1.b, ws->xn, M, d, dt, s));
@@ -474,6 +531,17 @@ wk_status wk_model_set_tensor(wk_model* m, const char* name, const void* data, i
     } else {
         st = convert_to_16(tmp, dtype, dst.p, dst.dtype, (int64_t)numel, m->stream);
         cudaStreamSynchronize(m->stream);
+    }
+    int li = -1;
+    char rest[128];
+    if (st == WK_OK && m->enc_fp8 && sscanf(name, "model.encoder.layers.%d.%127s", &li, rest) == 2) {
+        const std::string r = rest;   // a QKV / FC1 / FC2 weight of an FP8 encoder: refresh the layer's E4M3 copies
+        if (r == "self_attn.q_proj.weight" || r == "self_attn.k_proj.weight" || r == "self_attn.v_proj.weight" || r == "fc1.weight" ||
+            r == "fc2.weight") {
+            st = quantize_enc_layer(m, li);
+            const cudaError_t e = cudaStreamSynchronize(m->stream);
+            if (st == WK_OK && e != cudaSuccess) { set_error("wk_model_set_tensor: %s", cudaGetErrorString(e)); st = WK_ERR_CUDA; }
+        }
     }
     return st;
 }
@@ -719,6 +787,7 @@ wk_status wk_model_init_random(wk_model* m, uint64_t seed, float std) {
     WK_CHECK(F(m->bckv, (size_t)2 * m->dec.size() * d, 0.f));
     for (size_t i = 0; i < m->dec.size(); ++i) WK_CUDA_CHECK(cudaMemsetAsync(m->bckv + 2 * i * d, 0, d * 4, s));  // no key bias
     WK_CUDA_CHECK(cudaStreamSynchronize(s));
+    if (m->enc_fp8) WK_CHECK(quantize_enc_weights(m));
     m->finalized = true;
     return WK_OK;
 }
@@ -751,6 +820,49 @@ wk_status wk_model_set_cross_kv_dtype(wk_model* m, int32_t dtype) {
         return WK_ERR_INVALID_ARGUMENT;
     }
     m->cross_kv_fp8 = dtype == WK_DTYPE_FP8_E4M3;
+    return WK_OK;
+}
+
+wk_status wk_model_set_encoder_dtype(wk_model* m, int32_t dtype) {
+    if (!m) return WK_ERR_INVALID_ARGUMENT;
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);   // wk_session_create and wk_encode mark the model under the same lock
+    if (m->session_created || m->encoded) {
+        set_error("wk_model_set_encoder_dtype: the encoder precision is fixed once a session exists or wk_encode has run");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (dtype != WK_DTYPE_FP8_E4M3 && dtype != m->cfg.dtype) {
+        set_error("wk_model_set_encoder_dtype: dtype %d is neither WK_DTYPE_FP8_E4M3 nor the model's dtype %d", dtype, m->cfg.dtype);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (dtype == WK_DTYPE_FP8_E4M3 && !m->enc_fp8) {
+        const size_t d = m->cfg.d_model;
+        for (EncLayer& l : m->enc) {
+            if (l.wqkv8) continue;   // kept from an earlier FP8 setting
+            WK_CHECK(m->mem.dmalloc(&l.wqkv8, 3 * d * d, false)); WK_CHECK(m->mem.dmalloc(&l.sqkv, 3 * d, false));
+            WK_CHECK(m->mem.dmalloc(&l.w18, 4 * d * d, false)); WK_CHECK(m->mem.dmalloc(&l.s1, 4 * d, false));
+            WK_CHECK(m->mem.dmalloc(&l.w28, 4 * d * d, false)); WK_CHECK(m->mem.dmalloc(&l.s2, d, false));
+        }
+        WK_CHECK(quantize_enc_weights(m));
+    }
+    m->enc_fp8 = dtype == WK_DTYPE_FP8_E4M3;
+    return WK_OK;
+}
+
+wk_status wk_model_encoder_dtype(const wk_model* m, int32_t* dtype) {
+    if (!m || !dtype) return WK_ERR_INVALID_ARGUMENT;
+    *dtype = m->enc_fp8 ? WK_DTYPE_FP8_E4M3 : m->cfg.dtype;
+    return WK_OK;
+}
+
+wk_status wk_fp8_quantize_blocks(const float* x, int64_t rows, int64_t cols, int64_t block, uint8_t* codes, float* scales) {
+    if (!x || !codes || !scales || rows < 0 || block < 1 || cols < 0 || cols % block != 0) {
+        set_error("wk_fp8_quantize_blocks: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    const int64_t nb = cols / block;
+    for (int64_t r = 0; r < rows; ++r)
+        for (int64_t b = 0; b < nb; ++b) fp8_quantize_row(x + r * cols + b * block, (int)block, codes + r * cols + b * block, scales + r * nb + b);
     return WK_OK;
 }
 
@@ -884,6 +996,7 @@ wk_status wk_encode(wk_model* m, const wk_tensor* mel, wk_tensor** enc_out) {
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
     WK_CHECK(enc_ws_ensure(m, &m->ws, m->cfg.max_batch));
+    m->encoded = true;
     wk_tensor* t = nullptr;
     WK_CHECK(tensor_new(m, 1, m->cfg.dtype, mel->batch, (size_t)mel->batch * m->cfg.n_audio_ctx * m->cfg.d_model * 2, &t));
     wk_status s = encode_chunk(m, &m->ws, mel->data, (int)mel->batch, t->data, m->stream);
@@ -1016,6 +1129,22 @@ wk_status wk_test_gemm_residual(wk_model* m, const void* a, const void* w, const
     WK_CUDA_CHECK(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> lock(m->api_mu);
     WK_CHECK(gemm_wgmma(plain_gemm(a, M, K, w, N, in_dtype, GEMM_OUT_F32_ADD, out, N, bias, 0), m->num_sms, m->stream));
+    WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return WK_OK;
+}
+
+// The FP8 encoder GEMM alone: kind 0 QKV (16-bit out), 1 FC1 (GELU, E4M3 codes + block scales out), 2 FC2 (f32 residual in place)
+wk_status wk_test_gemm_fp8(wk_model* m, int32_t kind, const uint8_t* a, const float* a_scale, const uint8_t* w, const float* w_scale,
+                           const float* bias, void* out, float* out_scale, int32_t M, int32_t N, int32_t K, int32_t dtype) {
+    if (!m || !a || !a_scale || !w || !w_scale || !out || kind < 0 || kind > 2 || (kind == 1 && !out_scale) || M < 1) {
+        set_error("wk_test_gemm_fp8: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    static const int modes[3] = {GEMM_OUT_T16, GEMM_OUT_FP8_BLOCKS, GEMM_OUT_F32_ADD};
+    WK_CHECK(gemm_wgmma_fp8(fp8_gemm(a, a_scale, round_up(M, 128), M, K, w, w_scale, N, dtype, modes[kind], out, out_scale, bias, kind == 1),
+                            m->num_sms, m->stream));
     WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
     return WK_OK;
 }

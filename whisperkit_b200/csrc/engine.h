@@ -23,6 +23,10 @@ struct EncLayer {
     void* wo = nullptr; float* bo = nullptr;
     void* w1 = nullptr; float* b1 = nullptr;      // [4d, d]
     void* w2 = nullptr; float* b2 = nullptr;      // [d, 4d]
+    // FP8 encoder policy (wk_model_set_encoder_dtype): E4M3 copies of wqkv / w1 / w2 with one f32 scale per output channel
+    uint8_t* wqkv8 = nullptr; float* sqkv = nullptr;
+    uint8_t* w18 = nullptr; float* s1 = nullptr;
+    uint8_t* w28 = nullptr; float* s2 = nullptr;
 };
 struct DecLayer {
     LayerNormW ln1, lnx, ln3;
@@ -45,6 +49,9 @@ struct EncWorkspace {
     float* x = nullptr;        // f32 [Bm*1500][d]
     void* xn = nullptr; void* qkv = nullptr; void* attn = nullptr; void* ffn = nullptr;
     void* enc_out = nullptr;   // 16-bit [Bm*1500][d]
+    // FP8 encoder policy: xn / ffn then hold E4M3 codes; their block scales [d / 128][ld] and [4d / 128][ld], ld = Bm*1500 rounded up to
+    // 128 (allocated by the first FP8 encode)
+    float* xn_scale = nullptr; float* ffn_scale = nullptr;
 };
 
 }  // namespace wk
@@ -90,6 +97,9 @@ struct wk_model {
     // first session exists.  Both fields are read and written under api_mu.
     bool cross_kv_fp8 = false;
     bool session_created = false;
+    // encoder QKV / FC1 / FC2 GEMMs on E4M3 operands (wk_model_set_encoder_dtype); fixed once a session exists or wk_encode has run
+    bool enc_fp8 = false;
+    bool encoded = false;
 };
 
 namespace wk {

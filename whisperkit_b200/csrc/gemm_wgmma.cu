@@ -62,7 +62,8 @@ struct GemmKParams {
 //   kEpiFp8Heads  GEMM_OUT_FP8_HEADS, per-row quantization in registers (gemm_epilogue_fp8_heads)
 //   kEpiStore16   GEMM_OUT_T16 / GEMM_OUT_T16_HEADS and kEpiStore32  GEMM_OUT_F32 / _F32_ADD / _F32_GELU_POS: the per-element math in
 //                 registers, the tile through a shared-memory staging box and TMA bulk tensor stores (gemm_epilogue_store16 / _store32)
-enum GemmEpi { kEpiPartialT = 0, kEpiFp8Heads = 1, kEpiStore16 = 2, kEpiStore32 = 3 };
+//   kEpiFp8Blocks GEMM_OUT_FP8_BLOCKS (FP8 kernel only), per-row block quantization in registers (gemm_epilogue_fp8_blocks)
+enum GemmEpi { kEpiPartialT = 0, kEpiFp8Heads = 1, kEpiStore16 = 2, kEpiStore32 = 3, kEpiFp8Blocks = 4 };
 static int gemm_epi(int mode) {
     switch (mode) {
         case GEMM_OUT_PARTIAL_T: return kEpiPartialT;
@@ -442,6 +443,193 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (kStore && wg_tid == 0) bulk_wait_all();
 }
 
+// ------------------------------------------------------------------------------------------------ FP8 (E4M3) encoder GEMMs
+// The same producer / two-consumer structure with E4M3 operands: a k-block is 128 codes (one 128-byte swizzle row), so it is also one
+// activation scale block.  A stage holds the A tile, the B tile and the tile's 128 row scales of that k-block (a 512-byte bulk copy
+// from a_scale [K / 128][a_scale_ld]).  Each k-block's four m64n128k32 MMAs go into a temporary accumulator, which is then promoted:
+// acc += tmp * a_scale[kb][row].  The weight scale (one per output channel) multiplies acc once before the epilogue.
+static constexpr int kFp8BN = 128;
+static constexpr int kStageB8 = kFp8BN * kFp8Block;          // 16 KiB
+static constexpr int kStage8 = kStageA + kStageB8 + 1024;    // + the 512-byte scale row, padded to keep stages 1024-aligned
+
+struct GemmFp8Params {
+    GemmKParams g;
+    const float* a_scale;
+    long long a_scale_ld;
+    const float* w_scale;
+};
+
+// GEMM_OUT_FP8_BLOCKS epilogue of one consumer warpgroup (FC1 under the FP8 encoder policy): v = act(acc + bias) in f32, then per row
+// one scale over the tile's 128 columns - the 4 lanes of a quad hold a row, so its amax is two shuffles - and the codes into one
+// 64-row x 128-byte staging box, one TMA store.  The lane with c_lo == 0 stores the row's scale to out_scale[col_base / 128][row].
+__device__ __forceinline__ void gemm_epilogue_fp8_blocks(const GemmFp8Params& q, const CUtensorMap* tmO, float (&acc)[kFp8BN / 2],
+                                                         uint8_t* stage, int& sbuf, int wg_tid, int cw, int row0, int col_base) {
+    const GemmKParams& p = q.g;
+    const int lane = wg_tid & 31;
+    const int c_lo = 2 * (lane & 3);
+    const int r_top = 16 * (wg_tid >> 5) + (lane >> 2);   // and r_top + 8
+    float amax[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < kFp8BN / 8; ++j) {
+        const int col = col_base + 8 * j + c_lo;
+        float v0 = acc[4 * j], v1 = acc[4 * j + 1], v2 = acc[4 * j + 2], v3 = acc[4 * j + 3];
+        if (p.bias) {
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+            v0 += bb.x; v1 += bb.y; v2 += bb.x; v3 += bb.y;
+        }
+        if (p.gelu) {
+            const float2 g0 = gelu_erf2(make_float2(v0, v1)), g1 = gelu_erf2(make_float2(v2, v3));
+            v0 = g0.x; v1 = g0.y; v2 = g1.x; v3 = g1.y;
+        }
+        acc[4 * j] = v0; acc[4 * j + 1] = v1; acc[4 * j + 2] = v2; acc[4 * j + 3] = v3;
+        amax[0] = fmaxf(amax[0], fmaxf(fabsf(v0), fabsf(v1)));
+        amax[1] = fmaxf(amax[1], fmaxf(fabsf(v2), fabsf(v3)));
+    }
+    uint8_t* buf = stage + sbuf * kStoreBox;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float a = fmaxf(amax[h], __shfl_xor_sync(0xffffffffu, amax[h], 1));
+        a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, 2));
+        const float s = fp8_row_scale(a);
+        const int r = r_top + 8 * h;
+        // column 8 j + c_lo is byte 8 (j & 1) + c_lo of the row's 16-byte chunk j / 2
+#pragma unroll
+        for (int j = 0; j < kFp8BN / 8; ++j)
+            *reinterpret_cast<uint16_t*>(buf + swz128(r, j >> 1) + 8 * (j & 1) + c_lo) =
+                (uint16_t)(fp8_encode(acc[4 * j + 2 * h], s) | (fp8_encode(acc[4 * j + 2 * h + 1], s) << 8));
+        if (c_lo == 0 && row0 + r < p.m_rows_per_batch) p.out_scale[(long long)(col_base / kFp8Block) * q.a_scale_ld + row0 + r] = s;
+    }
+    store_box_begin(wg_tid, cw);
+    if (wg_tid == 0) {
+        tma_store_3d(tmO, buf, col_base, row0, 0);
+        bulk_commit();
+    }
+    sbuf ^= 1;
+}
+
+template <typename T, int EPI>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+                const GemmFp8Params q) {
+    constexpr int BN = kFp8BN;
+    const GemmKParams& p = q.g;
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* store_stage = smem + (size_t)p.stages * kStage8;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(store_stage + kStoreBytes);
+    uint64_t* empty_bar = full_bar + kMaxStages;
+    uint64_t* res_bar = empty_bar + kMaxStages;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    pdl_launch_dependents();
+
+    if (warp == 0 && lane == 0) {
+        tma_prefetch_desc(&tmA);
+        tma_prefetch_desc(&tmB);
+        tma_prefetch_desc(&tmO);
+        for (int i = 0; i < p.stages; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 8);
+        }
+        for (int i = 0; i < 4; ++i) mbar_init(&res_bar[i], 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();
+
+    if (warp < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp != 0) return;
+        // ===================== TMA producer =====================
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int w = blockIdx.x; w < p.work; w += gridDim.x) {
+            const int n_tile = w % p.tiles_n;
+            const int row0 = (w / p.tiles_n) * kBlockM;
+            for (int kb = 0; kb < p.kb_per_split; ++kb) {
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                __syncwarp();
+                uint8_t* sa = smem + (size_t)stage * kStage8;
+                mbar_expect_tx_elect(&full_bar[stage], (uint32_t)(kStageA + kStageB8 + kBlockM * 4));
+                tma_load_2d_elect(sa, &tmA, &full_bar[stage], kb * kFp8Block, row0);
+                tma_load_2d_elect(sa + kStageA, &tmB, &full_bar[stage], kb * kFp8Block, n_tile * BN);
+                bulk_load_1d_elect(sa + kStageA + kStageB8, q.a_scale + (long long)kb * q.a_scale_ld + row0, kBlockM * 4, &full_bar[stage]);
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumer warpgroups =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = (warp >> 2) - 1;
+    const int wg_tid = threadIdx.x & 127;
+    const int r_lo = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows in the tile: r_lo and r_lo + 8
+    const int c_lo = 2 * (lane & 3);
+    uint8_t* my_stage = store_stage + cw * 2 * kStoreBox;
+    uint64_t* my_res_bar = res_bar + 2 * cw;
+    int sbuf = 0;
+    uint32_t rphase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2], tmp[BN / 2];
+    for (int w = blockIdx.x; w < p.work; w += gridDim.x) {
+        const int n_tile = w % p.tiles_n;
+        const int tile_row0 = (w / p.tiles_n) * kBlockM;
+        const int col_base = n_tile * BN;
+        const int wg_row0 = tile_row0 + 64 * cw;
+        const bool wg_rows = wg_row0 < p.m_rows_per_batch;
+
+        for (int kb = 0; kb < p.kb_per_split; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            uint8_t* sa = smem + (size_t)stage * kStage8;
+            const uint64_t adesc = wgmma_desc_sw128(smem_u32(sa) + cw * 64 * 128);
+            const uint64_t bdesc = wgmma_desc_sw128(smem_u32(sa + kStageA));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kFp8Block / 32; ++k)   // +32 bytes per 32 K codes inside the swizzle row
+                WgmmaE4M3x128::ss(tmp, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+            wgmma_commit();
+            if (EPI == kEpiStore32 && kb == 0 && wg_tid == 0 && wg_rows) {
+                // residual chunks 0 and 1 of this tile (GEMM_OUT_F32_ADD), fetched while the MMAs run
+                bulk_wait_read_all();
+                for (int c = 0; c < 2 && col_base + 32 * c < p.n; ++c) {
+                    const int b = sbuf ^ c;
+                    mbar_expect_tx(&my_res_bar[b], kStoreBox);
+                    tma_load_3d(my_stage + b * kStoreBox, &tmO, &my_res_bar[b], col_base + 32 * c, wg_row0, 0);
+                }
+            }
+            const float* sc = reinterpret_cast<const float*>(sa + kStageA + kStageB8);
+            const float s0 = sc[r_lo], s1 = sc[r_lo + 8];
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                if (kb == 0) {
+                    acc[4 * j] = tmp[4 * j] * s0; acc[4 * j + 1] = tmp[4 * j + 1] * s0;
+                    acc[4 * j + 2] = tmp[4 * j + 2] * s1; acc[4 * j + 3] = tmp[4 * j + 3] * s1;
+                } else {
+                    acc[4 * j] = fmaf(tmp[4 * j], s0, acc[4 * j]); acc[4 * j + 1] = fmaf(tmp[4 * j + 1], s0, acc[4 * j + 1]);
+                    acc[4 * j + 2] = fmaf(tmp[4 * j + 2], s1, acc[4 * j + 2]); acc[4 * j + 3] = fmaf(tmp[4 * j + 3], s1, acc[4 * j + 3]);
+                }
+            }
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {   // dequantize: the weight scale of each output channel (n is a multiple of 128)
+            const float2 ws = __ldg(reinterpret_cast<const float2*>(q.w_scale + col_base + 8 * j + c_lo));
+            acc[4 * j] *= ws.x; acc[4 * j + 1] *= ws.y; acc[4 * j + 2] *= ws.x; acc[4 * j + 3] *= ws.y;
+        }
+        if (!wg_rows) continue;
+        if constexpr (EPI == kEpiStore16) gemm_epilogue_store16<T, BN>(p, &tmO, acc, my_stage, sbuf, wg_tid, cw, 0, wg_row0, col_base);
+        else if constexpr (EPI == kEpiStore32) gemm_epilogue_store32<BN>(p, &tmO, acc, my_stage, my_res_bar, sbuf, rphase, wg_tid, cw, 0, wg_row0, col_base);
+        else gemm_epilogue_fp8_blocks(q, &tmO, acc, my_stage, sbuf, wg_tid, cw, wg_row0, col_base);
+    }
+    if (wg_tid == 0) bulk_wait_all();
+}
+
 // ------------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -473,7 +661,8 @@ static wk_status make_tmap(CUtensorMap* tm, const void* base, int dtype, int ndi
     for (int i = 0; i < ndim; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; }
     for (int i = 0; i < ndim - 1; ++i) gstr[i] = strides_bytes[i];
     const CUtensorMapDataType ty = dtype == WK_DTYPE_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                   : dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+                                   : dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                   : dtype == WK_DTYPE_FP8_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     CUresult r = enc(tm, ty,
                      (cuuint32_t)ndim, const_cast<void*>(base), gdim, gstr, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -651,6 +840,91 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream) {
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) {
         set_error("gemm_wgmma launch: %s", cudaGetErrorString(e));
+        return WK_ERR_CUDA;
+    }
+    return WK_OK;
+}
+
+template <typename T, int EPI>
+static cudaError_t launch_gemm_fp8(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const GemmFp8Params& q, int grid,
+                                   size_t smem, cudaStream_t stream) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        const cudaError_t e = cudaFuncSetAttribute(gemm_fp8_kernel<T, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
+        if (e != cudaSuccess) return e;
+        attr_set = true;
+    }
+    return launch_k(gemm_fp8_kernel<T, EPI>, dim3(grid), dim3(kGemmThreads), smem, stream, 0, tmA, tmB, tmO, q);
+}
+
+template <typename T>
+static cudaError_t launch_gemm_fp8_mode(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const GemmFp8Params& q,
+                                        int grid, size_t smem, cudaStream_t stream) {
+    switch (q.g.mode) {
+        case GEMM_OUT_T16: return launch_gemm_fp8<T, kEpiStore16>(tmA, tmB, tmO, q, grid, smem, stream);
+        case GEMM_OUT_F32_ADD: return launch_gemm_fp8<T, kEpiStore32>(tmA, tmB, tmO, q, grid, smem, stream);
+        default: return launch_gemm_fp8<T, kEpiFp8Blocks>(tmA, tmB, tmO, q, grid, smem, stream);
+    }
+}
+
+wk_status gemm_wgmma_fp8(const GemmDesc& d, int num_sms, cudaStream_t stream) {
+    if (d.k % kFp8Block != 0 || d.n % kFp8BN != 0 || d.k < kFp8Block || d.n < kFp8BN || d.m_rows_per_batch < 1 || d.a_3d || d.taps != 1 ||
+        (d.mode != GEMM_OUT_T16 && d.mode != GEMM_OUT_F32_ADD && d.mode != GEMM_OUT_FP8_BLOCKS) || !d.a_scale || !d.w_scale ||
+        d.a_scale_ld % kBlockM != 0 || d.a_scale_ld < d.m_rows_per_batch || (d.mode == GEMM_OUT_FP8_BLOCKS && !d.out_scale) ||
+        (d.in_dtype != WK_DTYPE_BF16 && d.in_dtype != WK_DTYPE_F16)) {
+        set_error("gemm_wgmma_fp8: unsupported problem (m %d n %d k %d mode %d scale ld %lld)", d.m_rows_per_batch, d.n, d.k, d.mode,
+                  (long long)d.a_scale_ld);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    GemmFp8Params q;
+    memset(&q, 0, sizeof(q));
+    GemmKParams& p = q.g;
+    p.kb_per_tap = p.kb_per_split = d.k / kFp8Block;
+    p.splits = 1; p.taps = 1; p.n_batches = 1;
+    p.m_rows_per_batch = d.m_rows_per_batch;
+    p.tiles_per_batch = (d.m_rows_per_batch + kBlockM - 1) / kBlockM;
+    p.n = d.n; p.bn = kFp8BN;
+    p.tiles_n = d.n / kFp8BN;
+    p.work = p.tiles_per_batch * p.tiles_n;
+    p.stage_b_bytes = kStageB8;
+    p.store_bytes = kStoreBytes;
+    int stages = (kSmemMax - 1024 - 256 - kStoreBytes) / kStage8;
+    if (stages > kMaxStages) stages = kMaxStages;
+    p.stages = stages;
+    p.mode = d.mode; p.gelu = d.gelu; p.out = d.out; p.ld_out = d.ld_out; p.out_rows_per_batch = d.m_rows_per_batch;
+    p.bias = d.bias; p.out_scale = d.out_scale;
+    q.a_scale = d.a_scale; q.a_scale_ld = d.a_scale_ld; q.w_scale = d.w_scale;
+
+    CUtensorMap tmA, tmB, tmO;
+    {
+        uint64_t dims[2] = {(uint64_t)d.k, (uint64_t)d.a_rows};
+        uint64_t str[1] = {(uint64_t)d.a_ld};
+        uint32_t box[2] = {kFp8Block, kBlockM};
+        WK_CHECK(make_tmap(&tmA, d.a, WK_DTYPE_FP8_E4M3, 2, dims, str, box));
+    }
+    {
+        uint64_t dims[2] = {(uint64_t)d.k, (uint64_t)d.b_rows};
+        uint64_t str[1] = {(uint64_t)d.b_ld};
+        uint32_t box[2] = {kFp8Block, kFp8BN};
+        WK_CHECK(make_tmap(&tmB, d.b, WK_DTYPE_FP8_E4M3, 2, dims, str, box));
+    }
+    {
+        // [rows][ld_out] with n valid columns: 64 rows x 128 bytes per staging box (64 16-bit, 32 f32 or 128 E4M3 columns)
+        const int out_dtype = d.mode == GEMM_OUT_T16 ? d.in_dtype : d.mode == GEMM_OUT_F32_ADD ? WK_DTYPE_F32 : WK_DTYPE_FP8_E4M3;
+        const uint64_t es = d.mode == GEMM_OUT_T16 ? 2 : d.mode == GEMM_OUT_F32_ADD ? 4 : 1;
+        uint64_t dims[3] = {(uint64_t)d.n, (uint64_t)d.m_rows_per_batch, 1};
+        uint64_t str[2] = {(uint64_t)d.ld_out * es, (uint64_t)d.m_rows_per_batch * d.ld_out * es};
+        uint32_t box[3] = {(uint32_t)(128 / es), 64, 1};
+        WK_CHECK(make_tmap(&tmO, d.out, out_dtype, 3, dims, str, box));
+    }
+    const size_t smem_bytes = (size_t)stages * kStage8 + kStoreBytes + 1024 + 256;
+    const int grid = p.work < num_sms ? p.work : num_sms;
+    cudaError_t e = d.in_dtype == WK_DTYPE_F16 ? launch_gemm_fp8_mode<__half>(tmA, tmB, tmO, q, grid, smem_bytes, stream)
+                                               : launch_gemm_fp8_mode<__nv_bfloat16>(tmA, tmB, tmO, q, grid, smem_bytes, stream);
+    count_launch();
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        set_error("gemm_wgmma_fp8 launch: %s", cudaGetErrorString(e));
         return WK_ERR_CUDA;
     }
     return WK_OK;

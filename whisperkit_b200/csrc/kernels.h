@@ -69,6 +69,7 @@ enum GemmMode {
     GEMM_OUT_T16_HEADS = 4,  // out16[which][b][h][t][64] head-major scatter  (cross-attention K/V cache)
     GEMM_OUT_F32 = 5,        // out32[row, col] = acc + bias[col]
     GEMM_OUT_FP8_HEADS = 6,  // out8[which][b][h][t][64] E4M3 codes + out_scale[which][b][h][t] f32 (FP8 cross-attention K/V cache)
+    GEMM_OUT_FP8_BLOCKS = 7, // out8[row, col] E4M3 codes of act(acc + bias[col]) + out_scale[col / 128][row] f32 (FP8 encoder FC1)
 };
 
 struct GemmDesc {
@@ -111,9 +112,18 @@ struct GemmDesc {
     int pdl;                // launch with programmatic dependent launch (decode-step chain)
     int max_stages;          // 0 = as many smem stages as fit; >0 caps the ring (lets other kernels co-reside on the SM)
     int a_static;            // A operand (weights) does not depend on the upstream kernel: with PDL its first tiles are fetched before griddepcontrol.wait
+    // FP8 operands (gemm_wgmma_fp8 only): a / b hold E4M3 codes, a_scale [K / 128][a_scale_ld] one f32 per (row, 128-column block),
+    // w_scale [n] one f32 per output channel; FP8_BLOCKS writes its scales to out_scale with the same layout and ld (a_scale_ld)
+    const float* a_scale;
+    int64_t a_scale_ld;      // a multiple of 128 >= the rows: a tile's 128 row scales of one k-block are one 512-byte copy
+    const float* w_scale;
 };
 
 wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream);
+// The FP8 encoder GEMMs: D = sum over 128-wide k-blocks kb of (A8 W8^T)[kb] * a_scale[kb][row], times w_scale[col] in the epilogue;
+// plain 2-D operands, n and k multiples of 128, modes GEMM_OUT_T16 (QKV), GEMM_OUT_FP8_BLOCKS (FC1) and GEMM_OUT_F32_ADD (FC2).
+// in_dtype is the model's 16-bit type (the type of a T16 output)
+wk_status gemm_wgmma_fp8(const GemmDesc& d, int num_sms, cudaStream_t stream);
 // the wgmma tile width (N) a GEMM with bn output columns per tile runs with: bn rounded up to a power of two >= 16
 int wgmma_tile_n(int bn);
 
@@ -141,6 +151,11 @@ wk_status layernorm_f32_to_16(const float* x, const float* gamma, const float* b
                               cudaStream_t stream);
 wk_status layernorm_f32_to_f32(const float* x, const float* gamma, const float* beta, float* out, int64_t rows, int d,
                                cudaStream_t stream);
+// LayerNorm straight from f32 to E4M3: codes [rows][d], one scale per (row, 128-column block) in scales [d / 128][scale_ld]
+wk_status layernorm_f32_to_fp8(const float* x, const float* gamma, const float* beta, uint8_t* codes, float* scales, int64_t scale_ld,
+                               int64_t rows, int d, cudaStream_t stream);
+// 16-bit weights [rows][k] -> E4M3 codes [rows][k] with one scale per row (output channel) over the whole row
+wk_status quantize_weight_rows_fp8(const void* w, int dtype, uint8_t* codes, float* scales, int64_t rows, int k, cudaStream_t stream);
 wk_status encoder_attention(const void* qkv, void* out, int B, int T, int n_heads, int dtype, cudaStream_t stream);
 // TMA + wgmma implementation (attention_wgmma.cu) behind encoder_attention()
 wk_status encoder_attention_wgmma(const void* qkv, void* out, int B, int T, int n_heads, int dtype, cudaStream_t stream);

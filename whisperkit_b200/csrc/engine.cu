@@ -274,22 +274,29 @@ GemmDesc plain_gemm(const void* a, int64_t M, int K, const void* w, int N, int d
     return g;
 }
 
+wk_status mel_stage(EncWorkspace* ws, const float* pcm, int64_t n, int64_t stride, cudaStream_t stream, const float** src, int64_t* src_stride) {
+    cudaPointerAttributes at;
+    const bool on_device = cudaPointerGetAttributes(&at, pcm) == cudaSuccess && at.type == cudaMemoryTypeDevice;
+    cudaGetLastError();
+    *src = pcm;
+    *src_stride = stride;
+    if (on_device && stride >= kWindowSamples) return WK_OK;
+    // host PCM, or short rows: stage (padOrTrimAudio, AudioProcessor.swift:151-174)
+    if (stride < kWindowSamples) WK_CUDA_CHECK(cudaMemsetAsync(ws->pcm_dev, 0, (size_t)n * kWindowSamples * 4, stream));
+    WK_CUDA_CHECK(cudaMemcpy2DAsync(ws->pcm_dev, kWindowSamples * 4, pcm, stride * 4, std::min<int64_t>(stride, kWindowSamples) * 4, n,
+                                    cudaMemcpyDefault, stream));
+    *src = ws->pcm_dev;
+    *src_stride = kWindowSamples;
+    return WK_OK;
+}
+
 wk_status mel_run(wk_model* m, EncWorkspace* ws, const float* pcm, int64_t n, int64_t stride, const int32_t* samples_per_window,
                   void* mel_out, cudaStream_t stream) {
     if (n < 1 || n > ws->max_batch) { set_error("log-mel: %lld windows outside [1, %d]", (long long)n, ws->max_batch); return WK_ERR_AUDIO_PROCESSING_FAILED; }
     if (stride < kWindowSamples && !samples_per_window) { set_error("log-mel: stride %lld < 480000 requires samples_per_window", (long long)stride); return WK_ERR_AUDIO_PROCESSING_FAILED; }
-    cudaPointerAttributes at;
-    const bool on_device = cudaPointerGetAttributes(&at, pcm) == cudaSuccess && at.type == cudaMemoryTypeDevice;
-    cudaGetLastError();
-    const float* src = pcm;
-    int64_t src_stride = stride;
-    if (!on_device || stride < kWindowSamples) {   // host PCM, or short rows: stage (padOrTrimAudio, AudioProcessor.swift:151-174)
-        if (stride < kWindowSamples) WK_CUDA_CHECK(cudaMemsetAsync(ws->pcm_dev, 0, (size_t)n * kWindowSamples * 4, stream));
-        WK_CUDA_CHECK(cudaMemcpy2DAsync(ws->pcm_dev, kWindowSamples * 4, pcm, stride * 4, std::min<int64_t>(stride, kWindowSamples) * 4, n,
-                                        cudaMemcpyDefault, stream));
-        src = ws->pcm_dev;
-        src_stride = kWindowSamples;
-    }
+    const float* src;
+    int64_t src_stride;
+    WK_CHECK(mel_stage(ws, pcm, n, stride, stream, &src, &src_stride));
     const int32_t* nv = nullptr;
     if (samples_per_window) {
         for (int64_t i = 0; i < n; ++i)

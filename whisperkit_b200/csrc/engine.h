@@ -105,6 +105,9 @@ struct wk_model {
 namespace wk {
 
 wk_status enc_ws_ensure(wk_model* m, EncWorkspace* ws, int max_batch);
+// the staging half of mel_run: host PCM, or rows shorter than a window, copied into ws->pcm_dev (zero-padded) on `stream`; *src /
+// *src_stride are the rows the mel kernel reads
+wk_status mel_stage(EncWorkspace* ws, const float* pcm, int64_t n, int64_t stride, cudaStream_t stream, const float** src, int64_t* src_stride);
 // PCM rows (host or device) -> staged in ws->pcm_dev when needed -> log-mel into mel_out ([n][3002][128] f16), all on `stream`
 wk_status mel_run(wk_model* m, EncWorkspace* ws, const float* pcm, int64_t n, int64_t stride, const int32_t* samples_per_window_host,
                   void* mel_out, cudaStream_t stream);

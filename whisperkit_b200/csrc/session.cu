@@ -81,7 +81,6 @@ struct wk_session {
     BeamState bs = BeamState(); int bs_cap_rows = 0;
     int32_t *h_n_fin = nullptr, *h_fin_len = nullptr, *h_fin_tokens = nullptr; float *h_fin_score = nullptr, *h_fin_lps = nullptr, *h_sum_lp = nullptr;
     int graph_beam = 1;
-    std::vector<int> slot_window, slot_try;
     int64_t stats[4] = {0, 0, 0, 0};   // of the last batched call: step launches, sum of live rows over them, admissions, ladder re-admissions
     AudioWs* audio = nullptr;          // wk_audio_load / wk_audio_convert workspace (audio.cu)
     int32_t* pos100 = nullptr;         // wk_bench_kernel's self-attention positions (all 100)
@@ -217,25 +216,9 @@ static SamplerParams loop_sampler_params(wk_session* s, const wk_special_tokens*
     return p;
 }
 
-// TextUtilities.compressionRatio(of: [Int]) (TextUtilities.swift:14-28): raw DEFLATE of the Int32 LE bytes
-static float compression_ratio(const std::vector<int32_t>& toks) {
-    if (toks.empty()) return INFINITY;
-    const uLong n = (uLong)toks.size() * 4;
-    z_stream zs;
-    memset(&zs, 0, sizeof(zs));
-    if (deflateInit2(&zs, 5, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) != Z_OK) return INFINITY;
-    std::vector<unsigned char> out(deflateBound(&zs, n) + 64);
-    zs.next_in = (Bytef*)toks.data(); zs.avail_in = n;
-    zs.next_out = out.data(); zs.avail_out = (uInt)out.size();
-    const int r = deflate(&zs, Z_FINISH);
-    const uLong clen = zs.total_out;
-    deflateEnd(&zs);
-    if (r != Z_STREAM_END || clen == 0) return INFINITY;
-    return (float)n / (float)clen;
-}
-
-// the same ratio on one deflate state kept across calls (deflateReset instead of a fresh deflateInit2: same output, no allocation) -
-// the stream stop rule evaluates it once per decoded token
+// TextUtilities.compressionRatio(of: [Int]) (TextUtilities.swift:14-28): raw DEFLATE of the Int32 LE bytes, on one deflate state kept
+// across the windows of a call (deflateReset gives the output of a fresh deflateInit2 without its allocation) - the stream stop rule
+// evaluates it once per decoded token
 namespace {
 struct Deflater {
     z_stream zs;
@@ -275,7 +258,7 @@ static int stop_rule_index(const StopRule& rule, Deflater& z, const int32_t* tok
 
 // finalisation of one window on the host: finalize + slicing + averages (TextDecoder.swift:776-853)
 static void finalize_result(wk_decode_result& r, const int32_t* tokens, const float* lps, int n_tok, int steps, int first_low,
-                            const wk_special_tokens* st, const wk_decode_opts* o, float temperature, float no_speech_prob) {
+                            const wk_special_tokens* st, const wk_decode_opts* o, float temperature, float no_speech_prob, Deflater& z) {
     memset(&r, 0, sizeof(r));
     std::vector<int32_t> seg(tokens, tokens + n_tok);
     std::vector<float> slp(lps, lps + n_tok);
@@ -299,7 +282,7 @@ static void finalize_result(wk_decode_result& r, const int32_t* tokens, const fl
         ++r.n_tokens;
     }
     r.avg_logprob = sum / (float)r.n_tokens;
-    r.compression_ratio = compression_ratio(words);
+    r.compression_ratio = z.ratio(words.data(), (int)words.size());
     r.temperature = roundf(temperature * 1000.f) / 1000.f;
     // DecodingFallback (Models.swift:357-381); noSpeechProb is 0 unless the window computes it (the reference's is always 0,
     // TextDecoder.swift:802)
@@ -311,7 +294,7 @@ static void finalize_result(wk_decode_result& r, const int32_t* tokens, const fl
 }
 
 // prefillDecoderInputs (TextDecoder.swift:163-216)
-static wk_status build_prompt(const wk_model* m, const wk_special_tokens* st, const wk_decode_opts* o, int use_options, std::vector<int32_t>& p) {
+static void build_prompt(const wk_model* m, const wk_special_tokens* st, const wk_decode_opts* o, int use_options, std::vector<int32_t>& p) {
     p.clear();
     p.push_back(st->start_of_transcript_token);
     if (use_options && o) {
@@ -338,7 +321,6 @@ static wk_status build_prompt(const wk_model* m, const wk_special_tokens* st, co
                 if (o->prefix_tokens[i] < st->special_token_begin) p.push_back(o->prefix_tokens[i]);
         }
     }
-    return WK_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- the step and its graph
@@ -456,102 +438,110 @@ static wk_status ensure_beam(wk_session* s) {
     return WK_OK;
 }
 
-static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
-    wk_model* m = s->m;
-    const wk_model_config& c = m->cfg;
+// One window as the call decodes it: its prompt, the index of the prompt's first <|startoftranscript|> (-1: none) and whether the window
+// detects its language in the loop
+struct WindowPlan { const int32_t* p = nullptr; int np = 0, sot = -1; bool detects = false; };
+
+// What a call decodes, worked out on the host before any CUDA work
+struct CallPlan {
+    int beam = 1, best_of = 0, G = 1, max_cand = 0;   // G = max(beam, best_of): decode rows per window
+    std::vector<WindowPlan> win;
+    std::vector<std::vector<int32_t>> built;          // the prompts built from the options, when the call passes none
+    std::vector<int32_t> sup_pool;                    // suppress ids of every option set: set i's at [sup_off[i], sup_off[i] + sup_n[i])
+    std::vector<int> sup_off, sup_n;
+    std::vector<int32_t> lang_list, lang_sorted;      // the call's allLanguageTokens: one list for every detecting window (one device buffer)
+    std::vector<wk_status> st_local;
+    wk_status* status = nullptr;                      // per window: bo->status, or st_local
+    std::string first_err;                            // the message of the first window that failed
+    bool any_words = false, any_detect = false, any_nsp = false;
+    void fail(int64_t w, wk_status code, wk_decode_result* results) {
+        status[w] = code;
+        if (first_err.empty()) first_err = last_error_cstr();
+        memset(&results[w], 0, sizeof(wk_decode_result));
+    }
+};
+
+// Checks the call's options and windows and builds its plan; resets the session's per-window outputs of the last call.  A bad window
+// fails alone (WhisperKit.swift:775-790); a call without a status array returns the first failure in the order of the passes below
+static wk_status plan_call(wk_session* s, const CoreArgs& a, CallPlan& p) {
+    const wk_model_config& c = s->m->cfg;
     const wk_batch_opts* bo = a.bo;
     const wk_special_tokens* st = a.st;
-    const bool bound = a.pcm == nullptr;
     const int64_t n = a.n;
-    const int d = c.d_model, T = c.n_audio_ctx;
-    const int poll = bo->progress_every > 0 ? bo->progress_every : 16;
     // beam search / best-of: every window takes G = max(beam, best_of) consecutive decode rows; one setting per call (it shapes the step
     // graph).  best_of == 0 keeps the plain rule: beam search (no ladder) or one row; best_of >= 1 picks the rows per ladder rung
-    const int beam = bo->opts[0].beam_size > 1 ? bo->opts[0].beam_size : 1;
-    const int best_of = bo->best_of;
+    const int beam = p.beam = bo->opts[0].beam_size > 1 ? bo->opts[0].beam_size : 1;
+    const int best_of = p.best_of = bo->best_of;
     for (int i = 0; i < bo->n_opts; ++i)
         if ((bo->opts[i].beam_size > 1 ? bo->opts[i].beam_size : 1) != beam || (beam > 1 && bo->opts[i].beam_patience != bo->opts[0].beam_patience)) {
             set_error("beam size / patience must be the same for every window of a call"); return WK_ERR_INVALID_ARGUMENT;
         }
     if (best_of < 0 || best_of > kMaxBeam) { set_error("best_of %d outside [0, %d]", best_of, kMaxBeam); return WK_ERR_INVALID_ARGUMENT; }
-    const int G = std::max(beam, std::max(best_of, 1));
+    const int G = p.G = std::max(beam, std::max(best_of, 1));
     if (G > s->max_batch) {
         set_error("%d rows per window (beam size %d, best_of %d) exceed the session's %d rows", G, beam, best_of, s->max_batch);
         return WK_ERR_INVALID_ARGUMENT;
     }
     if (a.stop && (G != 1 || a.stop->window < 1)) { set_error("the stream stop rule needs single-row windows and a check window >= 1"); return WK_ERR_INVALID_ARGUMENT; }
-    int max_cand = 0;
     if (beam > 1) {
         const float patience = bo->opts[0].beam_patience > 0.f ? bo->opts[0].beam_patience : 1.f;
-        max_cand = (int)((float)beam * patience);                                  // TokenSampler.swift:266
-        if (beam > kMaxBeam || max_cand < 1 || max_cand > kMaxCand || s->max_batch < beam) {
+        p.max_cand = (int)((float)beam * patience);                                  // TokenSampler.swift:266
+        if (beam > kMaxBeam || p.max_cand < 1 || p.max_cand > kMaxCand || s->max_batch < beam) {
             set_error("beam size %d / patience %.2f unsupported (beam <= %d, candidates in [1, %d], session rows %d)", beam, patience, kMaxBeam, kMaxCand, s->max_batch);
             return WK_ERR_INVALID_ARGUMENT;
         }
         for (int i = 0; i < bo->n_opts; ++i)
             if (bo->opts[i].word_timestamps) { set_error("wordTimestamps with beam search is not supported"); return WK_ERR_INVALID_ARGUMENT; }
-        WK_CHECK(ensure_beam(s));
     }
-    s->bs.beam = beam; s->bs.max_candidates = max_cand; s->bs.group = G;
-    const int S = s->max_batch / G;        // decode slots (windows in flight)
-    if (bound && n > S) { set_error("wk_decode_text: %lld bound windows x %d rows exceed the session's %d rows", (long long)n, G, s->max_batch); return WK_ERR_PREPARE_DECODER_INPUTS; }
-    std::vector<wk_status> st_local((size_t)n, WK_OK);
-    wk_status* status = bo->status ? bo->status : st_local.data();
-    for (int64_t w = 0; w < n; ++w) status[w] = WK_OK;
-    std::string first_err;
-    auto fail_window = [&](int64_t w, wk_status code) {
-        status[w] = code;
-        if (first_err.empty()) first_err = last_error_cstr();
-        memset(&a.results[w], 0, sizeof(wk_decode_result));
-    };
-    // ---- per-window prompts, options, suppress lists (validated up front: a bad item fails alone, WhisperKit.swift:775-790)
-    std::vector<std::vector<int32_t>> prompts((size_t)(bo->prompts || bo->prompt ? 0 : (bo->n_opts == 1 ? 1 : n)));
-    std::vector<int32_t> shared_built;
-    auto prompt_of = [&](int64_t w, const int32_t** p, int* np) {
-        if (bo->prompts) { *p = bo->prompts[w]; *np = bo->prompt_lens[w]; }
-        else if (bo->prompt) { *p = bo->prompt; *np = bo->n_prompt; }
-        else { const auto& v = prompts[bo->n_opts == 1 ? 0 : (size_t)w]; *p = v.data(); *np = (int)v.size(); }
-    };
-    if (!bo->prompts && !bo->prompt)
-        for (size_t i = 0; i < prompts.size(); ++i) {
+    if (!a.pcm && n > s->max_batch / G) { set_error("wk_decode_text: %lld bound windows x %d rows exceed the session's %d rows", (long long)n, G, s->max_batch); return WK_ERR_PREPARE_DECODER_INPUTS; }
+    p.st_local.assign((size_t)n, WK_OK);
+    p.status = bo->status ? bo->status : p.st_local.data();
+    for (int64_t w = 0; w < n; ++w) p.status[w] = WK_OK;
+    // ---- per-window prompts, options, suppress lists
+    if (!bo->prompts && !bo->prompt) {
+        p.built.resize(bo->n_opts == 1 ? 1 : (size_t)n);
+        for (size_t i = 0; i < p.built.size(); ++i) {
             const wk_decode_opts& o = opts_of(bo, (int64_t)i);
-            build_prompt(m, st, &o, o.use_prefill_prompt, prompts[i]);
+            build_prompt(s->m, st, &o, o.use_prefill_prompt, p.built[i]);
         }
-    bool any_words = false;
-    std::vector<int32_t> sup_pool;
-    std::vector<int> sup_off((size_t)bo->n_opts), sup_n((size_t)bo->n_opts);
+    }
+    p.sup_off.resize(bo->n_opts);
+    p.sup_n.resize(bo->n_opts);
     for (int i = 0; i < bo->n_opts; ++i) {
         const wk_decode_opts& o = bo->opts[i];
-        any_words |= o.word_timestamps != 0;
-        sup_off[i] = (int)sup_pool.size();
+        p.any_words |= o.word_timestamps != 0;
+        p.sup_off[i] = (int)p.sup_pool.size();
         for (int k = 0; k < o.n_suppress_tokens; ++k)   // SuppressTokensFilter gets the (< specialTokenBegin) ids only (TextDecoder.swift:876-879)
-            if (o.suppress_tokens[k] >= 0 && o.suppress_tokens[k] < st->special_token_begin) sup_pool.push_back(o.suppress_tokens[k]);
-        sup_n[i] = (int)sup_pool.size() - sup_off[i];
+            if (o.suppress_tokens[k] >= 0 && o.suppress_tokens[k] < st->special_token_begin) p.sup_pool.push_back(o.suppress_tokens[k]);
+        p.sup_n[i] = (int)p.sup_pool.size() - p.sup_off[i];
     }
+    p.win.resize((size_t)n);
     for (int64_t w = 0; w < n; ++w) {
-        const int32_t* p; int np;
-        prompt_of(w, &p, &np);
-        if (!p || np < 1 || np >= kKvMaxLen) { set_error("window %lld: prompt length %d out of range", (long long)w, np); fail_window(w, WK_ERR_PREPARE_DECODER_INPUTS); continue; }
+        WindowPlan& wp = p.win[w];
+        if (bo->prompts) { wp.p = bo->prompts[w]; wp.np = bo->prompt_lens[w]; }
+        else if (bo->prompt) { wp.p = bo->prompt; wp.np = bo->n_prompt; }
+        else { const auto& v = p.built[bo->n_opts == 1 ? 0 : (size_t)w]; wp.p = v.data(); wp.np = (int)v.size(); }
+        if (!wp.p || wp.np < 1 || wp.np >= kKvMaxLen) { set_error("window %lld: prompt length %d out of range", (long long)w, wp.np); p.fail(w, WK_ERR_PREPARE_DECODER_INPUTS, a.results); continue; }
         bool ok = true;
-        for (int i = 0; i < np && ok; ++i)
-            if (p[i] < 0 || p[i] >= c.vocab) { set_error("window %lld: prompt token %d out of range", (long long)w, p[i]); ok = false; }
-        if (!ok) { fail_window(w, WK_ERR_PREPARE_DECODER_INPUTS); continue; }
-        if (!bound && a.spw && (a.spw[w] < 0 || a.spw[w] > kWindowSamples)) {
+        for (int i = 0; i < wp.np && ok; ++i)
+            if (wp.p[i] < 0 || wp.p[i] >= c.vocab) { set_error("window %lld: prompt token %d out of range", (long long)w, wp.p[i]); ok = false; }
+        if (!ok) { p.fail(w, WK_ERR_PREPARE_DECODER_INPUTS, a.results); continue; }
+        const int32_t* sot = std::find(wp.p, wp.p + wp.np, st->start_of_transcript_token);
+        wp.sot = sot == wp.p + wp.np ? -1 : (int)(sot - wp.p);
+        if (a.pcm && a.spw && (a.spw[w] < 0 || a.spw[w] > kWindowSamples)) {
             set_error("window %lld: samples_per_window %d out of range", (long long)w, a.spw[w]);
-            fail_window(w, WK_ERR_AUDIO_PROCESSING_FAILED);
+            p.fail(w, WK_ERR_AUDIO_PROCESSING_FAILED, a.results);
         }
     }
     // ---- in-loop language detection (DecodingOptions.detectLanguage): a multilingual model, no language set (TranscribeTask.swift:341)
     const bool multilingual = c.vocab != 51864;
-    auto detects = [&](const wk_decode_opts& o) { return o.detect_language != 0 && multilingual && o.language_token < 0; };
-    std::vector<int32_t> lang_list;   // the call's allLanguageTokens: one list for every detecting window (one device buffer)
-    bool any_detect = false;
     for (int64_t w = 0; w < n; ++w) {
         const wk_decode_opts& o = opts_of(bo, w);
-        if (status[w] != WK_OK || !detects(o)) continue;
+        p.win[w].detects = o.detect_language != 0 && multilingual && o.language_token < 0;
+        if (p.status[w] != WK_OK || !p.win[w].detects) continue;
         if (!o.language_tokens || o.n_language_tokens < 1 || o.n_language_tokens > 4096) {
             set_error("window %lld: detectLanguage needs 1..4096 language tokens (got %d)", (long long)w, o.language_tokens ? o.n_language_tokens : 0);
-            fail_window(w, WK_ERR_INVALID_ARGUMENT);
+            p.fail(w, WK_ERR_INVALID_ARGUMENT, a.results);
             continue;
         }
         bool ok = true;
@@ -560,295 +550,358 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 set_error("window %lld: language token %d outside the vocabulary (%d)", (long long)w, o.language_tokens[i], c.vocab);
                 ok = false;
             }
-        if (ok && any_detect &&
-            ((int)lang_list.size() != o.n_language_tokens || !std::equal(lang_list.begin(), lang_list.end(), o.language_tokens))) {
+        if (ok && p.any_detect &&
+            ((int)p.lang_list.size() != o.n_language_tokens || !std::equal(p.lang_list.begin(), p.lang_list.end(), o.language_tokens))) {
             set_error("window %lld: every detecting window of a call must carry the same language tokens", (long long)w);
             ok = false;
         }
-        if (!ok) { fail_window(w, WK_ERR_INVALID_ARGUMENT); continue; }
-        if (!any_detect) lang_list.assign(o.language_tokens, o.language_tokens + o.n_language_tokens);
-        any_detect = true;
+        if (!ok) { p.fail(w, WK_ERR_INVALID_ARGUMENT, a.results); continue; }
+        if (!p.any_detect) p.lang_list.assign(o.language_tokens, o.language_tokens + o.n_language_tokens);
+        p.any_detect = true;
     }
-    std::vector<int32_t> lang_sorted(lang_list);
-    std::sort(lang_sorted.begin(), lang_sorted.end());
-    s->win_lang.assign((size_t)n, -1);
-    s->win_lang_logprob.assign((size_t)n, 0.f);
+    p.lang_sorted = p.lang_list;
+    std::sort(p.lang_sorted.begin(), p.lang_sorted.end());
     // ---- noSpeechProb (compute_no_speech_prob): the value comes from the step that feeds the prompt's first SOT, so that SOT must exist
-    auto sot_index = [&](int64_t w) -> int {
-        const int32_t* p; int np;
-        prompt_of(w, &p, &np);
-        const int32_t* sot = std::find(p, p + np, st->start_of_transcript_token);
-        return sot == p + np ? -1 : (int)(sot - p);
-    };
-    bool any_nsp = false;
     for (int64_t w = 0; w < n; ++w) {
-        if (status[w] != WK_OK || !opts_of(bo, w).compute_no_speech_prob) continue;
-        if (sot_index(w) < 0) {
+        if (p.status[w] != WK_OK || !opts_of(bo, w).compute_no_speech_prob) continue;
+        if (p.win[w].sot < 0) {
             set_error("window %lld: computeNoSpeechProb needs <|startoftranscript|> (token %d) in the prompt, which has none", (long long)w,
                       st->start_of_transcript_token);
-            fail_window(w, WK_ERR_PREPARE_DECODER_INPUTS);
+            p.fail(w, WK_ERR_PREPARE_DECODER_INPUTS, a.results);
             continue;
         }
-        any_nsp = true;
+        p.any_nsp = true;
     }
+    s->win_lang.assign((size_t)n, -1);
+    s->win_lang_logprob.assign((size_t)n, 0.f);
     s->win_no_speech.assign((size_t)n, NAN);
-    if (!bound && a.stride < kWindowSamples && !a.spw) { set_error("wk_transcribe_windows: stride < 480000 requires samples_per_window"); return WK_ERR_AUDIO_PROCESSING_FAILED; }
+    if (a.pcm && a.stride < kWindowSamples && !a.spw) { set_error("wk_transcribe_windows: stride < 480000 requires samples_per_window"); return WK_ERR_AUDIO_PROCESSING_FAILED; }
     if (!bo->status)
-        for (int64_t w = 0; w < n; ++w) if (status[w] != WK_OK) { set_error("%s", first_err.c_str()); return status[w]; }
-    if (sup_pool.size() > s->suppress_cap) {
-        const size_t cap = std::max<size_t>(4096, sup_pool.size() * 2);
+        for (int64_t w = 0; w < n; ++w) if (p.status[w] != WK_OK) { set_error("%s", p.first_err.c_str()); return p.status[w]; }
+    return WK_OK;
+}
+
+// the plan's suppress pool and language list on the device
+static wk_status upload_plan(wk_session* s, const CallPlan& p) {
+    if (p.sup_pool.size() > s->suppress_cap) {
+        const size_t cap = std::max<size_t>(4096, p.sup_pool.size() * 2);
         WK_CHECK(s->mem.grow(&s->suppress_dev, cap, s->stream));
         s->suppress_cap = cap;
         drop_graphs(s);   // pool pointer is baked into the graphs
     }
-    if (!sup_pool.empty()) WK_CUDA_CHECK(cudaMemcpyAsync(s->suppress_dev, sup_pool.data(), sup_pool.size() * 4, cudaMemcpyHostToDevice, s->stream));
-    if (any_detect) WK_CUDA_CHECK(cudaMemcpyAsync(s->lang_dev, lang_list.data(), lang_list.size() * 4, cudaMemcpyHostToDevice, s->stream));
-    WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));   // sup_pool is pageable: the copy must land before it goes out of scope paths below reuse it
-    s->align_on = any_words;
+    if (!p.sup_pool.empty()) WK_CUDA_CHECK(cudaMemcpyAsync(s->suppress_dev, p.sup_pool.data(), p.sup_pool.size() * 4, cudaMemcpyHostToDevice, s->stream));
+    if (p.any_detect) WK_CUDA_CHECK(cudaMemcpyAsync(s->lang_dev, p.lang_list.data(), p.lang_list.size() * 4, cudaMemcpyHostToDevice, s->stream));
+    WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));   // the host lists are pageable
+    return WK_OK;
+}
+
+// temperature of ladder rung i, computed in Float16 like the reference (TranscribeTask.swift:327)
+static float rung_temperature(const wk_decode_opts& o, int i) {
+    if (i == 0) return o.temperature;
+    const float f16_t = __half2float(__float2half(o.temperature));
+    const float f16_step = __half2float(__float2half(__half2float(__float2half((float)i)) * __half2float(__float2half(o.temperature_increment_on_fallback))));
+    return __half2float(__float2half(f16_t + f16_step));
+}
+
+// the rows a rung decodes with (openai/whisper decode_with_fallback): best_of == 0 - beam search on every row of a beam call, else one
+// row; best_of >= 1 - beam search at temperature 0 when beam > 1, best_of independent samples at temperature > 0 when best_of > 1,
+// else one row.  The group's other rows stay ended
+static int rung_mode(int beam, int best_of, float temperature, int* active) {
+    if (beam > 1 && (best_of == 0 || temperature == 0.f)) { *active = beam; return kRowBeam; }
+    if (best_of > 1 && temperature > 0.f) { *active = best_of; return kRowSample; }
+    *active = 1;
+    return kRowSingle;
+}
+
+// the decode rows of window w at ladder rung `rung`; *active: how many of its G rows the rung decodes with
+static RowParams row_params(const CallPlan& p, const wk_batch_opts* bo, const wk_special_tokens* st, int64_t w, int rung, int* active) {
+    const wk_decode_opts& o = opts_of(bo, w);
+    const int oi = bo->n_opts == 1 ? 0 : (int)w;
+    const WindowPlan& wp = p.win[w];
+    RowParams R;
+    memset(&R, 0, sizeof(R));
+    R.prompt_len = wp.np;
+    // createLogitsFilters (TextDecoder.swift:857-899): SuppressBlank(sampleBegin = prefilledIndex = 0), TimestampRules(sampleBegin = initialPrompt.count)
+    R.sample_begin_ts = o.without_timestamps ? -1 : wp.np;
+    R.sample_begin_blank = o.suppress_blank ? 0 : -1;
+    R.max_steps = std::max(1, std::min(o.sample_length, kKvMaxLen - 1));   // TextDecoder.swift:566
+    R.temperature = rung_temperature(o, rung); R.top_k = o.top_k;
+    R.has_first_thr = o.has_first_token_logprob_threshold; R.first_thr = o.first_token_logprob_threshold;
+    R.seed = o.seed + (uint64_t)rung;
+    R.suppress_off = p.sup_off[oi]; R.n_suppress = p.sup_n[oi];
+    // every rung detects again at its own temperature (detectLanguage runs inside decodeWithFallback's loop, TranscribeTask.swift:333-365)
+    R.lead_token = st->start_of_transcript_token;
+    R.lang_pos = -1;
+    R.no_speech_pos = o.compute_no_speech_prob ? wp.sot : -1;   // the same step at every rung
+    if (wp.detects) {
+        R.detect = wp.p[0] == st->start_of_transcript_token ? 1 : 2;
+        R.n_lang = (int32_t)p.lang_list.size();
+        // usePrefillPrompt: the prompt is rebuilt with the detected language - prefillDecoderInputs puts <|xx|> right after the first
+        // SOT (TextDecoder.swift:176-186); a prompt without a language token there only reports the language
+        const int i = wp.sot + 1;
+        if (o.use_prefill_prompt && wp.sot >= 0 && i < wp.np && std::binary_search(p.lang_sorted.begin(), p.lang_sorted.end(), wp.p[i])) R.lang_pos = i;
+    }
+    R.mode = rung_mode(p.beam, p.best_of, R.temperature, active);
+    return R;
+}
+
+// The decode slots of a call: the window each holds (-1: free), its ladder rung, and the stream stop rule's progress through the window's
+// history (entries checked, their log-prob sum).  admit() stages the window's rows in the session's pinned buffers, flush() sends what
+// is staged to the device in one go
+struct Slots {
+    wk_session* s; const CallPlan& p; const CoreArgs& a;
+    std::vector<int> window, rung, stop_checked;
+    std::vector<float> stop_sum;
+    int live = 0, staged = 0;   // slots holding a window; rows staged since the last flush
+    Slots(wk_session* s, const CallPlan& p, const CoreArgs& a, int S) : s(s), p(p), a(a), window(S, -1), rung(S, 0), stop_checked(S, 0), stop_sum(S, 0.f) {}
+
+    // window w into free slot q at rung 0, or back into its slot at the next rung
+    wk_status admit(int q, int64_t w, int r) {
+        int active = 1;
+        const RowParams R = row_params(p, a.bo, a.st, w, r, &active);
+        if (staged == 0) WK_CUDA_CHECK(cudaEventSynchronize(s->ev_stage));   // the previous round's copies out of the pinned staging have landed
+        for (int j = 0; j < active; ++j) {                                     // beam search / best-of: `active` identical rows start the window
+            s->h_adm_slots[staged] = q * p.G + j;
+            memset(s->h_adm_prompts + (size_t)staged * kKvMaxLen, 0, kKvMaxLen * 4);
+            memcpy(s->h_adm_prompts + (size_t)staged * kKvMaxLen, p.win[w].p, (size_t)p.win[w].np * 4);
+            s->h_adm_rp[staged] = R;
+            ++staged;
+        }
+        if (r == 0) { ++live; ++s->stats[2]; } else { ++s->stats[3]; }
+        window[q] = (int)w; rung[q] = r; stop_checked[q] = 0; stop_sum[q] = 0.f;
+        return WK_OK;
+    }
+    wk_status flush() {
+        if (staged == 0) return WK_OK;
+        const int T = s->m->cfg.n_audio_ctx;
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->d_adm_slots, s->h_adm_slots, (size_t)staged * 4, cudaMemcpyHostToDevice, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->d_adm_prompts, s->h_adm_prompts, (size_t)staged * kKvMaxLen * 4, cudaMemcpyHostToDevice, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->d_adm_rp, s->h_adm_rp, (size_t)staged * sizeof(RowParams), cudaMemcpyHostToDevice, s->stream));
+        if (s->align_on)
+            for (int i = 0; i < staged; ++i)   // row 0 and unreached rows of alignmentWeights stay 0
+                WK_CUDA_CHECK(cudaMemsetAsync((char*)s->align_w + (size_t)s->h_adm_slots[i] * kKvMaxLen * T * 2, 0, (size_t)kKvMaxLen * T * 2, s->stream));
+        WK_CHECK(decode_slots_init(s->st, s->rp_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, staged, s->stream, s->bs));
+        WK_CUDA_CHECK(cudaEventRecord(s->ev_stage, s->stream));
+        staged = 0;
+        return WK_OK;
+    }
+};
+
+// samples_per_window of windows [w0, w0 + cnt), those that failed validation masked to 0: encoded as silence, they never reach a slot
+template <typename Status>
+static const int32_t* mask_failed(const int32_t* spw, const Status* status, int64_t w0, int64_t cnt, std::vector<int32_t>& buf) {
+    if (!spw) return nullptr;
+    buf.assign(spw + w0, spw + w0 + cnt);
+    for (int64_t i = 0; i < cnt; ++i) if (status[w0 + i] != WK_OK) buf[i] = 0;
+    return buf.data();
+}
+
+// The encoder side of a call: chunks of windows through mel + encoder on the encoder stream while the decode stream runs, and the
+// cross-attention K/V of the windows admitted from the chunk in enc_out.  acc: the stage times of wk_last_timings
+struct EncoderFeed {
+    wk_session* s; const CoreArgs& a; const wk_status* status; int Ec;
+    int64_t next = 0, w0 = 0, n = 0, adm = 0;   // the next window to encode; the chunk in enc_out - windows [w0, w0 + n), adm of them handled
+    bool waited = true;                         // the decode stream waits for the chunk's encoder output
+    bool pending = false, ckv_timing = false;   // the chunk's stage times are unread; ev_t[4..5] hold an unread projection region
+    float acc[6] = {0, 0, 0, 0, 0, 0};
+
+    wk_status encode() {
+        const int64_t nc = std::min<int64_t>(Ec, a.n - next);
+        std::vector<int32_t> spw_buf;
+        const int32_t* spw = mask_failed(a.spw, status, next, nc, spw_buf);
+        cudaStream_t es = s->enc_stream;
+        WK_CUDA_CHECK(cudaStreamWaitEvent(es, s->ev_adm, 0));   // the previous chunk's cross-KV projections have read enc_out
+        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[0], es));
+        const float* src;
+        int64_t src_stride;
+        WK_CHECK(mel_stage(&s->ws, a.pcm + next * a.stride, nc, a.stride, es, &src, &src_stride));   // timed apart from the mel kernel
+        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[1], es));
+        WK_CHECK(mel_run(s->m, &s->ws, src, nc, src_stride, spw, s->ws.mel, es));
+        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[2], es));
+        WK_CHECK(encode_chunk(s->m, &s->ws, s->ws.mel, (int)nc, s->ws.enc_out, es));
+        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[3], es));
+        WK_CUDA_CHECK(cudaEventRecord(s->ev_enc, es));
+        w0 = next; n = nc; adm = 0; next += nc; waited = false; pending = true;
+        return WK_OK;
+    }
+    // the chunk's windows into the free slots among the first `slots`, passing over the windows that failed validation; windows going
+    // to consecutive slots share one projection GEMM, and the round's first one opens the timed region unless one is still unread
+    wk_status admit(Slots& sl, int slots) {
+        const size_t win_bytes = (size_t)s->m->cfg.n_audio_ctx * s->m->cfg.d_model * 2;
+        bool first = true;
+        for (int q = 0;;) {
+            while (adm < n && status[w0 + adm] != WK_OK) ++adm;
+            while (q < slots && sl.window[q] >= 0) ++q;
+            if (adm == n || q == slots) break;
+            const int q0 = q;
+            const int64_t run0 = adm;
+            for (; q < slots && adm < n && sl.window[q] < 0 && status[w0 + adm] == WK_OK; ++q, ++adm) WK_CHECK(sl.admit(q, w0 + adm, 0));
+            if (!waited) { WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, s->ev_enc, 0)); waited = true; }
+            if (first && !ckv_timing) WK_CUDA_CHECK(cudaEventRecord(s->ev_t[4], s->stream));
+            first = false;
+            WK_CHECK(gemm_wgmma(cross_kv_gemm(s, (const char*)s->ws.enc_out + run0 * win_bytes, q - q0, q0), s->m->num_sms, s->stream));
+        }
+        if (!first && !ckv_timing) { WK_CUDA_CHECK(cudaEventRecord(s->ev_t[5], s->stream)); ckv_timing = true; }
+        if (adm == n) WK_CUDA_CHECK(cudaEventRecord(s->ev_adm, s->stream));
+        return sl.flush();
+    }
+    // the stage times of finished work: after a burst's readback the burst (ev_t[6..7]) and the projections before it, then the chunk's
+    // staging, mel and encoder once they have run
+    void collect(bool after_burst) {
+        float t;
+        if (after_burst) {
+            cudaEventElapsedTime(&t, s->ev_t[6], s->ev_t[7]); acc[3] += t;
+            if (ckv_timing) { cudaEventElapsedTime(&t, s->ev_t[4], s->ev_t[5]); acc[2] += t; ckv_timing = false; }
+        }
+        if (!pending || cudaEventQuery(s->ev_t[3]) != cudaSuccess) return;
+        cudaEventElapsedTime(&t, s->ev_t[0], s->ev_t[1]); acc[4] += t;
+        cudaEventElapsedTime(&t, s->ev_t[1], s->ev_t[2]); acc[0] += t;
+        cudaEventElapsedTime(&t, s->ev_t[2], s->ev_t[3]); acc[1] += t;
+        pending = false;
+    }
+};
+
+// the decode state of the step's rows back in the session's pinned buffers, in one synchronisation
+static wk_status read_back(wk_session* s, const CallPlan& p) {
+    const int rows = s->batch, slots = s->batch / p.G;
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_done, s->st.done, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_tokens, s->st.n_tokens, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_steps, s->st.steps, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_first_low, s->st.first_low, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_error, s->st.error, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_tokens, s->st.tokens, (size_t)rows * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
+    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_logprobs, s->st.logprobs, (size_t)rows * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
+    if (p.any_detect) {
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_token, s->st.lang_token, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_logprob, s->st.lang_logprob, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    }
+    if (p.any_nsp) WK_CUDA_CHECK(cudaMemcpyAsync(s->h_no_speech, s->st.no_speech, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    if (p.beam > 1) {
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_sum_lp, s->bs.sum_lp, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_fin, s->bs.n_fin, slots * 4, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_len, s->bs.fin_len, (size_t)slots * kMaxCand * 4, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_score, s->bs.fin_score, (size_t)slots * kMaxCand * 4, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_tokens, s->bs.fin_tokens, (size_t)slots * kMaxCand * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_lps, s->bs.fin_lps, (size_t)slots * kMaxCand * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
+    }
+    const cudaError_t e = cudaStreamSynchronize(s->stream);
+    if (e != cudaSuccess) { set_error("decode loop: %s", cudaGetErrorString(e)); return WK_ERR_DECODING_FAILED; }
+    return WK_OK;
+}
+
+// The sequence the window in slot q returns, from the readback of its rows (first row q * G) decoded in rung mode `mode`: the row's own
+// history, the best-ranked best-of sample or the beam search winner (P: prompt length); cut after the token the stream stop rule stops
+// at when stop_at >= 0.  Points into the session's pinned readback buffers
+struct Choice { int row; const int32_t* tok; const float* lp; int n; };
+static Choice select_result(const wk_session* s, int q, int G, int mode, int beam, int best_of, int P, int stop_at) {
+    const int r0 = q * G;
+    int rc = r0;                              // the row whose result the window returns
+    if (mode == kRowSample) {
+        // best-of: MaximumLikelihoodRanker without length penalty over the samples (oracle/best_of_ref.py rank_best_of) - the sum of
+        // the row's recorded log-probs over max(sampled tokens, 1); ties go to the lowest row
+        float best_rank = -INFINITY;
+        for (int j = 0; j < best_of; ++j) {
+            const int rr = r0 + j;
+            const float* lp = s->h_logprobs + (size_t)rr * kKvMaxLen;
+            float sum = 0.f;
+            for (int i = 0; i < s->h_n_tokens[rr]; ++i) sum += lp[i];
+            const float rk = sum / (float)std::max(s->h_n_tokens[rr] - P, 1);
+            if (j == 0 || rk > best_rank) { rc = rr; best_rank = rk; }
+        }
+    }
+    Choice ch{rc, s->h_tokens + (size_t)rc * kKvMaxLen, s->h_logprobs + (size_t)rc * kKvMaxLen, s->h_n_tokens[rc]};
+    if (mode == kRowBeam) {
+        // BeamSearchDecoder.finalize + MaximumLikelihoodRanker (oracle/beam_ref.py): the finished list, topped up with the live beams
+        // (best sum first) to `beam` entries; the winner maximises sum_logprob / sampled tokens
+        struct Cand { const int32_t* tok; const float* lp; int len; float score; bool live; };
+        std::vector<Cand> cands;
+        const int nf = std::min(s->h_n_fin[q], kMaxCand);
+        for (int f = 0; f < nf; ++f) {
+            const size_t slot = (size_t)q * kMaxCand + f;
+            cands.push_back(Cand{s->h_fin_tokens + slot * kKvMaxLen, s->h_fin_lps + slot * kKvMaxLen, s->h_fin_len[slot], s->h_fin_score[slot], false});
+        }
+        if ((int)cands.size() < beam) {
+            std::vector<int> order(beam);
+            for (int j = 0; j < beam; ++j) order[j] = j;
+            std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return s->h_sum_lp[r0 + x] > s->h_sum_lp[r0 + y]; });
+            for (int j : order) {
+                const int rr = r0 + j;
+                cands.push_back(Cand{s->h_tokens + (size_t)rr * kKvMaxLen, s->h_logprobs + (size_t)rr * kKvMaxLen, s->h_n_tokens[rr] + 1, s->h_sum_lp[rr], true});
+                if ((int)cands.size() >= beam) break;
+            }
+        }
+        int best = 0; float best_rank = -INFINITY;
+        for (size_t i = 0; i < cands.size(); ++i) {
+            const float rk = cands[i].score / (float)std::max(cands[i].len - P - 1, 1);
+            if (i == 0 || rk > best_rank) { best = (int)i; best_rank = rk; }
+        }
+        const Cand& cd = cands[best];
+        ch = Choice{r0, cd.tok, cd.lp, cd.live ? cd.len - 1 : cd.len};   // live beams carry no EOT yet: finalize_result appends it
+    }
+    // stream stop rule: the history cut after the stopping token (appended at step stop_at - 1), then the usual finalize
+    if (stop_at >= 0) ch.n = stop_at + 1;
+    return ch;
+}
+
+static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
+    wk_model* m = s->m;
+    const wk_batch_opts* bo = a.bo;
+    const bool bound = a.pcm == nullptr;
+    const int64_t n = a.n;
+    const int T = m->cfg.n_audio_ctx;
+    const int poll = bo->progress_every > 0 ? bo->progress_every : 16;
+    CallPlan p;
+    WK_CHECK(plan_call(s, a, p));
+    const int beam = p.beam, best_of = p.best_of, G = p.G;
+    if (beam > 1) WK_CHECK(ensure_beam(s));
+    s->bs.beam = beam; s->bs.max_candidates = p.max_cand; s->bs.group = G;
+    WK_CHECK(upload_plan(s, p));
+    s->align_on = p.any_words;
     s->win_align_lp.clear();   // the log-probs belong to the last align call only
-    if (any_words) WK_CHECK(ensure_align(s, n));
+    if (p.any_words) WK_CHECK(ensure_align(s, n));
 
     // ---- slots
+    const int S = s->max_batch / G;                    // decode slots (windows in flight)
     const int Brun = (int)std::min<int64_t>(S, n);     // slots in use; the step covers Brun * G rows
     s->batch = Brun * G;
     s->bp = round_up(s->batch, 16);
-    const int rows = s->batch;
-    s->slot_window.assign(S, -1);
-    s->slot_try.assign(S, 0);
-    // stream stop rule: per slot, the history entries already checked and the running log-prob sum over them
-    std::vector<int> stop_checked(a.stop ? S : 0, 0);
-    std::vector<float> stop_sum(a.stop ? S : 0, 0.f);
-    std::unique_ptr<Deflater> stop_deflater(a.stop ? new Deflater() : nullptr);   // zlib state only when the rule is on
+    Slots slots(s, p, a, S);
+    Deflater z;   // the compression ratios of the call's windows and of the stream stop rule
     {   // every slot starts free: done = 1 keeps its rows out of the step until a window is admitted
         std::vector<int32_t> ones(s->max_batch, 1);
         WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done, ones.data(), s->max_batch * 4, cudaMemcpyHostToDevice, s->stream));
         WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
     }
-    // temperature of ladder rung i, computed in Float16 like the reference (TranscribeTask.swift:327)
-    auto rung_temperature = [&](const wk_decode_opts& o, int i) -> float {
-        if (i == 0) return o.temperature;
-        const float f16_t = __half2float(__float2half(o.temperature));
-        const float f16_step = __half2float(__float2half(__half2float(__float2half((float)i)) * __half2float(__float2half(o.temperature_increment_on_fallback))));
-        return __half2float(__float2half(f16_t + f16_step));
-    };
-    // the rows a rung decodes with (openai/whisper decode_with_fallback): best_of == 0 - beam search on every row of a beam call, else one
-    // row; best_of >= 1 - beam search at temperature 0 when beam > 1, best_of independent samples at temperature > 0 when best_of > 1,
-    // else one row.  The group's other rows stay ended
-    auto rung_mode = [&](float temperature, int* active) -> int {
-        if (beam > 1 && (best_of == 0 || temperature == 0.f)) { *active = beam; return kRowBeam; }
-        if (best_of > 1 && temperature > 0.f) { *active = best_of; return kRowSample; }
-        *active = 1;
-        return kRowSingle;
-    };
-    int n_adm = 0;
-    auto stage_admission = [&](int slot, int64_t w, int rung) {
-        const wk_decode_opts& o = opts_of(bo, w);
-        const int oi = bo->n_opts == 1 ? 0 : (int)w;
-        const int32_t* p; int np;
-        prompt_of(w, &p, &np);
-        RowParams R;
-        memset(&R, 0, sizeof(R));
-        R.prompt_len = np;
-        // createLogitsFilters (TextDecoder.swift:857-899): SuppressBlank(sampleBegin = prefilledIndex = 0), TimestampRules(sampleBegin = initialPrompt.count)
-        R.sample_begin_ts = o.without_timestamps ? -1 : np;
-        R.sample_begin_blank = o.suppress_blank ? 0 : -1;
-        R.max_steps = std::max(1, std::min(o.sample_length, kKvMaxLen - 1));   // TextDecoder.swift:566
-        R.temperature = rung_temperature(o, rung); R.top_k = o.top_k;
-        R.has_first_thr = o.has_first_token_logprob_threshold; R.first_thr = o.first_token_logprob_threshold;
-        R.seed = o.seed + (uint64_t)rung;
-        R.suppress_off = sup_off[oi]; R.n_suppress = sup_n[oi];
-        // every rung detects again at its own temperature (detectLanguage runs inside decodeWithFallback's loop, TranscribeTask.swift:333-365)
-        R.lead_token = st->start_of_transcript_token;
-        R.lang_pos = -1;
-        R.no_speech_pos = o.compute_no_speech_prob ? sot_index(w) : -1;   // the same step at every rung
-        if (detects(o)) {
-            R.detect = p[0] == st->start_of_transcript_token ? 1 : 2;
-            R.n_lang = (int32_t)lang_list.size();
-            // usePrefillPrompt: the prompt is rebuilt with the detected language - prefillDecoderInputs puts <|xx|> right after the first
-            // SOT (TextDecoder.swift:176-186); a prompt without a language token there only reports the language
-            if (o.use_prefill_prompt) {
-                const int32_t* sot = std::find(p, p + np, st->start_of_transcript_token);
-                const int i = (int)(sot - p) + 1;
-                if (i < np && std::binary_search(lang_sorted.begin(), lang_sorted.end(), p[i])) R.lang_pos = i;
-            }
-        }
-        int active = 1;
-        R.mode = rung_mode(R.temperature, &active);
-        if (n_adm == 0) cudaEventSynchronize(s->ev_stage);   // the previous round's copies out of the pinned staging have landed
-        for (int j = 0; j < active; ++j) {                   // beam search / best-of: `active` identical rows start the window
-            s->h_adm_slots[n_adm] = slot * G + j;
-            memset(s->h_adm_prompts + (size_t)n_adm * kKvMaxLen, 0, kKvMaxLen * 4);
-            memcpy(s->h_adm_prompts + (size_t)n_adm * kKvMaxLen, p, (size_t)np * 4);
-            s->h_adm_rp[n_adm] = R;
-            ++n_adm;
-        }
-        s->slot_window[slot] = (int)w;
-        s->slot_try[slot] = rung;
-        if (a.stop) { stop_checked[slot] = 0; stop_sum[slot] = 0.f; }
-    };
-    auto prompt_len_of = [&](int64_t w) -> int { const int32_t* p; int np; prompt_of(w, &p, &np); return np; };
-    auto flush_admissions = [&]() -> wk_status {
-        if (n_adm == 0) return WK_OK;
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->d_adm_slots, s->h_adm_slots, (size_t)n_adm * 4, cudaMemcpyHostToDevice, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->d_adm_prompts, s->h_adm_prompts, (size_t)n_adm * kKvMaxLen * 4, cudaMemcpyHostToDevice, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->d_adm_rp, s->h_adm_rp, (size_t)n_adm * sizeof(RowParams), cudaMemcpyHostToDevice, s->stream));
-        if (s->align_on)
-            for (int i = 0; i < n_adm; ++i)   // row 0 and unreached rows of alignmentWeights stay 0
-                WK_CUDA_CHECK(cudaMemsetAsync((char*)s->align_w + (size_t)s->h_adm_slots[i] * kKvMaxLen * T * 2, 0, (size_t)kKvMaxLen * T * 2, s->stream));
-        WK_CHECK(decode_slots_init(s->st, s->rp_dev, s->d_adm_slots, s->d_adm_prompts, s->d_adm_rp, n_adm, s->stream, s->bs));
-        WK_CUDA_CHECK(cudaEventRecord(s->ev_stage, s->stream));
-        n_adm = 0;
-        return WK_OK;
-    };
-
-    // ---- encoder pipeline state
-    const int Ec = bound ? 0 : std::max(1, std::min(bo->encoder_chunk > 0 ? bo->encoder_chunk : c.max_batch, c.max_batch));
-    int64_t enc_next = 0, chunk_w0 = 0, chunk_n = 0, chunk_adm = 0;
-    bool chunk_waited = true;
-    float acc[6] = {0, 0, 0, 0, 0, 0};
-    struct EncTiming { bool pending = false; } et;
-    if (!bound) WK_CHECK(enc_ws_ensure(m, &s->ws, c.max_batch));
-    auto launch_encode = [&]() -> wk_status {
-        const int64_t nc = std::min<int64_t>(Ec, n - enc_next);
-        std::vector<int32_t> spw_fixed;
-        const int32_t* spw = a.spw ? a.spw + enc_next : nullptr;
-        if (a.spw) {   // windows that already failed validation are encoded as silence: they never reach a slot
-            bool any_bad = false;
-            for (int64_t i = 0; i < nc; ++i) any_bad |= status[enc_next + i] != WK_OK;
-            if (any_bad) {
-                spw_fixed.assign(a.spw + enc_next, a.spw + enc_next + nc);
-                for (int64_t i = 0; i < nc; ++i) if (status[enc_next + i] != WK_OK) spw_fixed[i] = 0;
-                spw = spw_fixed.data();
-            }
-        }
-        cudaStream_t es = s->enc_stream;
-        WK_CUDA_CHECK(cudaStreamWaitEvent(es, s->ev_adm, 0));   // the previous chunk's cross-KV projections have read enc_out
-        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[0], es));
-        const float* src = a.pcm + enc_next * a.stride;
-        cudaPointerAttributes pat;
-        const bool on_dev = cudaPointerGetAttributes(&pat, src) == cudaSuccess && pat.type == cudaMemoryTypeDevice;
-        cudaGetLastError();
-        if (!on_dev || a.stride < kWindowSamples) {   // stage here so that the copy is timed apart from the mel kernel
-            if (a.stride < kWindowSamples) WK_CUDA_CHECK(cudaMemsetAsync(s->ws.pcm_dev, 0, (size_t)nc * kWindowSamples * 4, es));
-            WK_CUDA_CHECK(cudaMemcpy2DAsync(s->ws.pcm_dev, kWindowSamples * 4, src, a.stride * 4, std::min<int64_t>(a.stride, kWindowSamples) * 4, nc,
-                                            cudaMemcpyDefault, es));
-            src = s->ws.pcm_dev;
-        }
-        const int64_t src_stride = (!on_dev || a.stride < kWindowSamples) ? kWindowSamples : a.stride;
-        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[1], es));
-        WK_CHECK(mel_run(m, &s->ws, src, nc, src_stride, spw, s->ws.mel, es));
-        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[2], es));
-        WK_CHECK(encode_chunk(m, &s->ws, s->ws.mel, (int)nc, s->ws.enc_out, es));
-        WK_CUDA_CHECK(cudaEventRecord(s->ev_t[3], es));
-        WK_CUDA_CHECK(cudaEventRecord(s->ev_enc, es));
-        chunk_w0 = enc_next; chunk_n = nc; chunk_adm = 0; enc_next += nc; chunk_waited = false;
-        et.pending = true;
-        return WK_OK;
-    };
-    auto collect_enc_timing = [&]() {
-        if (!et.pending || cudaEventQuery(s->ev_t[3]) != cudaSuccess) return;
-        float t;
-        cudaEventElapsedTime(&t, s->ev_t[0], s->ev_t[1]); acc[4] += t;
-        cudaEventElapsedTime(&t, s->ev_t[1], s->ev_t[2]); acc[0] += t;
-        cudaEventElapsedTime(&t, s->ev_t[2], s->ev_t[3]); acc[1] += t;
-        et.pending = false;
-    };
-    // cross-attention K/V of windows [w0, w0+cnt) of the encoded chunk into slots [q0, q0+cnt)
-    auto project_cross_kv = [&](int64_t w0, int q0, int cnt) -> wk_status {
-        if (!chunk_waited) { WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, s->ev_enc, 0)); chunk_waited = true; }
-        const char* src = (const char*)s->ws.enc_out + (size_t)(w0 - chunk_w0) * T * d * 2;
-        return gemm_wgmma(cross_kv_gemm(s, src, cnt, q0), m->num_sms, s->stream);
-    };
-
+    const int Ec = bound ? 0 : std::max(1, std::min(bo->encoder_chunk > 0 ? bo->encoder_chunk : m->cfg.max_batch, m->cfg.max_batch));
+    EncoderFeed feed{s, a, p.status, Ec};
+    if (!bound) WK_CHECK(enc_ws_ensure(m, &s->ws, m->cfg.max_batch));
     int64_t finished = 0;
-    for (int64_t w = 0; w < n; ++w) if (status[w] != WK_OK) ++finished;
+    for (int64_t w = 0; w < n; ++w) if (p.status[w] != WK_OK) ++finished;
     memset(s->stats, 0, sizeof(s->stats));
-    int live = 0;
-    bool ckv_timing = false;
     if (bound) {
         // decodeText on the bound rows: window w sits in slot w with its cross K/V already projected
-        for (int64_t w = 0; w < n; ++w)
-            if (status[w] == WK_OK) { stage_admission((int)w, w, 0); ++live; ++s->stats[2]; }
-        WK_CHECK(flush_admissions());
+        for (int64_t w = 0; w < n; ++w) if (p.status[w] == WK_OK) WK_CHECK(slots.admit((int)w, w, 0));
+        WK_CHECK(slots.flush());
     }
     while (finished < n) {
         // (A) next chunk through mel + encoder as soon as the previous chunk has left enc_out
-        if (!bound && chunk_adm == chunk_n && enc_next < n) WK_CHECK(launch_encode());
-        // (B) admit encoded windows into free slots; consecutive windows going to consecutive slots share one projection GEMM
-        if (!bound && chunk_adm < chunk_n) {
-            int run_q0 = -1, run_cnt = 0; int64_t run_w0 = 0;
-            bool first_gemm = true;
-            auto flush_run = [&]() -> wk_status {
-                if (run_cnt == 0) return WK_OK;
-                if (first_gemm && !ckv_timing) {
-                    if (!chunk_waited) { WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, s->ev_enc, 0)); chunk_waited = true; }   // timed region starts once the encoder output exists
-                    WK_CUDA_CHECK(cudaEventRecord(s->ev_t[4], s->stream));
-                }
-                first_gemm = false;
-                wk_status r = project_cross_kv(run_w0, run_q0, run_cnt);
-                run_cnt = 0;
-                return r;
-            };
-            for (int q = 0; q < Brun && chunk_adm < chunk_n; ++q) {
-                if (s->slot_window[q] >= 0) { WK_CHECK(flush_run()); continue; }
-                while (chunk_adm < chunk_n && status[chunk_w0 + chunk_adm] != WK_OK) { WK_CHECK(flush_run()); ++chunk_adm; }
-                if (chunk_adm >= chunk_n) break;
-                const int64_t w = chunk_w0 + chunk_adm;
-                if (run_cnt > 0 && (q != run_q0 + run_cnt || w != run_w0 + run_cnt)) WK_CHECK(flush_run());
-                if (run_cnt == 0) { run_q0 = q; run_w0 = w; }
-                ++run_cnt;
-                stage_admission(q, w, 0);
-                ++live; ++s->stats[2];
-                ++chunk_adm;
-            }
-            WK_CHECK(flush_run());
-            while (chunk_adm < chunk_n && status[chunk_w0 + chunk_adm] != WK_OK) ++chunk_adm;
-            if (!first_gemm && !ckv_timing) { WK_CUDA_CHECK(cudaEventRecord(s->ev_t[5], s->stream)); ckv_timing = true; }
-            if (chunk_adm == chunk_n) WK_CUDA_CHECK(cudaEventRecord(s->ev_adm, s->stream));
-            WK_CHECK(flush_admissions());
-        }
-        if (live == 0) {
-            if (!bound && (chunk_adm < chunk_n || enc_next < n)) continue;
+        if (!bound && feed.adm == feed.n && feed.next < n) WK_CHECK(feed.encode());
+        // (B) admit encoded windows into free slots
+        if (!bound && feed.adm < feed.n) WK_CHECK(feed.admit(slots, Brun));
+        if (slots.live == 0) {
+            if (!bound && (feed.adm < feed.n || feed.next < n)) continue;
             break;
         }
         // (C) a burst of decode steps, then the state comes back in one go
         WK_CUDA_CHECK(cudaEventRecord(s->ev_t[6], s->stream));
-        WK_CHECK(run_steps(s, st, poll, live == Brun));
-        s->stats[0] += poll; s->stats[1] += (int64_t)poll * live;
+        WK_CHECK(run_steps(s, a.st, poll, slots.live == Brun));
+        s->stats[0] += poll; s->stats[1] += (int64_t)poll * slots.live;
         WK_CUDA_CHECK(cudaEventRecord(s->ev_t[7], s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_done, s->st.done, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_tokens, s->st.n_tokens, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_steps, s->st.steps, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_first_low, s->st.first_low, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_error, s->st.error, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_tokens, s->st.tokens, (size_t)rows * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
-        WK_CUDA_CHECK(cudaMemcpyAsync(s->h_logprobs, s->st.logprobs, (size_t)rows * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
-        if (any_detect) {
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_token, s->st.lang_token, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_logprob, s->st.lang_logprob, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        }
-        if (any_nsp) WK_CUDA_CHECK(cudaMemcpyAsync(s->h_no_speech, s->st.no_speech, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-        if (beam > 1) {
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_sum_lp, s->bs.sum_lp, rows * 4, cudaMemcpyDeviceToHost, s->stream));
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_fin, s->bs.n_fin, Brun * 4, cudaMemcpyDeviceToHost, s->stream));
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_len, s->bs.fin_len, (size_t)Brun * kMaxCand * 4, cudaMemcpyDeviceToHost, s->stream));
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_score, s->bs.fin_score, (size_t)Brun * kMaxCand * 4, cudaMemcpyDeviceToHost, s->stream));
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_tokens, s->bs.fin_tokens, (size_t)Brun * kMaxCand * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
-            WK_CUDA_CHECK(cudaMemcpyAsync(s->h_fin_lps, s->bs.fin_lps, (size_t)Brun * kMaxCand * kKvMaxLen * 4, cudaMemcpyDeviceToHost, s->stream));
-        }
-        {
-            cudaError_t e = cudaStreamSynchronize(s->stream);
-            if (e != cudaSuccess) { set_error("decode loop: %s", cudaGetErrorString(e)); return WK_ERR_DECODING_FAILED; }
-        }
-        {
-            float t;
-            cudaEventElapsedTime(&t, s->ev_t[6], s->ev_t[7]); acc[3] += t;
-            if (ckv_timing) { cudaEventElapsedTime(&t, s->ev_t[4], s->ev_t[5]); acc[2] += t; ckv_timing = false; }
-            collect_enc_timing();
-        }
+        WK_CHECK(read_back(s, p));
+        feed.collect(true);
         // (D) retire ended windows; progress callback / early stop for the live ones
         for (int q = 0; q < Brun; ++q) {
-            const int w = s->slot_window[q];
+            const int w = slots.window[q];
             if (w < 0) continue;
             const int r0 = q * G;                     // first decode row of the slot (the only one of a single-row rung)
             const wk_decode_opts& o = opts_of(bo, w);
@@ -858,9 +911,9 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             if (a.stop) {
                 // every history entry since the last check (the history is causal: steps run past the stopping token are only lost time)
                 const int nt = s->h_n_tokens[r0];
-                stop_at = stop_rule_index(*a.stop, *stop_deflater, s->h_tokens + (size_t)r0 * kKvMaxLen, s->h_logprobs + (size_t)r0 * kKvMaxLen,
-                                          stop_checked[q], nt, prompt_len_of(w), &stop_sum[q]);
-                stop_checked[q] = nt;
+                stop_at = stop_rule_index(*a.stop, z, s->h_tokens + (size_t)r0 * kKvMaxLen, s->h_logprobs + (size_t)r0 * kKvMaxLen,
+                                          slots.stop_checked[q], nt, p.win[w].np, &slots.stop_sum[q]);
+                slots.stop_checked[q] = nt;
                 if (stop_at >= 0 && !ended) {
                     const int32_t one = 1;
                     WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done + r0, &one, 4, cudaMemcpyHostToDevice, s->stream));
@@ -882,103 +935,48 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 }
             }
             if (!ended) continue;
-            wk_decode_result r;
-            const int rung = s->slot_try[q];
-            const int32_t* seq_tok = s->h_tokens + (size_t)r0 * kKvMaxLen;
-            const float* seq_lp = s->h_logprobs + (size_t)r0 * kKvMaxLen;
-            int seq_n = s->h_n_tokens[r0];
-            int rc = r0;                              // the row whose result the window returns
-            std::vector<int32_t> btok; std::vector<float> blp;
+            const float temperature = rung_temperature(o, slots.rung[q]);
             int active = 1;
-            const int rmode = rung_mode(rung_temperature(o, rung), &active);
-            if (rmode == kRowSample) {
-                // best-of: MaximumLikelihoodRanker without length penalty over the samples (oracle/best_of_ref.py rank_best_of) - the sum of
-                // the row's recorded log-probs over max(sampled tokens, 1); ties go to the lowest row
-                const int P = prompt_len_of(w);
-                float best_rank = -INFINITY;
-                for (int j = 0; j < best_of; ++j) {
-                    const int rr = r0 + j;
-                    const float* lp = s->h_logprobs + (size_t)rr * kKvMaxLen;
-                    float sum = 0.f;
-                    for (int i = 0; i < s->h_n_tokens[rr]; ++i) sum += lp[i];
-                    const float rk = sum / (float)std::max(s->h_n_tokens[rr] - P, 1);
-                    if (j == 0 || rk > best_rank) { rc = rr; best_rank = rk; }
-                }
-                seq_tok = s->h_tokens + (size_t)rc * kKvMaxLen;
-                seq_lp = s->h_logprobs + (size_t)rc * kKvMaxLen;
-                seq_n = s->h_n_tokens[rc];
-            } else if (rmode == kRowBeam) {
-                // BeamSearchDecoder.finalize + MaximumLikelihoodRanker (oracle/beam_ref.py): the finished list, topped up with the live beams
-                // (best sum first) to `beam` entries; the winner maximises sum_logprob / sampled tokens
-                struct Cand { const int32_t* tok; const float* lp; int len; float score; bool live; };
-                std::vector<Cand> cands;
-                const int nf = std::min(s->h_n_fin[q], kMaxCand);
-                for (int f = 0; f < nf; ++f) {
-                    const size_t slot = (size_t)q * kMaxCand + f;
-                    cands.push_back(Cand{s->h_fin_tokens + slot * kKvMaxLen, s->h_fin_lps + slot * kKvMaxLen, s->h_fin_len[slot], s->h_fin_score[slot], false});
-                }
-                if ((int)cands.size() < beam) {
-                    std::vector<int> order(beam);
-                    for (int j = 0; j < beam; ++j) order[j] = j;
-                    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return s->h_sum_lp[r0 + x] > s->h_sum_lp[r0 + y]; });
-                    for (int j : order) {
-                        const int rr = r0 + j;
-                        cands.push_back(Cand{s->h_tokens + (size_t)rr * kKvMaxLen, s->h_logprobs + (size_t)rr * kKvMaxLen, s->h_n_tokens[rr] + 1, s->h_sum_lp[rr], true});
-                        if ((int)cands.size() >= beam) break;
-                    }
-                }
-                const int P = prompt_len_of(w);
-                int best = 0; float best_rank = -INFINITY;
-                for (size_t i = 0; i < cands.size(); ++i) {
-                    const float rk = cands[i].score / (float)std::max(cands[i].len - P - 1, 1);
-                    if (i == 0 || rk > best_rank) { best = (int)i; best_rank = rk; }
-                }
-                const Cand& cd = cands[best];
-                const int body = cd.live ? cd.len - 1 : cd.len;      // live beams carry no EOT yet: finalize_result appends it
-                btok.assign(cd.tok, cd.tok + body); blp.assign(cd.lp, cd.lp + body);
-                seq_tok = btok.data(); seq_lp = blp.data(); seq_n = body;
-            }
-            // stream stop rule: the history cut after the stopping token (appended at step stop_at - 1), then the usual finalize
-            if (stop_at >= 0) seq_n = stop_at + 1;
+            const Choice ch = select_result(s, q, G, rung_mode(beam, best_of, temperature, &active), beam, best_of, p.win[w].np, stop_at);
             // beam search: every beam of the window is the same forced copy through the prefill, so row r0 holds the value
             const float nsp = o.compute_no_speech_prob ? s->h_no_speech[r0] : NAN;
-            finalize_result(r, seq_tok, seq_lp, seq_n, stop_at >= 0 ? stop_at : s->h_steps[rc], s->h_first_low[rc], st, &o, rung_temperature(o, rung),
-                            isnan(nsp) ? 0.f : nsp);
+            wk_decode_result r;
+            finalize_result(r, ch.tok, ch.lp, ch.n, stop_at >= 0 ? stop_at : s->h_steps[ch.row], s->h_first_low[ch.row], a.st, &o, temperature,
+                            isnan(nsp) ? 0.f : nsp, z);
             int err_row = -1;                         // a row of the rung without a finite logit fails the window
             for (int j = 0; j < active && err_row < 0; ++j) if (s->h_error[r0 + j]) err_row = r0 + j;
             if (err_row >= 0) {
                 set_error("window %d: no finite logit at decoder step %d", w, s->h_steps[err_row] - 1);
-                fail_window(w, WK_ERR_DECODING_LOGITS_FAILED);
-            } else if (a.ladder && (beam == 1 || best_of >= 1) && !stopped && r.needs_fallback && s->slot_try[q] < o.temperature_fallback_count) {
+                p.fail(w, WK_ERR_DECODING_LOGITS_FAILED, a.results);
+            } else if (a.ladder && (beam == 1 || best_of >= 1) && !stopped && r.needs_fallback && slots.rung[q] < o.temperature_fallback_count) {
                 // decodeWithFallback (TranscribeTask.swift:316-411): same encoder output (the slot keeps its cross K/V), next temperature
-                stage_admission(q, w, s->slot_try[q] + 1);
-                ++s->stats[3];
+                WK_CHECK(slots.admit(q, w, slots.rung[q] + 1));
                 continue;
             } else {
                 a.results[w] = r;
-                if (any_detect) { s->win_lang[w] = s->h_lang_token[r0]; s->win_lang_logprob[w] = s->h_lang_logprob[r0]; }   // the returned rung's
+                if (p.any_detect) { s->win_lang[w] = s->h_lang_token[r0]; s->win_lang_logprob[w] = s->h_lang_logprob[r0]; }   // the returned rung's
                 s->win_no_speech[w] = nsp;
             }
-            if (s->align_on && status[w] == WK_OK && stop_at >= 0)   // rows of the steps run past the stopping token: the reference never ran them
-                WK_CUDA_CHECK(cudaMemsetAsync((char*)s->align_w + ((size_t)rc * kKvMaxLen + stop_at + 1) * T * 2, 0,
+            if (s->align_on && p.status[w] == WK_OK && stop_at >= 0)   // rows of the steps run past the stopping token: the reference never ran them
+                WK_CUDA_CHECK(cudaMemsetAsync((char*)s->align_w + ((size_t)ch.row * kKvMaxLen + stop_at + 1) * T * 2, 0,
                                               (size_t)(kKvMaxLen - stop_at - 1) * T * 2, s->stream));
-            if (s->align_on && status[w] == WK_OK)
-                WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)rc * kKvMaxLen * T * 2,
+            if (s->align_on && p.status[w] == WK_OK)
+                WK_CUDA_CHECK(cudaMemcpyAsync((char*)s->align_store + (size_t)w * kKvMaxLen * T * 2, (char*)s->align_w + (size_t)ch.row * kKvMaxLen * T * 2,
                                               (size_t)kKvMaxLen * T * 2, cudaMemcpyDeviceToDevice, s->stream));
-            s->slot_window[q] = -1;
-            --live;
+            slots.window[q] = -1;
+            --slots.live;
             ++finished;
         }
-        WK_CHECK(flush_admissions());   // ladder re-admissions
+        WK_CHECK(slots.flush());   // ladder re-admissions
     }
     WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
     if (!bound) {
         WK_CUDA_CHECK(cudaStreamSynchronize(s->enc_stream));
-        collect_enc_timing();
-        memcpy(m->timings, acc, sizeof(acc));
+        feed.collect(false);
+        memcpy(m->timings, feed.acc, sizeof(feed.acc));
     }
     if (!bo->status)
-        for (int64_t w = 0; w < n; ++w) if (status[w] != WK_OK) { set_error("%s", first_err.c_str()); return status[w]; }
+        for (int64_t w = 0; w < n; ++w) if (p.status[w] != WK_OK) { set_error("%s", p.first_err.c_str()); return p.status[w]; }
     return WK_OK;
 }
 
@@ -1129,12 +1127,8 @@ static wk_status align_core(wk_session* s, const wk_special_tokens* st, const fl
         const int cnt = (int)std::min<int64_t>(Wc, n - w0);
         int slot0 = (int)w0;
         if (pcm) {
-            std::vector<int32_t> spw_fixed;
-            if (spw) {   // windows that failed validation are encoded as silence
-                spw_fixed.assign(spw + w0, spw + w0 + cnt);
-                for (int i = 0; i < cnt; ++i) if (status[w0 + i] != WK_OK) spw_fixed[i] = 0;
-            }
-            WK_CHECK(mel_run(m, &s->ws, pcm + w0 * stride, cnt, stride, spw ? spw_fixed.data() : nullptr, s->ws.mel, s->stream));
+            std::vector<int32_t> spw_buf;
+            WK_CHECK(mel_run(m, &s->ws, pcm + w0 * stride, cnt, stride, mask_failed(spw, status, w0, cnt, spw_buf), s->ws.mel, s->stream));
             WK_CHECK(encode_chunk(m, &s->ws, s->ws.mel, cnt, s->ws.enc_out, s->stream));
             WK_CHECK(gemm_wgmma(cross_kv_gemm(s, s->ws.enc_out, cnt, 0), m->num_sms, s->stream));
             slot0 = 0;
@@ -1237,8 +1231,6 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CUDA_CHECK(cudaDeviceSynchronize());  // setup memsets ran on the legacy default stream
     WK_CUDA_CHECK(cudaEventRecord(s->ev_adm, s->stream));
     WK_CUDA_CHECK(cudaEventRecord(s->ev_stage, s->stream));
-    s->slot_window.assign(S, -1);
-    s->slot_try.assign(S, 0);
     *out = s.release();
     return WK_OK;
 }
@@ -1283,7 +1275,7 @@ wk_status wk_session_set_encoder_output(wk_session* s, const wk_tensor* enc) {
 wk_status wk_build_prompt(const wk_model* m, const wk_special_tokens* st, const wk_decode_opts* o, int32_t use_options, int32_t* out, int32_t cap, int32_t* n) {
     if (!m || !st || !out || !n) return WK_ERR_INVALID_ARGUMENT;
     std::vector<int32_t> p;
-    WK_CHECK(build_prompt(m, st, o, use_options, p));
+    build_prompt(m, st, o, use_options, p);
     if ((int)p.size() > cap) { set_error("wk_build_prompt: capacity %d < %zu", cap, p.size()); return WK_ERR_PREPARE_DECODER_INPUTS; }
     memcpy(out, p.data(), p.size() * 4);
     *n = (int)p.size();

@@ -209,6 +209,21 @@ wk_status wk_model_encoder_dtype(const wk_model* m, int32_t* dtype);
  * `block` columns (cols a multiple of block) -> codes [rows][cols], scales [rows][cols / block].  block = 128 is the activation rule,
  * block = cols the weight rule (one scale per row). */
 wk_status wk_fp8_quantize_blocks(const float* x, int64_t rows, int64_t cols, int64_t block, uint8_t* codes, float* scales);
+/* ---- draft decoder for speculative greedy decoding (wk_transcribe_windows_draft) ----
+ * A second, smaller Whisper decoder that reads the model's encoder output (distil-large-v3 for large-v3: its encoder is large-v3's,
+ * copied and frozen).  It only proposes tokens; the model's own decoder checks them, so the output never depends on the draft.  A draft
+ * has its own embedding, positional table, layers, final LayerNorm and cross-attention K/V projections, and the model's d_model, heads,
+ * vocabulary and n_audio_ctx.  Every call below fails with WK_ERR_INVALID_ARGUMENT once a session of the model exists.
+ * wk_model_load_draft: an HF Whisper checkpoint directory (config.json + *.safetensors); only the model.decoder.* tensors (and
+ * proj_out.weight) are read, encoder tensors are ignored; a config whose d_model, heads, vocab_size or max_source_positions differ from
+ * the model's is refused.  wk_model_create_draft allocates a zeroed draft of dec_layers layers (replacing any earlier one), which
+ * wk_model_set_draft_tensor (HF decoder names, as wk_model_set_tensor) and wk_model_init_draft_random (seeded, as wk_model_init_random)
+ * fill.  wk_model_draft_layers: the draft's decoder layers, 0 without one. */
+wk_status wk_model_load_draft(wk_model* m, const char* weights_dir);
+wk_status wk_model_create_draft(wk_model* m, int32_t dec_layers);
+wk_status wk_model_set_draft_tensor(wk_model* m, const char* name, const void* data, int32_t dtype, const int64_t* shape, int32_t ndim);
+wk_status wk_model_init_draft_random(wk_model* m, uint64_t seed, float std);
+wk_status wk_model_draft_layers(const wk_model* m, int32_t* n);
 void wk_model_free(wk_model* m);
 
 /* ---- tensors (opaque device buffers passed mel -> encoder -> decoder without touching the host) ---- */
@@ -309,6 +324,9 @@ wk_status wk_decode_text(wk_session* s, const wk_special_tokens* st, const wk_de
  * live when their burst started (an upper bound of the rows that actually streamed K/V), [2] windows admitted to a slot, [3] ladder
  * re-admissions. */
 wk_status wk_session_stats(const wk_session* s, int64_t* out4);
+/* Speculative decoding counters of the session's last batched call (wk_transcribe_windows_draft, wk_decode_text_draft): [0] rounds in which a window verified
+ * proposals, [1] tokens the draft proposed in them, [2] proposals accepted.  All 0 after a call without a draft. */
+wk_status wk_session_draft_stats(const wk_session* s, int64_t* out3);
 /* Language detected for windows [first, first + n) of the session's last batched call (DecodingResult.language as a token id):
  * tokens[i] = the <|xx|> id from the rung whose result was returned, logprobs[i] = its log-prob (log-softmax over language_tokens at
  * temperature 0); -1 and 0 for a window that did not detect.  Either output may be NULL. */
@@ -364,6 +382,25 @@ wk_status wk_decode_text_ex(wk_session* s, const wk_special_tokens* st, const wk
 wk_status wk_transcribe_windows_ex(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
                                    const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
                                    wk_decode_result* results);
+/* Speculative greedy decoding with the model's draft decoder: wk_transcribe_windows_ex / wk_decode_text_ex with draft_tokens = k
+ * (0 = the plain entries).  The setting is an argument, not a wk_batch_opts field, so that struct keeps its size and layout for callers
+ * built against it.  Each window takes G = k + 1 decode rows, so a session holds max_batch / G windows in flight.  On a
+ * temperature-0 rung, once a window is past its prompt, every step of the loop becomes a round: the draft proposes k tokens, the model's
+ * decoder checks all k + 1 positions in one step, and the longest prefix on which they agree is committed together with the model's own
+ * next token.  The draft only changes how many decoder steps run, never which tokens come out: compared with the plain entry on a session
+ * with as many decode slots, the result of every window decoded at temperature 0 is byte-identical, and so is every window's result
+ * when the call has no more windows than slots.  A draw at temperature > 0 (a hotter ladder rung, a first rung above 0, language
+ * detection on such a rung) uses the Philox subsequence of the window's slot; with more windows than slots, the slot a window is admitted
+ * to depends on when earlier windows retire, which the draft changes, so such a window draws a different, equally valid sample.
+ * Prompts and rungs at temperature > 0 advance one token per round.
+ * One exception: a progress callback that stops a window takes effect at a round boundary, so such a window may carry up to k more
+ * tokens; progress_every counts rounds.  Refused (WK_ERR_INVALID_ARGUMENT): a model without a draft decoder, k outside [1, 7], G above
+ * the session's rows, beam_size > 1, best_of >= 1 and word timestamps. */
+wk_status wk_transcribe_windows_draft(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
+                                      const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
+                                      int32_t draft_tokens, wk_decode_result* results);
+wk_status wk_decode_text_draft(wk_session* s, const wk_special_tokens* st, const wk_batch_opts* bo, int32_t draft_tokens,
+                               wk_decode_result* results);
 
 /* ---- multi-GPU edges (SURVEY section 8e): one process per GPU, windows sharded, weights replicated; NCCL only moves PCM out and
  * results back (grouped ncclSend / ncclRecv over NVLink).  NCCL is resolved at run time from the process; wk_comm_unique_id fails with
@@ -430,6 +467,12 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
                                    const wk_special_tokens* st, const wk_decode_opts* opts, const int32_t* prompt, int32_t n_prompt,
                                    const float* clip_timestamps, int32_t n_clip_timestamps, float window_clip_time, int64_t max_window_seek,
                                    int32_t chunking_vad, const wk_tokenizer_hooks* hooks, int32_t best_of, wk_transcription** out);
+/* The same with speculative decoding (wk_transcribe_windows_draft) for every window of the call (0 = wk_transcribe_streams_ex). */
+wk_status wk_transcribe_streams_draft(wk_model* m, wk_session* s, const float* const* audio, const int64_t* n_samples, int32_t n_streams,
+                                      const wk_special_tokens* st, const wk_decode_opts* opts, const int32_t* prompt, int32_t n_prompt,
+                                      const float* clip_timestamps, int32_t n_clip_timestamps, float window_clip_time, int64_t max_window_seek,
+                                      int32_t chunking_vad, const wk_tokenizer_hooks* hooks, int32_t best_of, int32_t draft_tokens,
+                                      wk_transcription** out);
 int32_t wk_transcription_segment_count(const wk_transcription* t);
 int32_t wk_transcription_window_count(const wk_transcription* t);
 int64_t wk_transcription_token_count(const wk_transcription* t);
@@ -666,6 +709,10 @@ wk_status wk_test_decoder_reduce(wk_model* m, int32_t kind, const float* partial
 wk_status wk_test_self_attention_splitk(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bq, const float* bv, void* kcache,
                                         void* vcache, const int32_t* pos, const int32_t* done, const int32_t* anc, void* out, int32_t B, int32_t H,
                                         int32_t dtype);
+/* The K/V append a draft verification step runs before the self-attention: every row b with done[b] == 0 (done may be NULL) gets the
+ * reduced, rounded k / v of its partials at position pos[b] of its own cache row, as wk_test_self_attention_splitk would write it. */
+wk_status wk_test_kv_append(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bv, void* kcache, void* vcache,
+                            const int32_t* pos, const int32_t* done, int32_t B, int32_t H, int32_t dtype);
 /* Decoder cross-attention on q split-K partials [splits][Bp][H*64] with bias bq; K/V [B / kv_div][H][T][64] 16-bit, or E4M3 codes with row
  * scales [B / kv_div][H][T] when kscale / vscale are non-NULL; kv_div = 1 runs the single-query kernel, 2..8 the beam kernel. */
 wk_status wk_test_cross_attention_splitk(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bq, const void* kcross,

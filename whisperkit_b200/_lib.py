@@ -154,6 +154,11 @@ SYMBOLS = [
     ("wk_model_set_encoder_dtype", I32, [P, I32]),
     ("wk_model_encoder_dtype", I32, [P, P]),
     ("wk_fp8_quantize_blocks", I32, [P, I64, I64, I64, P, P]),
+    ("wk_model_load_draft", I32, [P, C.c_char_p]),
+    ("wk_model_create_draft", I32, [P, I32]),
+    ("wk_model_set_draft_tensor", I32, [P, C.c_char_p, P, I32, PI64, I32]),
+    ("wk_model_init_draft_random", I32, [P, C.c_uint64, F32]),
+    ("wk_model_draft_layers", I32, [P, PI32]),
     ("wk_model_free", None, [P]),
     ("wk_tensor_shape", I32, [P, PI64, PI32, PI32]),
     ("wk_tensor_to_host", I32, [P, P, I64]),
@@ -178,11 +183,15 @@ SYMBOLS = [
                              C.POINTER(wk_decode_result)]),
     ("wk_session_last_logits", I32, [P, P]),
     ("wk_session_stats", I32, [P, PI64]),
+    ("wk_session_draft_stats", I32, [P, PI64]),
     ("wk_session_languages", I32, [P, I32, I32, PI32, PF32]),
     ("wk_session_no_speech_probs", I32, [P, I32, I32, PF32]),
     ("wk_decode_text_ex", I32, [P, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts), C.POINTER(wk_decode_result)]),
     ("wk_transcribe_windows_ex", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts),
                                        C.POINTER(wk_decode_result)]),
+    ("wk_transcribe_windows_draft", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts), I32,
+                                          C.POINTER(wk_decode_result)]),
+    ("wk_decode_text_draft", I32, [P, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts), I32, C.POINTER(wk_decode_result)]),
     ("wk_transcribe_windows", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts),
                                     PI32, I32, C.POINTER(wk_decode_result)]),
     ("wk_comm_shard_bounds", None, [I64, I32, I32, PI64, PI64]),
@@ -205,6 +214,8 @@ SYMBOLS = [
                                     PF32, I32, F32, I64, I32, C.POINTER(wk_tokenizer_hooks), C.POINTER(P)]),
     ("wk_transcribe_streams_ex", I32, [P, P, C.POINTER(P), PI64, I32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts), PI32, I32,
                                        PF32, I32, F32, I64, I32, C.POINTER(wk_tokenizer_hooks), I32, C.POINTER(P)]),
+    ("wk_transcribe_streams_draft", I32, [P, P, C.POINTER(P), PI64, I32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts), PI32, I32,
+                                          PF32, I32, F32, I64, I32, C.POINTER(wk_tokenizer_hooks), I32, I32, C.POINTER(P)]),
     ("wk_transcription_segment_count", I32, [P]),
     ("wk_transcription_window_count", I32, [P]),
     ("wk_transcription_token_count", I64, [P]),
@@ -274,6 +285,7 @@ SYMBOLS = [
     ("wk_test_gemm_partial", I32, [P, P, P, P, I32, I32, I32, I32, I32, I32]),
     ("wk_test_decoder_reduce", I32, [P, I32, P, I32, I32, P, P, P, P, P, I32, I32, I32]),
     ("wk_test_self_attention_splitk", I32, [P, P, I32, I32, P, P, P, P, P, P, P, P, I32, I32, I32]),
+    ("wk_test_kv_append", I32, [P, P, I32, I32, P, P, P, P, P, I32, I32, I32]),
     ("wk_test_cross_attention_splitk", I32, [P, P, I32, I32, P, P, P, P, P, P, I32, I32, I32, I32, P, I32]),
     ("wk_debug_read", I32, [P, P, I32, I64, P, I64]),
     ("wk_bench_kernel", I32, [P, P, I32, I32, I32, PF32, C.POINTER(C.c_double)]),

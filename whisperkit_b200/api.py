@@ -120,6 +120,14 @@ class DecodingOptions:
     # bestOf samples (the most likely kept) at temperature > 0, on every rung of the ladder, beam calls included.  One value per call
     # (C: wk_batch_opts.best_of, wk_transcribe_streams_ex)
     bestOf: Optional[int] = None
+    # speculative greedy decoding with the model's draft decoder (Model.loadDraftDecoder / setDraftDecoder): 0 = off; k in 1..7 = the
+    # draft proposes k tokens per round and the model checks them in one step.  Against draftTokens=0 on a session with as many decode
+    # slots (maxBatch / (k + 1)), windows decoded at temperature 0 are byte-identical, and every window is when the call has no more
+    # windows than slots; with more, a temperature > 0 draw follows the slot a window lands in, which the draft's timing changes (C
+    # header, wk_transcribe_windows_draft).  A progress callback that stops
+    # a window takes effect at a round boundary.  One value per call; refused with beamSize > 1, bestOf, wordTimestamps and streams
+    # (C: wk_transcribe_windows_draft, wk_decode_text_draft, wk_transcribe_streams_draft)
+    draftTokens: int = 0
 
     @property
     def detectsLanguage(self) -> bool:
@@ -310,6 +318,9 @@ class Model:
             raise
 
     def set_tensor(self, name: str, t) -> None:
+        self._store(self.lib.wk_model_set_tensor, name, t)
+
+    def _store(self, fn, name: str, t) -> None:
         if hasattr(t, "data_ptr"):
             import torch
             t = t.contiguous()
@@ -320,7 +331,28 @@ class Model:
             dt = {np.dtype("float32"): WK_DTYPE_F32, np.dtype("float16"): WK_DTYPE_F16}[t.dtype]
             shape = list(t.shape)
         shp = (C.c_int64 * len(shape))(*shape)
-        check(self.lib.wk_model_set_tensor(self.handle, name.encode(), _ptr(t), dt, shp, len(shape)))
+        check(fn(self.handle, name.encode(), _ptr(t), dt, shp, len(shape)))
+
+    def loadDraftDecoder(self, weights_dir: str) -> None:
+        """The draft decoder for speculative decoding (DecodingOptions.draftTokens) from an HF Whisper checkpoint directory: its
+        model.decoder.* tensors only (distil-large-v3 for large-v3).  Before the model's first session."""
+        check(self.lib.wk_model_load_draft(self.handle, weights_dir.encode()))
+
+    def setDraftDecoder(self, decLayers: int, weights: Optional[Dict[str, object]] = None, seed: Optional[int] = None,
+                        std: float = 0.02) -> None:
+        """A draft decoder of decLayers layers (the model's dimensions): seeded random weights when seed is given, then `weights` (HF
+        decoder names -> tensors) on top.  Before the model's first session."""
+        check(self.lib.wk_model_create_draft(self.handle, int(decLayers)))
+        if seed is not None:
+            check(self.lib.wk_model_init_draft_random(self.handle, int(seed), float(std)))
+        for k, v in (weights or {}).items():
+            self._store(self.lib.wk_model_set_draft_tensor, k, v)
+
+    @property
+    def draftLayers(self) -> int:
+        n = C.c_int32()
+        check(self.lib.wk_model_draft_layers(self.handle, C.byref(n)))
+        return n.value
 
     def load_state_dict(self, weights: Dict[str, object]) -> None:
         for k, v in weights.items():
@@ -519,7 +551,11 @@ class TextDecoder:
             else with_language_tokens(options, specialTokens, self.logitsSize)
         bo, keep = make_batch_opts(n, opts, prompt, callback, callbackEvery, None)
         res = (wk_decode_result * n)()
-        check(self.lib.wk_decode_text_ex(self.handle, C.byref(st), C.byref(bo), res))
+        draft = draft_tokens_of(opts)
+        if draft:
+            check(self.lib.wk_decode_text_draft(self.handle, C.byref(st), C.byref(bo), draft, res))
+        else:
+            check(self.lib.wk_decode_text_ex(self.handle, C.byref(st), C.byref(bo), res))
         out = [DecodingResult.from_c(r) for r in res]
         attach_languages(out, *session_languages(self.lib, self.handle, n))
         attach_no_speech_probs(out, session_no_speech_probs(self.lib, self.handle, n))
@@ -569,6 +605,13 @@ class TextDecoder:
         a = (C.c_int64 * 4)()
         check(self.lib.wk_session_stats(self.handle, a))
         return dict(zip(("steps", "row_steps", "admissions", "ladder"), [int(v) for v in a]))
+
+    def draftStats(self) -> dict:
+        """Speculative decoding counters of the last batched call (DecodingOptions.draftTokens): rounds that verified proposals, the
+        proposals verified, the proposals accepted."""
+        a = (C.c_int64 * 3)()
+        check(self.lib.wk_session_draft_stats(self.handle, a))
+        return dict(zip(("rounds", "proposed", "accepted"), [int(v) for v in a]))
 
     def lastLogits(self) -> np.ndarray:
         out = np.empty((self.batch, self.logitsSize), dtype=np.float32)
@@ -626,6 +669,15 @@ def with_language_tokens(opts: DecodingOptions, specialTokens: SpecialTokens, vo
     return dataclasses.replace(opts, allLanguageTokens=language_tokens(specialTokens, vocab, tokenizer))
 
 
+def draft_tokens_of(options) -> int:
+    """The call's DecodingOptions.draftTokens: one value for every window (C: the draft_tokens argument of wk_transcribe_windows_draft)."""
+    opt_list = list(options) if isinstance(options, (list, tuple)) else [options]
+    draft = {int(o.draftTokens or 0) for o in opt_list}
+    if len(draft) != 1:
+        raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"draftTokens must be the same for every window of a call (got {sorted(draft)})")
+    return draft.pop()
+
+
 def make_batch_opts(n: int, options, prompt, callback=None, callbackEvery: int = 0, status=None, encoderChunk: int = 0):
     """wk_batch_opts for n windows.  options: DecodingOptions or a list of n; prompt: None (built per window from the options), one token
     list, or a list of n token lists.  Returns (struct, keepalive)."""
@@ -645,6 +697,7 @@ def make_batch_opts(n: int, options, prompt, callback=None, callbackEvery: int =
     if len(best_of) != 1:
         raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"bestOf must be the same for every window of a call (got {sorted(best_of)})")
     bo.best_of = best_of.pop()
+    draft_tokens_of(opt_list)
     if prompt is not None and len(prompt) > 0 and isinstance(prompt[0], (list, tuple, np.ndarray)):
         if len(prompt) != n:
             raise ValueError(f"{len(prompt)} prompts for {n} windows")
@@ -716,6 +769,7 @@ class WhisperKitConfig:
     modelFolder: Optional[str] = None            # HuggingFace checkpoint directory: config.json + *.safetensors (+ tokenizer.json / vocab.json)
     crossKVDtype: Optional[str] = None           # "fp8": E4M3 cross-attention K/V cache (Model); None = dtype
     encoderDtype: Optional[str] = None           # "fp8": encoder QKV / FC1 / FC2 GEMMs on E4M3 operands (Model); None = dtype
+    draftModelFolder: Optional[str] = None       # HF checkpoint whose decoder becomes the draft of DecodingOptions.draftTokens (Model.loadDraftDecoder)
     # audioInputConfig.channelMode: how transcribe(audioPath=...) mixes multi-channel files, ("sum", None | [indices]) or ("channel", i)
     channelMode: tuple = ("sum", None)
 
@@ -742,6 +796,8 @@ class WhisperKit:
                 self.model.load_state_dict(config.weights)
             else:
                 self.model.init_random(config.seed)
+        if config.draftModelFolder is not None:
+            self.model.loadDraftDecoder(config.draftModelFolder)
         self.featureExtractor = FeatureExtractor(self.model)
         self.audioEncoder = AudioEncoder(self.model)
         self.textDecoder = TextDecoder(self.model, config.maxBatch)
@@ -816,8 +872,13 @@ class WhisperKit:
         res = (wk_decode_result * n)()
         # the prompt of every window is built inside the library from that window's options (prefillDecoderInputs); decodeWithFallback
         # (TranscribeTask.swift:316-411) runs there too: a window whose DecodingFallback asks for it is decoded again at the next temperature
-        check(self.model.lib.wk_transcribe_windows_ex(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw, C.byref(st),
-                                                      C.byref(bo), res))
+        draft = draft_tokens_of(opts)
+        if draft:
+            check(self.model.lib.wk_transcribe_windows_draft(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw, C.byref(st),
+                                                             C.byref(bo), draft, res))
+        else:
+            check(self.model.lib.wk_transcribe_windows_ex(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw, C.byref(st),
+                                                          C.byref(bo), res))
         self.textDecoder.batch = min(n, self.config.maxBatch)
         out = []
         for i, r in enumerate(res):

@@ -52,7 +52,7 @@ __global__ void decode_slots_init_kernel(DecodeState st, RowParams* __restrict__
         st.logprobs[b * kMaxCtx + t] = 0.f;
         // the call has beam rows, so the self-attention reads every row through the cache ancestry: a row that never reorders (single or
         // sample rung) must read its own cache rows.  beam_update_kernel rewrites the entries of beam rows before they are read
-        if (bs.beam > 1) bs.anc[b * kMaxCtx + t] = b;
+        if (bs.use_anc) bs.anc[b * kMaxCtx + t] = b;
     }
     if (threadIdx.x == 0) {
         rp_dev[b] = R;
@@ -427,6 +427,43 @@ wk_status decoder_self_attention(const float* partial, int splits, int Bp, const
     return WK_OK;
 }
 
+// The K/V append of decoder_self_attention_kernel's warp 0 alone (same sums in the same order, same rounding): one warp per (b, h)
+template <typename T>
+__global__ void __launch_bounds__(32)
+decoder_kv_append_kernel(const float* __restrict__ partial, int splits, int Bp, const float* __restrict__ bv, T* __restrict__ kcache,
+                         T* __restrict__ vcache, const int32_t* __restrict__ pos_ptr, const int32_t* __restrict__ done, int H, int max_len) {
+    const int lane = threadIdx.x, bh = blockIdx.x, b = bh / H, h = bh % H;
+    pdl_launch_dependents();
+    pdl_wait();
+    if (done != nullptr && done[b]) return;
+    const int dm = H * 64, e = 2 * lane;
+    const long long own = (long long)bh * max_len + pos_ptr[b];
+    float2 k = make_float2(0.f, 0.f);
+    float2 v = make_float2(bv[h * 64 + e], bv[h * 64 + e + 1]);
+    for (int s = 0; s < splits; ++s) {
+        const float* pr = partial + ((long long)s * Bp + b) * (3LL * dm) + h * 64 + e;
+        const float2 pk = *reinterpret_cast<const float2*>(pr + dm);
+        const float2 pv = *reinterpret_cast<const float2*>(pr + 2 * dm);
+        k.x += pk.x; k.y += pk.y; v.x += pv.x; v.y += pv.y;
+    }
+    *reinterpret_cast<uint32_t*>(kcache + own * 64 + e) = T16<T>::pack2(k.x, k.y);
+    *reinterpret_cast<uint32_t*>(vcache + own * 64 + e) = T16<T>::pack2(v.x, v.y);
+}
+
+wk_status decoder_kv_append(const float* partial, int splits, int Bp, const float* bv, void* kcache, void* vcache, const int32_t* pos,
+                            const int32_t* done, int B, int H, int max_len, int dtype, cudaStream_t stream) {
+    if (max_len > kMaxCtx) { set_error("decoder_kv_append: max_len %d > %d", max_len, kMaxCtx); return WK_ERR_INVALID_ARGUMENT; }
+    if (dtype == WK_DTYPE_F16)
+        launch_k(decoder_kv_append_kernel<__half>, dim3(B * H), dim3(32), 0, stream, 2, partial, splits, Bp, bv, (__half*)kcache, (__half*)vcache, pos, done, H, max_len);
+    else
+        launch_k(decoder_kv_append_kernel<__nv_bfloat16>, dim3(B * H), dim3(32), 0, stream, 2, partial, splits, Bp, bv, (__nv_bfloat16*)kcache,
+                 (__nv_bfloat16*)vcache, pos, done, H, max_len);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("decoder_kv_append launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
+}
+
 // =====================================================================================================
 // cross attention for one query per (b, h) over T encoder positions.  HBM-streaming kernel: each CTA pulls its
 // contiguous K block then V block through a ring of 16000-byte bulk-copy stages (cp.async.bulk + mbarrier), a dedicated producer warp
@@ -701,11 +738,11 @@ wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* s
 wk_status decoder_cross_attention(const float* partial, int splits, int Bp, const float* bq, const void* kcross,
                                   const void* vcross, void* out, int B, int H, int T, int dtype, cudaStream_t stream,
                                   const int32_t* done, float* align_scratch, uint32_t align_mask, int kv_div, const float* kscale,
-                                  const float* vscale) {
+                                  const float* vscale, bool single_query) {
     const bool fp8 = kscale != nullptr;
     if (kv_div < 1 || B % kv_div != 0) { set_error("decoder_cross_attention: %d rows do not split into groups of %d", B, kv_div); return WK_ERR_INVALID_ARGUMENT; }
     if (!fp8 && T % kCrossRows != 0) { set_error("decoder_cross_attention: n_audio_ctx %d not a multiple of %d", T, kCrossRows); return WK_ERR_INVALID_ARGUMENT; }
-    if (kv_div > 1 && kv_div <= 8 && align_scratch == nullptr)   // beam search: one CTA per (window, head) serves all beams from one K/V pass
+    if (kv_div > 1 && kv_div <= 8 && align_scratch == nullptr && !single_query)   // beam search: one CTA per (window, head) serves all beams from one K/V pass
         return decoder_cross_attention_mq(partial, splits, Bp, bq, kcross, vcross, out, B, H, T, dtype, stream, done, kv_div, kscale, vscale);
     // FP8: the scale vectors are bulk-copied, so T * 4 bytes per (window, head) must keep 16-byte alignment
     if (fp8 && (T % CrossCfg<true>::kRows != 0 || T % 4 != 0)) { set_error("decoder_cross_attention (fp8): n_audio_ctx %d not a multiple of 500", T); return WK_ERR_INVALID_ARGUMENT; }
@@ -872,7 +909,8 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
             // every row of a group draws with the group's first row's subsequence: the group's rows are copies of one window, so its
             // best-of candidates (and beams) share one detected language
             const int g0 = p.beam.group > 1 ? b - b % p.beam.group : b;
-            const ArgMax d = sample_row(srow, 0, V, mx, mx + logf(sm), R.temperature, R.top_k, R.seed, kDetectSubsequence + (unsigned long long)g0, 0ull,
+            const ArgMax d = sample_row(srow, 0, V, mx, mx + logf(sm), R.temperature, R.top_k, R.seed,
+                                        kDetectSubsequence + (unsigned long long)(g0 / max(1, p.rng_div)), 0ull,
                                         scratch, sarg);
             if (tid == 0) {
                 const bool ok = d.i >= 0 && d.i < V;
@@ -1031,8 +1069,8 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         }
         return;
     }
-    // the row's draw: Philox(seed, row, step) at temperature > 0
-    const ArgMax best = sample_row(srow, lo, V, ts_wins ? mts : mall, lse, R.temperature, R.top_k, R.seed, (unsigned long long)b,
+    // the row's draw: Philox(seed, row, step) at temperature > 0 (row: the slot in a draft call, whose windows sample on row 0 only)
+    const ArgMax best = sample_row(srow, lo, V, ts_wins ? mts : mall, lse, R.temperature, R.top_k, R.seed, (unsigned long long)(b / max(1, p.rng_div)),
                                    (unsigned long long)(loop_mode ? st.steps[b] : n_tok), scratch, sarg);
     const float lp_sampled = best.v;
     if (tid == 0) {
@@ -1196,6 +1234,171 @@ wk_status beam_update(DecodeState st, BeamState beam, wk_special_tokens sp, int 
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("beam_update launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
+}
+
+// =====================================================================================================
+// Speculative greedy decoding: the draft rounds' bookkeeping kernels (session.cu enqueue_round).  Row r0 = q * group is the window's
+// committed row; its state after the main step is exactly the sequential decode's, and verify row j (input: proposal j - 1 at position
+// p0 + j, history: row 0's plus proposals 0..j-1) is the sequential step p0 + j whenever proposals 0..j-1 match what the model sampled.
+// =====================================================================================================
+__global__ void draft_round_begin_kernel(DecodeState st, DecodeState ds, RowParams* __restrict__ drp, DraftRound R) {
+    const int q = blockIdx.x, r0 = q * R.group;
+    const bool live = !st.done[r0];
+    const int p0 = st.steps[r0], n = st.n_tokens[r0];
+    const RowParams rp = st.rp[r0];
+    for (int t = threadIdx.x; t < kMaxCtx; t += blockDim.x) ds.tokens[q * kMaxCtx + t] = st.tokens[r0 * kMaxCtx + t];
+    if (threadIdx.x != 0) return;
+    // past the prompt (tokens[p0] is the committed input of position p0), greedy, not in a leading language-detection step
+    R.verify[q] = live && p0 >= rp.prompt_len && rp.temperature == 0.f && rp.mode == kRowSingle && st.lang_state[r0] == 0;
+    R.p0[q] = live ? p0 : -1;
+    R.nprop[q] = 0;
+    R.cur[q] = -1;
+    if (live) R.fed[q] = min(R.fed[q], p0);   // positions past the committed ones held rejected proposals (or a previous window's)
+    ds.done[q] = 1;
+    ds.n_tokens[q] = n;
+    // the draft's filters are the window's; it always feeds its input token (no prompt forcing, no detection) and proposes greedily
+    RowParams d = rp;
+    d.prompt_len = 0; d.temperature = 0.f; d.has_first_thr = 0; d.detect = 0; d.lang_pos = -1; d.n_lang = 0; d.no_speech_pos = -1;
+    d.mode = kRowSingle;
+    drp[q] = d;
+}
+
+wk_status draft_round_begin(DecodeState st, DecodeState ds, RowParams* drp, DraftRound R, cudaStream_t stream) {
+    launch_k(draft_round_begin_kernel, dim3(R.slots), dim3(64), 0, stream, 0, st, ds, drp, R);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("draft_round_begin launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
+}
+
+__device__ __forceinline__ void draft_collect(DecodeState ds, DraftRound R, int q) {
+    const int c = R.cur[q];
+    if (c < 0) return;
+    R.prop[q * 8 + c] = ds.next_token[q];   // the draft sampler's token (EOT when its row had no finite logit)
+    R.nprop[q] = c + 1;
+    R.cur[q] = -1;
+}
+
+__global__ void draft_feed_kernel(DecodeState st, DecodeState ds, DraftRound R, int collect_only) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= R.slots) return;
+    draft_collect(ds, R, q);
+    if (collect_only) return;
+    const bool ended = ds.done[q];              // the previous draft step ended the draft's sequence (EOT, length limit)
+    ds.done[q] = 1;
+    const int p0 = R.p0[q], f = R.fed[q], r0 = q * R.group;
+    if (p0 < 0) return;
+    int tok, n;
+    if (f < p0) {                               // catch up on a committed token (its sample is not a proposal)
+        tok = st.tokens[r0 * kMaxCtx + f];
+        n = st.n_tokens[r0];
+    } else {
+        const int i = f - p0;                   // proposal i: input = the committed token at p0, then the draft's own proposals
+        if (!R.verify[q] || i >= R.k || f >= st.rp[r0].max_steps || i != R.nprop[q] || (i > 0 && ended)) return;
+        tok = i == 0 ? st.tokens[r0 * kMaxCtx + p0] : R.prop[q * 8 + i - 1];
+        n = p0 + 1 + i;
+        R.cur[q] = i;
+    }
+    ds.n_tokens[q] = n;
+    ds.next_token[q] = tok;
+    ds.steps[q] = f;
+    ds.done[q] = 0;
+    R.fed[q] = f + 1;
+}
+
+wk_status draft_feed(DecodeState st, DecodeState ds, DraftRound R, int collect_only, cudaStream_t stream) {
+    launch_k(draft_feed_kernel, dim3((R.slots + 127) / 128), dim3(128), 0, stream, 0, st, ds, R, collect_only);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("draft_feed launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
+}
+
+__global__ void draft_verify_setup_kernel(DecodeState st, RowParams* __restrict__ rp, int32_t* __restrict__ anc, DraftRound R) {
+    const int q = blockIdx.x, r0 = q * R.group, tid = threadIdx.x;
+    __shared__ int s_nv;
+    if (tid == 0) {
+        const int p0 = R.p0[q];
+        int nv = 0;
+        if (p0 >= 0 && R.verify[q]) {
+            // row j runs step p0 + j, which the sequential loop reaches only below max_steps (<= 223: positions stay inside the cache)
+            nv = min(min(R.nprop[q], R.group - 1), st.rp[r0].max_steps - 1 - p0);
+            nv = max(nv, 0);
+        }
+        R.rows[q] = nv;
+        s_nv = nv;
+    }
+    __syncthreads();
+    const int nv = s_nv;
+    if (nv == 0) return;
+    const int p0 = R.p0[q];
+    const int32_t* prop = R.prop + q * 8;
+    for (int i = tid; i < nv * kMaxCtx; i += blockDim.x) {
+        const int j = 1 + i / kMaxCtx, t = i % kMaxCtx, r = r0 + j;
+        if (t <= p0) st.tokens[r * kMaxCtx + t] = st.tokens[r0 * kMaxCtx + t];
+        else if (t <= p0 + j) st.tokens[r * kMaxCtx + t] = prop[t - p0 - 1];
+        if (t < p0) anc[r * kMaxCtx + t] = anc[r0 * kMaxCtx + t];
+        else if (t < p0 + j) anc[r * kMaxCtx + t] = r0 + (t - p0);   // position p0 + i of this step is row i's
+    }
+    if (tid < nv) {
+        const int j = tid + 1, r = r0 + j;
+        rp[r] = st.rp[r0];
+        st.next_token[r] = prop[j - 1];
+        st.steps[r] = p0 + j;
+        st.n_tokens[r] = p0 + 1 + j;
+        st.done[r] = 0;
+        st.error[r] = 0;
+        st.first_low[r] = 0;
+        st.lang_state[r] = 0;
+    }
+}
+
+wk_status draft_verify_setup(DecodeState st, RowParams* rp, int32_t* anc, DraftRound R, cudaStream_t stream) {
+    launch_k(draft_verify_setup_kernel, dim3(R.slots), dim3(256), 0, stream, 0, st, rp, anc, R);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("draft_verify_setup launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+    return WK_OK;
+}
+
+__global__ void draft_accept_kernel(DecodeState st, int32_t* __restrict__ anc, DraftRound R) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= R.slots) return;
+    const int r0 = q * R.group, rows = R.rows[q], p0 = R.p0[q];
+    const int compared = rows > 0 ? min(R.nprop[q], rows + 1) : 0;   // proposal i is checked against the sample of row i
+    int a = 0;
+    for (int i = 0; i < compared; ++i) {
+        // row 0 holds the state after step p0 + i: its sample must be proposal i, which row i + 1 took as its input
+        if (st.next_token[r0] != R.prop[q * 8 + i]) break;
+        ++a;
+        if (st.done[r0] || i + 1 > rows) break;   // the window ended at this token, or step p0 + i + 1 had no row
+        const int j = i + 1, r = r0 + j, at = p0 + 1 + j, n = st.n_tokens[r];
+        if (n > at) {   // row j appended its sample to the history
+            st.tokens[r0 * kMaxCtx + at] = st.tokens[r * kMaxCtx + at];
+            st.logprobs[r0 * kMaxCtx + at] = st.logprobs[r * kMaxCtx + at];
+        }
+        st.n_tokens[r0] = n;
+        st.steps[r0] = st.steps[r];
+        st.next_token[r0] = st.next_token[r];
+        st.done[r0] = st.done[r];
+        st.first_low[r0] = st.first_low[r];
+        st.error[r0] = st.error[r];
+        anc[r0 * kMaxCtx + p0 + j] = r;
+    }
+    for (int j = 1; j < R.group; ++j) st.done[r0 + j] = 1;
+    if (compared > 0) {
+        atomicAdd(&R.counters[0], 1ull);
+        atomicAdd(&R.counters[1], (unsigned long long)compared);
+        atomicAdd(&R.counters[2], (unsigned long long)a);
+    }
+}
+
+wk_status draft_accept(DecodeState st, int32_t* anc, DraftRound R, cudaStream_t stream) {
+    launch_k(draft_accept_kernel, dim3((R.slots + 127) / 128), dim3(128), 0, stream, 0, st, anc, R);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("draft_accept launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
     return WK_OK;
 }
 

@@ -189,6 +189,50 @@ __global__ void conv_w_rearrange_kernel(const float* __restrict__ src, __half* _
 
 struct Dest { void* p; int dtype; size_t numel; int special; };  // special: 1 conv1, 2 conv2
 
+// The decoder's HF parameter names (model.decoder.*, proj_out.weight) into decoder weight set w: the model's own decoder or its draft
+static bool resolve_decoder_name(const wk_model* m, const DecoderWeights& w, const std::string& name, Dest* out) {
+    const int d = m->cfg.d_model, dt = m->cfg.dtype;
+    auto W = [&](void* p, size_t rows_off, size_t n) { *out = {(char*)p + rows_off * (size_t)d * 2, dt, n, 0}; return true; };
+    auto F = [&](float* p, size_t n) { *out = {p, WK_DTYPE_F32, n, 0}; return true; };
+    int i = -1;
+    char rest[128];
+    if (name == "model.decoder.embed_tokens.weight" || name == "proj_out.weight") { *out = {w.emb, dt, (size_t)m->cfg.vocab * d, 0}; return true; }
+    if (name == "model.decoder.embed_positions.weight") return F(w.pos, (size_t)m->cfg.n_text_ctx * d);
+    if (name == "model.decoder.layer_norm.weight") return F(w.ln.g, d);
+    if (name == "model.decoder.layer_norm.bias") return F(w.ln.b, d);
+    if (sscanf(name.c_str(), "model.decoder.layers.%d.%127s", &i, rest) == 2 && i >= 0 && i < w.n_layers) {
+        DecLayer& l = w.layers[i];
+        const std::string r = rest;
+        const size_t dd = (size_t)d * d;
+        if (r == "self_attn.q_proj.weight") return W(l.wqkv, 0, dd);
+        if (r == "self_attn.k_proj.weight") return W(l.wqkv, d, dd);
+        if (r == "self_attn.v_proj.weight") return W(l.wqkv, 2 * (size_t)d, dd);
+        if (r == "self_attn.q_proj.bias") return F(l.bq, d);
+        if (r == "self_attn.v_proj.bias") return F(l.bv, d);
+        if (r == "self_attn.out_proj.weight") return W(l.wo, 0, dd);
+        if (r == "self_attn.out_proj.bias") return F(l.bo, d);
+        if (r == "self_attn_layer_norm.weight") return F(l.ln1.g, d);
+        if (r == "self_attn_layer_norm.bias") return F(l.ln1.b, d);
+        if (r == "encoder_attn.q_proj.weight") return W(l.wcq, 0, dd);
+        if (r == "encoder_attn.q_proj.bias") return F(l.bcq, d);
+        if (r == "encoder_attn.k_proj.weight") return W(w.wckv, (size_t)(2 * i) * d, dd);
+        if (r == "encoder_attn.v_proj.weight") return W(w.wckv, (size_t)(2 * i + 1) * d, dd);
+        if (r == "encoder_attn.v_proj.bias") return F(w.bckv + (size_t)(2 * i + 1) * d, d);
+        if (r == "encoder_attn.out_proj.weight") return W(l.wco, 0, dd);
+        if (r == "encoder_attn.out_proj.bias") return F(l.bco, d);
+        if (r == "encoder_attn_layer_norm.weight") return F(l.lnx.g, d);
+        if (r == "encoder_attn_layer_norm.bias") return F(l.lnx.b, d);
+        if (r == "final_layer_norm.weight") return F(l.ln3.g, d);
+        if (r == "final_layer_norm.bias") return F(l.ln3.b, d);
+        if (r == "fc1.weight") return W(l.w1, 0, 4 * dd);
+        if (r == "fc1.bias") return F(l.b1, 4 * (size_t)d);
+        if (r == "fc2.weight") return W(l.w2, 0, 4 * dd);
+        if (r == "fc2.bias") return F(l.b2, d);
+        return false;
+    }
+    return false;
+}
+
 static bool resolve_name(wk_model* m, const std::string& name, Dest* out) {
     const int d = m->cfg.d_model, dt = m->cfg.dtype;
     auto W = [&](void* p, size_t rows_off, size_t n) { *out = {(char*)p + rows_off * (size_t)d * 2, dt, n, 0}; return true; };
@@ -202,10 +246,7 @@ static bool resolve_name(wk_model* m, const std::string& name, Dest* out) {
     if (name == "model.encoder.embed_positions.weight") return F(m->enc_pos, (size_t)m->cfg.n_audio_ctx * d);
     if (name == "model.encoder.layer_norm.weight") return F(m->enc_ln.g, d);
     if (name == "model.encoder.layer_norm.bias") return F(m->enc_ln.b, d);
-    if (name == "model.decoder.embed_tokens.weight" || name == "proj_out.weight") { *out = {m->emb, dt, (size_t)m->cfg.vocab * d, 0}; return true; }
-    if (name == "model.decoder.embed_positions.weight") return F(m->dec_pos, (size_t)m->cfg.n_text_ctx * d);
-    if (name == "model.decoder.layer_norm.weight") return F(m->dec_ln.g, d);
-    if (name == "model.decoder.layer_norm.bias") return F(m->dec_ln.b, d);
+    if (resolve_decoder_name(m, m->main_decoder(), name, out)) return true;
     if (sscanf(name.c_str(), "model.encoder.layers.%d.%127s", &i, rest) == 2 && i >= 0 && i < (int)m->enc.size()) {
         EncLayer& l = m->enc[i];
         const std::string r = rest;
@@ -222,36 +263,6 @@ static bool resolve_name(wk_model* m, const std::string& name, Dest* out) {
         if (r == "self_attn_layer_norm.bias") return F(l.ln1.b, d);
         if (r == "final_layer_norm.weight") return F(l.ln2.g, d);
         if (r == "final_layer_norm.bias") return F(l.ln2.b, d);
-        if (r == "fc1.weight") return W(l.w1, 0, 4 * dd);
-        if (r == "fc1.bias") return F(l.b1, 4 * (size_t)d);
-        if (r == "fc2.weight") return W(l.w2, 0, 4 * dd);
-        if (r == "fc2.bias") return F(l.b2, d);
-        return false;
-    }
-    if (sscanf(name.c_str(), "model.decoder.layers.%d.%127s", &i, rest) == 2 && i >= 0 && i < (int)m->dec.size()) {
-        DecLayer& l = m->dec[i];
-        const std::string r = rest;
-        const size_t dd = (size_t)d * d;
-        if (r == "self_attn.q_proj.weight") return W(l.wqkv, 0, dd);
-        if (r == "self_attn.k_proj.weight") return W(l.wqkv, d, dd);
-        if (r == "self_attn.v_proj.weight") return W(l.wqkv, 2 * (size_t)d, dd);
-        if (r == "self_attn.q_proj.bias") return F(l.bq, d);
-        if (r == "self_attn.v_proj.bias") return F(l.bv, d);
-        if (r == "self_attn.out_proj.weight") return W(l.wo, 0, dd);
-        if (r == "self_attn.out_proj.bias") return F(l.bo, d);
-        if (r == "self_attn_layer_norm.weight") return F(l.ln1.g, d);
-        if (r == "self_attn_layer_norm.bias") return F(l.ln1.b, d);
-        if (r == "encoder_attn.q_proj.weight") return W(l.wcq, 0, dd);
-        if (r == "encoder_attn.q_proj.bias") return F(l.bcq, d);
-        if (r == "encoder_attn.k_proj.weight") return W(m->wckv, (size_t)(2 * i) * d, dd);
-        if (r == "encoder_attn.v_proj.weight") return W(m->wckv, (size_t)(2 * i + 1) * d, dd);
-        if (r == "encoder_attn.v_proj.bias") return F(m->bckv + (size_t)(2 * i + 1) * d, d);
-        if (r == "encoder_attn.out_proj.weight") return W(l.wco, 0, dd);
-        if (r == "encoder_attn.out_proj.bias") return F(l.bco, d);
-        if (r == "encoder_attn_layer_norm.weight") return F(l.lnx.g, d);
-        if (r == "encoder_attn_layer_norm.bias") return F(l.lnx.b, d);
-        if (r == "final_layer_norm.weight") return F(l.ln3.g, d);
-        if (r == "final_layer_norm.bias") return F(l.ln3.b, d);
         if (r == "fc1.weight") return W(l.w1, 0, 4 * dd);
         if (r == "fc1.bias") return F(l.b1, 4 * (size_t)d);
         if (r == "fc2.weight") return W(l.w2, 0, 4 * dd);
@@ -505,15 +516,8 @@ wk_status wk_model_create(const wk_model_config* cfg, int32_t device, wk_model**
     return WK_OK;
 }
 
-wk_status wk_model_set_tensor(wk_model* m, const char* name, const void* data, int32_t dtype, const int64_t* shape, int32_t ndim) {
-    if (!m || !name || !data) { set_error("wk_model_set_tensor: null argument"); return WK_ERR_INVALID_ARGUMENT; }
-    WK_CUDA_CHECK(cudaSetDevice(m->device));
-    Dest dst;
-    if (!resolve_name(m, name, &dst)) {
-        if (strstr(name, "k_proj.bias")) return WK_OK;  // Whisper has no key bias; tolerate zero tensors
-        set_error("wk_model_set_tensor: unknown parameter '%s'", name);
-        return WK_ERR_INVALID_ARGUMENT;
-    }
+// host tensor `data` (dtype, shape) converted into the weight buffer dst resolved from `name`
+static wk_status store_tensor(wk_model* m, const Dest& dst, const char* name, const void* data, int32_t dtype, const int64_t* shape, int32_t ndim) {
     size_t numel = 1;
     for (int i = 0; i < ndim; ++i) numel *= (size_t)shape[i];
     if (numel != dst.numel) {
@@ -539,6 +543,19 @@ wk_status wk_model_set_tensor(wk_model* m, const char* name, const void* data, i
         st = convert_to_16(tmp, dtype, dst.p, dst.dtype, (int64_t)numel, m->stream);
         cudaStreamSynchronize(m->stream);
     }
+    return st;
+}
+
+wk_status wk_model_set_tensor(wk_model* m, const char* name, const void* data, int32_t dtype, const int64_t* shape, int32_t ndim) {
+    if (!m || !name || !data) { set_error("wk_model_set_tensor: null argument"); return WK_ERR_INVALID_ARGUMENT; }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    Dest dst;
+    if (!resolve_name(m, name, &dst)) {
+        if (strstr(name, "k_proj.bias")) return WK_OK;  // Whisper has no key bias; tolerate zero tensors
+        set_error("wk_model_set_tensor: unknown parameter '%s'", name);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    wk_status st = store_tensor(m, dst, name, data, dtype, shape, ndim);
     int li = -1;
     char rest[128];
     if (st == WK_OK && m->enc_fp8 && sscanf(name, "model.encoder.layers.%d.%127s", &li, rest) == 2) {
@@ -608,7 +625,8 @@ static bool read_file(const std::string& path, std::vector<char>* buf) {
 }
 }  // namespace
 
-static wk_status load_safetensors_file(wk_model* m, const std::string& path, int* n_loaded) {
+// draft: the file's decoder tensors go to the model's draft decoder (wk_model_set_draft_tensor); everything else is skipped
+static wk_status load_safetensors_file(wk_model* m, const std::string& path, int* n_loaded, bool draft = false) {
     FILE* f = fopen(path.c_str(), "rb");
     if (!f) { set_error("cannot open %s", path.c_str()); return WK_ERR_MODELS_UNAVAILABLE; }
     uint64_t hlen = 0;
@@ -643,16 +661,29 @@ static wk_status load_safetensors_file(wk_model* m, const std::string& path, int
         long long off[2] = {0, 0};
         { const char* q = obj.c_str() + obj.find('[', op) + 1; off[0] = atoll(q); while (*q && *q != ',') ++q; if (*q) off[1] = atoll(q + 1); }
         Dest d;
-        if (dt < 0 || !resolve_name(m, name, &d)) continue;   // not a hot-path parameter (or unsupported dtype)
+        if (dt < 0 || !(draft ? resolve_decoder_name(m, m->draft->view(), name, &d) : resolve_name(m, name, &d))) continue;   // not a hot-path parameter (or unsupported dtype)
         const size_t bytes = (size_t)(off[1] - off[0]);
         buf.resize(bytes);
         if (fseek(f, data0 + off[0], SEEK_SET) != 0 || fread(buf.data(), 1, bytes, f) != bytes) { fclose(f); set_error("%s: truncated tensor %s", path.c_str(), name.c_str()); return WK_ERR_MODELS_UNAVAILABLE; }
-        wk_status st = wk_model_set_tensor(m, name.c_str(), buf.data(), dt, shape, nd);
+        wk_status st = draft ? wk_model_set_draft_tensor(m, name.c_str(), buf.data(), dt, shape, nd) : wk_model_set_tensor(m, name.c_str(), buf.data(), dt, shape, nd);
         if (st != WK_OK) { fclose(f); return st; }
         ++*n_loaded;
     }
     fclose(f);
     return WK_OK;
+}
+
+static std::vector<std::string> safetensors_files(const std::string& dir) {
+    std::vector<std::string> files;
+    if (DIR* d = opendir(dir.c_str())) {
+        while (dirent* e = readdir(d)) {
+            const std::string fn = e->d_name;
+            if (fn.size() > 12 && fn.substr(fn.size() - 12) == ".safetensors") files.push_back(dir + "/" + fn);
+        }
+        closedir(d);
+    }
+    std::sort(files.begin(), files.end());
+    return files;
 }
 
 wk_status wk_model_load(const char* weights_dir, int32_t device, int32_t max_batch, int32_t dtype, wk_model** out) {
@@ -678,19 +709,7 @@ wk_status wk_model_load(const char* weights_dir, int32_t device, int32_t max_bat
     WK_CHECK(wk_model_create(&c, device, &m));
     // every *.safetensors in the directory (single file or HF shards)
     int n_loaded = 0;
-    std::vector<std::string> files;
-    {
-        std::string cmd_dir = dir;
-        DIR* d = opendir(dir.c_str());
-        if (d) {
-            while (dirent* e = readdir(d)) {
-                const std::string fn = e->d_name;
-                if (fn.size() > 12 && fn.substr(fn.size() - 12) == ".safetensors") files.push_back(dir + "/" + fn);
-            }
-            closedir(d);
-        }
-    }
-    std::sort(files.begin(), files.end());
+    const std::vector<std::string> files = safetensors_files(dir);
     if (files.empty()) { wk_model_free(m); set_error("wk_model_load: no *.safetensors in %s", weights_dir); return WK_ERR_MODELS_UNAVAILABLE; }
     for (const auto& fp : files) {
         wk_status st = load_safetensors_file(m, fp, &n_loaded);
@@ -731,6 +750,33 @@ wk_status wk_model_finalize(wk_model* m) {
     if (!m) return WK_ERR_INVALID_ARGUMENT;
     WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
     m->finalized = true;
+    return WK_OK;
+}
+
+// seeded synthetic weights of decoder weight set w (the model's decoder or its draft); *k numbers the fills
+static wk_status init_decoder_random(wk_model* m, const DecoderWeights& w, uint64_t* k, float std) {
+    const wk_model_config& c = m->cfg;
+    const int d = c.d_model, dt = c.dtype;
+    cudaStream_t s = m->stream;
+    auto W = [&](void* p, size_t n, int dtype) { return fill_random_16(p, (int64_t)n, ++*k, std, 0.f, dtype, s); };
+    auto F = [&](float* p, size_t n, float mean) { return fill_random_f32(p, (int64_t)n, ++*k, std, mean, s); };
+    auto LN = [&](const LayerNormW& l) { wk_status r = F(l.g, d, 1.f); return r != WK_OK ? r : F(l.b, d, 0.f); };
+    WK_CHECK(W(w.emb, (size_t)c.vocab * d, dt));
+    WK_CHECK(F(w.pos, (size_t)c.n_text_ctx * d, 0.f));
+    for (int i = 0; i < w.n_layers; ++i) {
+        const DecLayer& l = w.layers[i];
+        WK_CHECK(LN(l.ln1)); WK_CHECK(LN(l.lnx)); WK_CHECK(LN(l.ln3));
+        WK_CHECK(W(l.wqkv, (size_t)3 * d * d, dt)); WK_CHECK(F(l.bq, d, 0.f)); WK_CHECK(F(l.bv, d, 0.f));
+        WK_CHECK(W(l.wo, (size_t)d * d, dt)); WK_CHECK(F(l.bo, d, 0.f));
+        WK_CHECK(W(l.wcq, (size_t)d * d, dt)); WK_CHECK(F(l.bcq, d, 0.f));
+        WK_CHECK(W(l.wco, (size_t)d * d, dt)); WK_CHECK(F(l.bco, d, 0.f));
+        WK_CHECK(W(l.w1, (size_t)4 * d * d, dt)); WK_CHECK(F(l.b1, 4 * d, 0.f));
+        WK_CHECK(W(l.w2, (size_t)4 * d * d, dt)); WK_CHECK(F(l.b2, d, 0.f));
+    }
+    WK_CHECK(LN(w.ln));
+    WK_CHECK(W(w.wckv, (size_t)2 * w.n_layers * d * d, dt));
+    WK_CHECK(F(w.bckv, (size_t)2 * w.n_layers * d, 0.f));
+    for (int i = 0; i < w.n_layers; ++i) WK_CUDA_CHECK(cudaMemsetAsync(w.bckv + 2 * (size_t)i * d, 0, d * 4, s));  // no key bias
     return WK_OK;
 }
 
@@ -777,22 +823,7 @@ wk_status wk_model_init_random(wk_model* m, uint64_t seed, float std) {
         WK_CHECK(W(l.w2, (size_t)4 * d * d, dt)); WK_CHECK(F(l.b2, d, 0.f));
     }
     WK_CHECK(LN(m->enc_ln));
-    WK_CHECK(W(m->emb, (size_t)c.vocab * d, dt));
-    WK_CHECK(F(m->dec_pos, (size_t)c.n_text_ctx * d, 0.f));
-    for (size_t i = 0; i < m->dec.size(); ++i) {
-        DecLayer& l = m->dec[i];
-        WK_CHECK(LN(l.ln1)); WK_CHECK(LN(l.lnx)); WK_CHECK(LN(l.ln3));
-        WK_CHECK(W(l.wqkv, (size_t)3 * d * d, dt)); WK_CHECK(F(l.bq, d, 0.f)); WK_CHECK(F(l.bv, d, 0.f));
-        WK_CHECK(W(l.wo, (size_t)d * d, dt)); WK_CHECK(F(l.bo, d, 0.f));
-        WK_CHECK(W(l.wcq, (size_t)d * d, dt)); WK_CHECK(F(l.bcq, d, 0.f));
-        WK_CHECK(W(l.wco, (size_t)d * d, dt)); WK_CHECK(F(l.bco, d, 0.f));
-        WK_CHECK(W(l.w1, (size_t)4 * d * d, dt)); WK_CHECK(F(l.b1, 4 * d, 0.f));
-        WK_CHECK(W(l.w2, (size_t)4 * d * d, dt)); WK_CHECK(F(l.b2, d, 0.f));
-    }
-    WK_CHECK(LN(m->dec_ln));
-    WK_CHECK(W(m->wckv, (size_t)2 * m->dec.size() * d * d, dt));
-    WK_CHECK(F(m->bckv, (size_t)2 * m->dec.size() * d, 0.f));
-    for (size_t i = 0; i < m->dec.size(); ++i) WK_CUDA_CHECK(cudaMemsetAsync(m->bckv + 2 * i * d, 0, d * 4, s));  // no key bias
+    WK_CHECK(init_decoder_random(m, m->main_decoder(), &k, std));
     WK_CUDA_CHECK(cudaStreamSynchronize(s));
     if (m->enc_fp8) WK_CHECK(quantize_enc_weights(m));
     m->finalized = true;
@@ -882,6 +913,116 @@ wk_status wk_cross_kv_quantize_rows(const float* x, int64_t rows, uint8_t* codes
 wk_model::~wk_model() {
     for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
     if (stream) cudaStreamDestroy(stream);
+}
+
+// ---------------------------------------------------------------------------------------------- draft decoder (speculative decoding)
+// Refuses once a session exists: sessions size their draft buffers from the draft decoder they first see.  Called under api_mu.
+static wk_status draft_settable(wk_model* m, const char* fn) {
+    if (m->session_created) { set_error("%s: the draft decoder is fixed once a session exists", fn); return WK_ERR_INVALID_ARGUMENT; }
+    return WK_OK;
+}
+
+wk_status wk_model_create_draft(wk_model* m, int32_t dec_layers) {
+    if (!m) return WK_ERR_INVALID_ARGUMENT;
+    if (dec_layers < 1 || dec_layers > 64) { set_error("wk_model_create_draft: %d decoder layers outside [1, 64]", dec_layers); return WK_ERR_INVALID_ARGUMENT; }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    WK_CHECK(draft_settable(m, "wk_model_create_draft"));
+    const wk_model_config& c = m->cfg;
+    const int d = c.d_model;
+    std::unique_ptr<DraftDecoder> dr(new DraftDecoder());
+    Buffers& b = dr->mem;
+    WK_CHECK(b.alloc16(&dr->emb, (size_t)round_up(c.vocab, 128) * d));   // padded like the model's: the logits GEMM's last TMA tile
+    WK_CHECK(b.dmalloc(&dr->pos, (size_t)c.n_text_ctx * d));
+    dr->dec.resize(dec_layers);
+    for (auto& l : dr->dec) {
+        WK_CHECK(alloc_ln(b, l.ln1, d)); WK_CHECK(alloc_ln(b, l.lnx, d)); WK_CHECK(alloc_ln(b, l.ln3, d));
+        WK_CHECK(b.alloc16(&l.wqkv, (size_t)3 * d * d)); WK_CHECK(b.dmalloc(&l.bq, d)); WK_CHECK(b.dmalloc(&l.bv, d));
+        WK_CHECK(b.alloc16(&l.wo, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bo, d));
+        WK_CHECK(b.alloc16(&l.wcq, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bcq, d));
+        WK_CHECK(b.alloc16(&l.wco, (size_t)d * d)); WK_CHECK(b.dmalloc(&l.bco, d));
+        WK_CHECK(b.alloc16(&l.w1, (size_t)4 * d * d)); WK_CHECK(b.dmalloc(&l.b1, 4 * d));
+        WK_CHECK(b.alloc16(&l.w2, (size_t)4 * d * d)); WK_CHECK(b.dmalloc(&l.b2, d));
+    }
+    WK_CHECK(alloc_ln(b, dr->ln, d));
+    WK_CHECK(b.alloc16(&dr->wckv, (size_t)2 * dec_layers * d * d));
+    WK_CHECK(b.dmalloc(&dr->bckv, (size_t)2 * dec_layers * d));
+    WK_CUDA_CHECK(cudaDeviceSynchronize());   // the zero fills ran on the legacy default stream
+    m->draft = std::move(dr);
+    return WK_OK;
+}
+
+wk_status wk_model_set_draft_tensor(wk_model* m, const char* name, const void* data, int32_t dtype, const int64_t* shape, int32_t ndim) {
+    if (!m || !name || !data) { set_error("wk_model_set_draft_tensor: null argument"); return WK_ERR_INVALID_ARGUMENT; }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    {
+        std::lock_guard<std::mutex> lock(m->api_mu);
+        WK_CHECK(draft_settable(m, "wk_model_set_draft_tensor"));
+    }
+    if (!m->draft) { set_error("wk_model_set_draft_tensor: the model has no draft decoder (wk_model_create_draft)"); return WK_ERR_INVALID_ARGUMENT; }
+    Dest dst;
+    if (!resolve_decoder_name(m, m->draft->view(), name, &dst)) {
+        if (strstr(name, "k_proj.bias")) return WK_OK;
+        set_error("wk_model_set_draft_tensor: unknown draft decoder parameter '%s'", name);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    return store_tensor(m, dst, name, data, dtype, shape, ndim);
+}
+
+wk_status wk_model_init_draft_random(wk_model* m, uint64_t seed, float std) {
+    if (!m) return WK_ERR_INVALID_ARGUMENT;
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    {
+        std::lock_guard<std::mutex> lock(m->api_mu);
+        WK_CHECK(draft_settable(m, "wk_model_init_draft_random"));
+    }
+    if (!m->draft) { set_error("wk_model_init_draft_random: the model has no draft decoder (wk_model_create_draft)"); return WK_ERR_INVALID_ARGUMENT; }
+    uint64_t k = seed * 1000003ull;
+    WK_CHECK(init_decoder_random(m, m->draft->view(), &k, std));
+    WK_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return WK_OK;
+}
+
+wk_status wk_model_load_draft(wk_model* m, const char* weights_dir) {
+    if (!m || !weights_dir) { set_error("wk_model_load_draft: null argument"); return WK_ERR_INVALID_ARGUMENT; }
+    const std::string dir = weights_dir;
+    std::vector<char> cfgbuf;
+    if (!read_file(dir + "/config.json", &cfgbuf)) { set_error("wk_model_load_draft: %s/config.json not found", weights_dir); return WK_ERR_MODELS_UNAVAILABLE; }
+    const std::string cj(cfgbuf.begin(), cfgbuf.end());
+    const wk_model_config& c = m->cfg;
+    long long dm = 0, heads = 0, vocab = 0, layers = 0, ctx = 1500;
+    json_int(cj, "d_model", &dm);
+    if (!json_int(cj, "decoder_attention_heads", &heads)) json_int(cj, "encoder_attention_heads", &heads);
+    json_int(cj, "vocab_size", &vocab);
+    json_int(cj, "decoder_layers", &layers);
+    json_int(cj, "max_source_positions", &ctx);
+    if (dm != c.d_model || heads != c.n_heads || vocab != c.vocab || ctx != c.n_audio_ctx) {
+        set_error("wk_model_load_draft: the draft (d_model %lld, heads %lld, vocab %lld, n_audio_ctx %lld) does not match the model (%d, %d, %d, %d)",
+                  dm, heads, vocab, ctx, c.d_model, c.n_heads, c.vocab, c.n_audio_ctx);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    const std::vector<std::string> files = safetensors_files(dir);
+    if (files.empty()) { set_error("wk_model_load_draft: no *.safetensors in %s", weights_dir); return WK_ERR_MODELS_UNAVAILABLE; }
+    WK_CHECK(wk_model_create_draft(m, (int32_t)layers));
+    int n_loaded = 0;
+    wk_status st = WK_OK;
+    for (const auto& fp : files) if (st == WK_OK) st = load_safetensors_file(m, fp, &n_loaded, true);
+    const int expected = 4 + (int)layers * 24;
+    if (st == WK_OK && n_loaded < expected) {
+        set_error("wk_model_load_draft: only %d of %d expected decoder tensors found in %s", n_loaded, expected, weights_dir);
+        st = WK_ERR_MODELS_UNAVAILABLE;
+    }
+    if (st != WK_OK) {
+        std::lock_guard<std::mutex> lock(m->api_mu);
+        m->draft.reset();   // a half-loaded draft is never used
+    }
+    return st;
+}
+
+wk_status wk_model_draft_layers(const wk_model* m, int32_t* n) {
+    if (!m || !n) return WK_ERR_INVALID_ARGUMENT;
+    *n = m->draft ? (int32_t)m->draft->dec.size() : 0;
+    return WK_OK;
 }
 
 void wk_model_free(wk_model* m) {
@@ -1324,6 +1465,20 @@ wk_status wk_test_self_attention_splitk(wk_model* m, const float* partial, int32
     wk_status r = decoder_self_attention(partial, splits, Bp, bq, bv, kcache, vcache, pos, done, out, B, H, kKvMaxLen, dtype, m->stream, anc);
     cudaError_t e = cudaStreamSynchronize(m->stream);
     if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_self_attention_splitk: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+wk_status wk_test_kv_append(wk_model* m, const float* partial, int32_t splits, int32_t Bp, const float* bv, void* kcache, void* vcache,
+                            const int32_t* pos, const int32_t* done, int32_t B, int32_t H, int32_t dtype) {
+    if (!m || !partial || !bv || !kcache || !vcache || !pos || B < 1 || Bp < B || splits < 1 || H < 1) {
+        set_error("wk_test_kv_append: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    wk_status r = decoder_kv_append(partial, splits, Bp, bv, kcache, vcache, pos, done, B, H, kKvMaxLen, dtype, m->stream);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_kv_append: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
     return r;
 }
 

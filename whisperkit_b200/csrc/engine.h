@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -36,6 +37,26 @@ struct DecLayer {
     void* wco = nullptr; float* bco = nullptr;
     void* w1 = nullptr; float* b1 = nullptr;
     void* w2 = nullptr; float* b2 = nullptr;
+};
+
+// One decoder's weights as the decode step reads them: the model's own decoder, or its draft decoder (speculative decoding)
+struct DecoderWeights {
+    void* emb = nullptr;                 // [V][d], tied output projection
+    float* pos = nullptr;                // [n_text_ctx][d]
+    DecLayer* layers = nullptr; int n_layers = 0;
+    LayerNormW ln;                       // final LayerNorm
+    void* wckv = nullptr; float* bckv = nullptr;   // cross-attention K/V projection [2L*d][d], [2L*d]
+};
+
+// A draft decoder (wk_model_create_draft / wk_model_load_draft): its own embedding, positional table, layers, final LayerNorm and
+// cross-K/V projection, with the main model's d_model, heads, vocabulary and n_audio_ctx.  It reads the main model's encoder output.
+struct DraftDecoder {
+    Buffers mem;
+    void* emb = nullptr; float* pos = nullptr;
+    std::vector<DecLayer> dec;
+    LayerNormW ln;
+    void* wckv = nullptr; float* bckv = nullptr;
+    DecoderWeights view() { return DecoderWeights{emb, pos, dec.data(), (int)dec.size(), ln, wckv, bckv}; }
 };
 
 // Mel + encoder activations for up to max_batch windows.  The model keeps one for the piecewise API (wk_mel / wk_encode, serialised by
@@ -100,6 +121,9 @@ struct wk_model {
     // encoder QKV / FC1 / FC2 GEMMs on E4M3 operands (wk_model_set_encoder_dtype); fixed once a session exists or wk_encode has run
     bool enc_fp8 = false;
     bool encoded = false;
+    // speculative decoding (wk_model_create_draft / wk_model_load_draft): null = the model has no draft decoder; fixed once a session exists
+    std::unique_ptr<wk::DraftDecoder> draft;
+    wk::DecoderWeights main_decoder() { return wk::DecoderWeights{emb, dec_pos, dec.data(), (int)dec.size(), dec_ln, wckv, bckv}; }
 };
 
 namespace wk {

@@ -225,6 +225,7 @@ struct BeamState {
     int32_t* fin_tokens; float* fin_lps;   // [groups][kMaxCand][224] finished sequences (EOT included), per-token log-probs (EOT -> 0)
     int32_t* fin_len; float* fin_score;    // [groups][kMaxCand]
     int32_t* n_fin;                // [groups]
+    int use_anc;                   // the loop's rows read their self K/V through anc (beam search, or draft verification)
 };
 
 struct SamplerParams {
@@ -237,6 +238,8 @@ struct SamplerParams {
     int max_ctx;             // 224
     const int32_t* detect_tokens;   // loop mode: allLanguageTokens of the rows with RowParams.detect (in-loop language detection)
     BeamState beam;         // loop mode: rows with RowParams.mode == kRowBeam only rank candidates; beam_update() does their bookkeeping
+    int rng_div;            // loop mode: decode rows per Philox subsequence (a draft call's G, so that row 0 of slot q draws as row q of a
+                            // draft-less call); 0 or 1 = every row its own
     // stateless mode only
     int sample_begin_ts, sample_begin_blank, n_suppress;
     float temperature; int top_k; uint64_t seed;
@@ -257,6 +260,12 @@ wk_status decoder_reduce_bias_gelu(const float* partial, int splits, int Bp, con
 wk_status decoder_self_attention(const float* partial, int splits, int Bp, const float* bq, const float* bv, void* kcache,
                                  void* vcache, const int32_t* pos, const int32_t* done, void* out, int B, int H,
                                  int max_len, int dtype, cudaStream_t stream, const int32_t* anc = nullptr);
+// the K/V half of decoder_self_attention alone: reduces the k / v partials of every live row and appends them at pos[b] of its own cache
+// row, with the same arithmetic and rounding.  Run before decoder_self_attention(anc) when rows of one step read each other's new
+// positions (draft verification: row j attends to rows 0..j-1 of its window at this step); the attention kernel's own append then
+// writes the same bits again
+wk_status decoder_kv_append(const float* partial, int splits, int Bp, const float* bv, void* kcache, void* vcache, const int32_t* pos,
+                            const int32_t* done, int B, int H, int max_len, int dtype, cudaStream_t stream);
 // cross attention over T encoder positions; reduces q partials [S][Bp][d]; K/V [B][H][T][64]
 // align_scratch != nullptr: heads h with bit h of align_mask set also write their softmax row (f32, [slot][B][T], slot = rank of h in
 // the mask) - the alignment heads behind the reference decoder's `alignment_heads_weights` output (TextDecoder.swift:310,414)
@@ -265,9 +274,10 @@ wk_status decoder_self_attention(const float* partial, int splits, int Bp, const
 wk_status decoder_cross_attention(const float* partial, int splits, int Bp, const float* bq, const void* kcross,
                                   const void* vcross, void* out, int B, int H, int T, int dtype, cudaStream_t stream,
                                   const int32_t* done = nullptr, float* align_scratch = nullptr, uint32_t align_mask = 0, int kv_div = 1,
-                                  const float* kscale = nullptr, const float* vscale = nullptr);
+                                  const float* kscale = nullptr, const float* vscale = nullptr, bool single_query = false);
 // kv_div > 1 (beam search): row b reads the K/V block of window b / kv_div; the CTAs of one (window, head) are adjacent in the grid so that
-// their K/V stream is shared through L2
+// their K/V stream is shared through L2.  single_query: never the tensor-core form below (its arithmetic differs): every row computes
+// exactly what it would as the only row of its window
 // tensor-core variant for nq = 2..8 rows per K/V block (cross_attention_mq.cu): one K/V stream per (window, head) serves all nq beams
 wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, void* out, int B, int H,
                                      int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq,
@@ -288,6 +298,33 @@ wk_status decode_slots_init(DecodeState st, RowParams* rp_dev, const int32_t* sl
 // to the finished list, permute token / log-prob histories and cache ancestry to the surviving beams, advance the loop state.  One CTA per
 // group of beam.group rows; groups whose rung is not in beam mode return at once
 wk_status beam_update(DecodeState st, BeamState beam, wk_special_tokens sp, int max_ctx, int groups, cudaStream_t stream);
+
+// ---- speculative greedy decoding (session.cu's draft rounds).  A window holds G = k + 1 decode rows; the draft decoder has one row per
+// window slot with its own DecodeState (history = the window's, plus its proposals).  One round: draft_round_begin; k + 1 times
+// draft_feed + draft forward + draft sampler (a step either catches the draft up on a committed token or makes proposal i); verify_setup;
+// the main step over every row; draft_accept.
+struct DraftRound {
+    int k, group, slots;
+    int32_t* fed;        // [S] the draft's self K/V holds positions 0 .. fed - 1 of the window's committed tokens
+    int32_t* p0;         // [S] the window's committed position (main row 0's steps) at the round start, -1 = no live window
+    int32_t* verify;     // [S] 1: the window verifies proposals this round (past its prompt, live, temperature 0)
+    int32_t* prop;       // [S][8] proposals of the round
+    int32_t* nprop;      // [S] proposals made
+    int32_t* rows;       // [S] verification rows 1..rows set up this round (row j runs step p0 + j)
+    int32_t* cur;        // [S] proposal index the draft step just run makes, -1 = none
+    unsigned long long* counters;   // [3] rounds that verified, proposals verified, proposals accepted
+};
+constexpr int kMaxDraftTokens = 7;
+// main row 0 of every slot -> the round's plan; the draft's history and options from the window's
+wk_status draft_round_begin(DecodeState st, DecodeState ds, RowParams* drp, DraftRound R, cudaStream_t stream);
+// the previous draft step's proposal recorded; the next draft step's token and position (or the draft row idle); collect_only: record only
+wk_status draft_feed(DecodeState st, DecodeState ds, DraftRound R, int collect_only, cudaStream_t stream);
+// rows 1..nv of each verifying window: history = row 0's + proposals 0..j-1, input = proposal j-1 at position p0 + j, ancestry through
+// the rows of this step
+wk_status draft_verify_setup(DecodeState st, RowParams* rp, int32_t* anc, DraftRound R, cudaStream_t stream);
+// proposal i is accepted when it equals the token row 0 holds after taking over rows 1..i (the model's sample at step p0 + i); row 0
+// takes over row i + 1 while the window runs on; rows 1..G-1 end
+wk_status draft_accept(DecodeState st, int32_t* anc, DraftRound R, cudaStream_t stream);
 
 // ---- teacher-forced alignment pass (align_pass.cu): rows are (window, position) pairs, 224 rows per window, row w * 224 + t = position t.
 // seq_len[w] = the window's token count (0 = skipped); cross K/V of window w sit in cache block slot0 + w ([slot][H][T][64])
@@ -322,8 +359,9 @@ struct StopRule {
 };
 // wk_transcribe_windows_ex with the stop rule applied to every window (stop == nullptr: wk_transcribe_windows_ex).  Single-row windows
 // only (no beam search, no best-of).
+// draft: speculative decoding's proposals per round (wk_transcribe_windows_draft), 0 = none
 wk_status transcribe_windows_stop(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
                                   const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
-                                  wk_decode_result* results, const StopRule* stop);
+                                  wk_decode_result* results, const StopRule* stop, int draft = 0);
 
 }  // namespace wk

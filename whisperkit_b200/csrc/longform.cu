@@ -284,6 +284,14 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
                                    const wk_special_tokens* st, const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt,
                                    const float* cts, int32_t n_cts, float window_clip_time, int64_t max_window_seek, int32_t chunking_vad,
                                    const wk_tokenizer_hooks* hooks, int32_t best_of, wk_transcription** out) {
+    return wk_transcribe_streams_draft(m, s, audio, n_samples, n_streams, st, o, prompt, n_prompt, cts, n_cts, window_clip_time, max_window_seek,
+                                       chunking_vad, hooks, best_of, 0, out);
+}
+
+wk_status wk_transcribe_streams_draft(wk_model* m, wk_session* s, const float* const* audio, const int64_t* n_samples, int32_t n_streams,
+                                      const wk_special_tokens* st, const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt,
+                                      const float* cts, int32_t n_cts, float window_clip_time, int64_t max_window_seek, int32_t chunking_vad,
+                                      const wk_tokenizer_hooks* hooks, int32_t best_of, int32_t draft_tokens, wk_transcription** out) {
     if (!m || !s || !audio || !n_samples || n_streams < 1 || !st || !o || !prompt || !out) { set_error("wk_transcribe_streams: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (o->word_timestamps && (!hooks || !hooks->split_to_word_tokens)) { set_error("wk_transcribe_streams: wordTimestamps needs the tokenizer's split_to_word_tokens hook"); return WK_ERR_INVALID_ARGUMENT; }
     wk_status rc;
@@ -313,14 +321,15 @@ wk_status wk_transcribe_streams_ex(wk_model* m, wk_session* s, const float* cons
             units.push_back(std::move(u));
         }
     }
-    return seek_loop_units(m, s, units, n_streams, st, o, prompt, n_prompt, window_clip_time, max_window_seek, hooks, best_of, nullptr, true, out);
+    return seek_loop_units(m, s, units, n_streams, st, o, prompt, n_prompt, window_clip_time, max_window_seek, hooks, best_of, draft_tokens, nullptr, true, out);
 }
 
 }  // extern "C"
 
 wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& units, int n_streams, const wk_special_tokens* st,
                               const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt, float window_clip_time, int64_t max_window_seek,
-                              const wk_tokenizer_hooks* hooks, int32_t best_of, const StopRule* stop, bool renumber_ids, wk_transcription** out) {
+                              const wk_tokenizer_hooks* hooks, int32_t best_of, int32_t draft_tokens, const StopRule* stop, bool renumber_ids,
+                              wk_transcription** out) {
     if (o->word_timestamps && (!hooks || !hooks->split_to_word_tokens)) { set_error("wordTimestamps needs the tokenizer's split_to_word_tokens hook"); return WK_ERR_INVALID_ARGUMENT; }
     wk_model_info info;
     wk_status rc = wk_model_info_get(m, &info);
@@ -372,7 +381,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         wk_batch_opts bo;
         memset(&bo, 0, sizeof(bo));
         bo.opts = o; bo.n_opts = 1; bo.prompt = prompt; bo.n_prompt = n_prompt; bo.best_of = best_of;
-        rc = transcribe_windows_stop(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data(), stop);
+        rc = transcribe_windows_stop(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data(), stop, draft_tokens);
         if (rc != WK_OK) return rc;
         T->windows += (int)active.size();
         if (o->detect_language) {   // TranscriptionResult.language: the stream keeps the language of its last detecting window

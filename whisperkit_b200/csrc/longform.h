@@ -47,6 +47,7 @@ struct Unit {                 // one independently advancing cursor: a stream, o
 // which keeps the gaps the reference leaves where word timing drops a zero-length segment (one unit per stream).
 wk_status seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& units, int n_streams, const wk_special_tokens* st,
                           const wk_decode_opts* o, const int32_t* prompt, int32_t n_prompt, float window_clip_time, int64_t max_window_seek,
-                          const wk_tokenizer_hooks* hooks, int32_t best_of, const StopRule* stop, bool renumber_ids, wk_transcription** out);
+                          const wk_tokenizer_hooks* hooks, int32_t best_of, int32_t draft_tokens, const StopRule* stop, bool renumber_ids,
+                          wk_transcription** out);
 
 }  // namespace wk

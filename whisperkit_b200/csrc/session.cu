@@ -84,6 +84,15 @@ struct wk_session {
     int64_t stats[4] = {0, 0, 0, 0};   // of the last batched call: step launches, sum of live rows over them, admissions, ladder re-admissions
     AudioWs* audio = nullptr;          // wk_audio_load / wk_audio_convert workspace (audio.cu)
     int32_t* pos100 = nullptr;         // wk_bench_kernel's self-attention positions (all 100)
+    // speculative decoding (wk_transcribe_windows_draft), allocated on first use when the model has a draft decoder: the draft's self K/V
+    // (one row per slot) and cross K/V (the session's storage policy), its decode state, and the rounds' device bookkeeping
+    int draft_k = 0;                   // proposals per round of the current call, 0 = no draft
+    bool draft_ready = false;
+    void* dr_self_k = nullptr; void* dr_self_v = nullptr; void* dr_cross_kv = nullptr; float* dr_cross_scale = nullptr;
+    DecodeState dst; RowParams* drp = nullptr;
+    DraftRound dr = DraftRound();
+    int64_t draft_stats[3] = {0, 0, 0};   // of the last batched call: rounds that verified, proposals verified, proposals accepted
+    int graph_draft = 0;
 };
 
 // The cached step graphs bake in the call's shape and the session's buffer pointers: dropped, they are captured again on the next step
@@ -110,89 +119,108 @@ cudaStream_t session_stream(wk_session* s) { return s->stream; }
 int session_device(wk_session* s) { return s->m->device; }
 
 // ---------------------------------------------------------------------------------------------- decoder schedule
-static wk_status dec_gemm(wk_session* s, const void* w, int N, int K, const void* act, int* splits_out) {
+static wk_status dec_gemm(wk_session* s, const void* w, int N, int K, const void* act, int* splits_out, int bp = 0) {
     wk_model* m = s->m;
+    if (bp == 0) bp = s->bp;
     GemmDesc g;
     memset(&g, 0, sizeof(g));
     // swap-AB: A = weights [N, K] (128 output features per tile), B = activations [Bp, K]
     g.a = w; g.a_rows = N; g.a_cols = K; g.a_ld = K; g.a_batches = 1;
-    g.b = act; g.b_rows = s->bp; g.b_ld = K; g.in_dtype = m->cfg.dtype;
-    g.m_rows_per_batch = N; g.n = s->bp; g.k = K; g.taps = 1; g.bn = s->bp;
+    g.b = act; g.b_rows = bp; g.b_ld = K; g.in_dtype = m->cfg.dtype;
+    g.m_rows_per_batch = N; g.n = bp; g.k = K; g.taps = 1; g.bn = bp;
     const int tiles = (N + 127) / 128;
     g.splits = choose_splits(tiles, K / 64, m->num_sms);
-    g.mode = GEMM_OUT_PARTIAL_T; g.out = s->partial; g.ld_out = N; g.out_rows_per_batch = N; g.partial_cols = s->bp;
+    g.mode = GEMM_OUT_PARTIAL_T; g.out = s->partial; g.ld_out = N; g.out_rows_per_batch = N; g.partial_cols = bp;
     g.pdl = 1; g.a_static = 1;
-    if ((size_t)g.splits * s->bp * N > s->partial_elems) { set_error("partial workspace too small"); return WK_ERR_DECODING_FAILED; }
+    if ((size_t)g.splits * bp * N > s->partial_elems) { set_error("partial workspace too small"); return WK_ERR_DECODING_FAILED; }
     *splits_out = g.splits;
     return gemm_wgmma(g, m->num_sms, s->stream);
 }
 
 // Bytes of one cross K/V element, and the projection of `cnt` windows of encoder output `src` ([cnt * T][d]) into slots [q0, q0 + cnt) of
-// the cache in the session's storage policy
+// the cache in the session's storage policy: the model's decoder's cache, or (draft) the draft decoder's
 static size_t ckv_esize(const wk_session* s) { return s->ckv_fp8 ? 1 : 2; }
-static GemmDesc cross_kv_gemm(const wk_session* s, const void* src, int cnt, int q0) {
+// the draft decoder's buffers hold one row per window slot; a draft call has at most max_batch / 2 (G = k + 1 >= 2 rows per window)
+static int draft_slots(const wk_session* s) { return s->max_batch / 2; }
+static GemmDesc cross_kv_gemm(const wk_session* s, const void* src, int cnt, int q0, bool draft = false) {
     const wk_model_config& c = s->m->cfg;
     const int T = c.n_audio_ctx, H = c.n_heads;
-    GemmDesc g = plain_gemm(src, (int64_t)cnt * T, c.d_model, s->m->wckv, 2 * c.dec_layers * c.d_model, c.dtype,
-                            s->ckv_fp8 ? GEMM_OUT_FP8_HEADS : GEMM_OUT_T16_HEADS, (char*)s->cross_kv + (size_t)q0 * H * T * 64 * ckv_esize(s), 0,
-                            s->m->bckv, 0);
-    g.heads_T = T; g.heads_B = s->max_batch; g.heads_H = H; g.heads_dmodel = c.d_model;
-    if (s->ckv_fp8) g.out_scale = s->cross_scale + (size_t)q0 * H * T;
+    const DecoderWeights w = draft ? s->m->draft->view() : s->m->main_decoder();
+    void* cache = draft ? s->dr_cross_kv : s->cross_kv;
+    float* scale = draft ? s->dr_cross_scale : s->cross_scale;
+    GemmDesc g = plain_gemm(src, (int64_t)cnt * T, c.d_model, w.wckv, 2 * w.n_layers * c.d_model, c.dtype,
+                            s->ckv_fp8 ? GEMM_OUT_FP8_HEADS : GEMM_OUT_T16_HEADS, (char*)cache + (size_t)q0 * H * T * 64 * ckv_esize(s), 0,
+                            w.bckv, 0);
+    g.heads_T = T; g.heads_B = draft ? draft_slots(s) : s->max_batch; g.heads_H = H; g.heads_dmodel = c.d_model;
+    if (s->ckv_fp8) g.out_scale = scale + (size_t)q0 * H * T;
     return g;
 }
 
-// one decoder forward for every row of the step.  explicit_pos == nullptr: loop mode (token / position from DecodeState, ended rows skipped)
-static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* explicit_pos, bool check_done = true) {
+// One decoder forward: which decoder (the model's or its draft), its caches (every layer strided by the session's max_batch rows or slots),
+// the decode state and the rows.  kv_div: rows per cross K/V block (window); anc: rows read their self K/V through the cache ancestry;
+// verify: the rows of a window are consecutive positions of one step (draft verification) - every row's K/V is appended before any row
+// attends, and the cross-attention keeps its single-query form so that each row computes what it would alone
+struct DecPass {
+    DecoderWeights w;
+    int cap;                       // rows (or window slots) the caches hold per layer
+    void* self_k; void* self_v; void* cross_kv; float* cross_scale;
+    DecodeState st;
+    int B, Bp, kv_div;
+    const int32_t* anc;
+    bool verify, align;
+};
+
+// explicit_pos == nullptr: loop mode (token / position from the pass's DecodeState, ended rows skipped)
+static wk_status decoder_pass(wk_session* s, const DecPass& P, int ts_begin, const int32_t* explicit_pos, bool check_done) {
     wk_model* m = s->m;
     const wk_model_config& c = m->cfg;
-    const int d = c.d_model, H = c.n_heads, dt = c.dtype, B = s->batch, Bp = s->bp, T = c.n_audio_ctx;
+    const int d = c.d_model, H = c.n_heads, dt = c.dtype, B = P.B, Bp = P.Bp, T = c.n_audio_ctx;
     cudaStream_t st = s->stream;
-    const size_t self_layer = (size_t)s->max_batch * H * kKvMaxLen * 64 * 2;   // bytes per layer
-    const size_t cross_rows = (size_t)s->max_batch * H * T;                    // rows of 64 per (layer, k|v)
+    const size_t self_layer = (size_t)P.cap * H * kKvMaxLen * 64 * 2;   // bytes per layer
+    const size_t cross_rows = (size_t)P.cap * H * T;                    // rows of 64 per (layer, k|v)
     const size_t cross_block = cross_rows * 64 * ckv_esize(s);                 // bytes per (layer, k|v)
-    const int32_t* pos = explicit_pos ? explicit_pos : s->st.steps;
+    const int32_t* pos = explicit_pos ? explicit_pos : P.st.steps;
     // ended rows are skipped by the attention kernels; a burst that starts with every slot live runs the variant without the checks (a
     // row that ends inside it just keeps computing until the next poll, as harmlessly as before it ended)
-    const int32_t* done = (explicit_pos || !check_done) ? nullptr : s->st.done;
-    // loop mode: the window's G rows share one cross K/V block; a call with beam rows reads the self K/V through the cache ancestry
-    const bool beam_rows = !explicit_pos && s->bs.beam > 1;
-    const int kv_div = explicit_pos ? 1 : std::max(1, s->bs.group);
-    const int n_layers = c.dec_layers;
+    const int32_t* done = (explicit_pos || !check_done) ? nullptr : P.st.done;
+    const int n_layers = P.w.n_layers;
     int sp = 1;
-    WK_CHECK(decoder_embed_ln(m->emb, m->dec_pos, m->dec[0].ln1.g, m->dec[0].ln1.b, s->st, c.vocab, ts_begin, s->x, s->xn, B, d, dt, explicit_pos, st));
+    WK_CHECK(decoder_embed_ln(P.w.emb, P.w.pos, P.w.layers[0].ln1.g, P.w.layers[0].ln1.b, P.st, c.vocab, ts_begin, s->x, s->xn, B, d, dt, explicit_pos, st));
     auto self_attn = [&](int li, const DecLayer& l) {
-        return decoder_self_attention(s->partial, sp, Bp, l.bq, l.bv, (char*)s->self_k + li * self_layer, (char*)s->self_v + li * self_layer, pos, done,
-                                      s->attn, B, H, kKvMaxLen, dt, st, beam_rows ? s->bs.anc : nullptr);
+        char* kc = (char*)P.self_k + li * self_layer;
+        char* vc = (char*)P.self_v + li * self_layer;
+        if (P.verify) WK_CHECK(decoder_kv_append(s->partial, sp, Bp, l.bv, kc, vc, pos, done, B, H, kKvMaxLen, dt, st));
+        return decoder_self_attention(s->partial, sp, Bp, l.bq, l.bv, kc, vc, pos, done, s->attn, B, H, kKvMaxLen, dt, st, P.anc);
     };
     auto cross_attn = [&](int li, const DecLayer& l) {
-        const bool align = s->align_on && !explicit_pos && m->align_mask[li] != 0;
-        return decoder_cross_attention(s->partial, sp, Bp, l.bcq, (char*)s->cross_kv + (size_t)(2 * li) * cross_block,
-                                       (char*)s->cross_kv + (size_t)(2 * li + 1) * cross_block, s->attn, B, H, T, dt, st, done,
+        const bool align = P.align && m->align_mask[li] != 0;
+        return decoder_cross_attention(s->partial, sp, Bp, l.bcq, (char*)P.cross_kv + (size_t)(2 * li) * cross_block,
+                                       (char*)P.cross_kv + (size_t)(2 * li + 1) * cross_block, s->attn, B, H, T, dt, st, done,
                                        align ? s->align_scratch + (size_t)m->align_base[li] * B * T : nullptr, align ? m->align_mask[li] : 0u,
-                                       kv_div, s->ckv_fp8 ? s->cross_scale + (2 * li) * cross_rows : nullptr,
-                                       s->ckv_fp8 ? s->cross_scale + (2 * li + 1) * cross_rows : nullptr);
+                                       P.kv_div, s->ckv_fp8 ? P.cross_scale + (2 * li) * cross_rows : nullptr,
+                                       s->ckv_fp8 ? P.cross_scale + (2 * li + 1) * cross_rows : nullptr, P.verify);
     };
     for (int li = 0; li < n_layers; ++li) {
-        DecLayer& l = m->dec[li];
-        WK_CHECK(dec_gemm(s, l.wqkv, 3 * d, d, s->xn, &sp));
+        const DecLayer& l = P.w.layers[li];
+        WK_CHECK(dec_gemm(s, l.wqkv, 3 * d, d, s->xn, &sp, Bp));
         WK_CHECK(self_attn(li, l));
-        WK_CHECK(dec_gemm(s, l.wo, d, d, s->attn, &sp));
+        WK_CHECK(dec_gemm(s, l.wo, d, d, s->attn, &sp, Bp));
         WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.bo, l.lnx.g, l.lnx.b, s->x, s->xn, B, d, dt, st));
-        WK_CHECK(dec_gemm(s, l.wcq, d, d, s->xn, &sp));
+        WK_CHECK(dec_gemm(s, l.wcq, d, d, s->xn, &sp, Bp));
         WK_CHECK(cross_attn(li, l));
-        WK_CHECK(dec_gemm(s, l.wco, d, d, s->attn, &sp));
+        WK_CHECK(dec_gemm(s, l.wco, d, d, s->attn, &sp, Bp));
         WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.bco, l.ln3.g, l.ln3.b, s->x, s->xn, B, d, dt, st));
-        WK_CHECK(dec_gemm(s, l.w1, 4 * d, d, s->xn, &sp));
+        WK_CHECK(dec_gemm(s, l.w1, 4 * d, d, s->xn, &sp, Bp));
         WK_CHECK(decoder_reduce_bias_gelu(s->partial, sp, Bp, l.b1, s->ffn, B, 4 * d, dt, st));
-        WK_CHECK(dec_gemm(s, l.w2, d, 4 * d, s->ffn, &sp));
-        const LayerNormW& nxt = (li + 1 < n_layers) ? m->dec[li + 1].ln1 : m->dec_ln;
+        WK_CHECK(dec_gemm(s, l.w2, d, 4 * d, s->ffn, &sp, Bp));
+        const LayerNormW& nxt = (li + 1 < n_layers) ? P.w.layers[li + 1].ln1 : P.w.ln;
         WK_CHECK(decoder_reduce_resid_ln(s->partial, sp, Bp, l.b2, nxt.g, nxt.b, s->x, s->xn, B, d, dt, st));
     }
     // logits = xn . E^T  (tied embedding), written [B][V] f32 by the transposed-store epilogue (splits = 1)
     {
         GemmDesc g;
         memset(&g, 0, sizeof(g));
-        g.a = m->emb; g.a_rows = c.vocab; g.a_cols = d; g.a_ld = d; g.a_batches = 1;
+        g.a = P.w.emb; g.a_rows = c.vocab; g.a_cols = d; g.a_ld = d; g.a_batches = 1;
         g.b = s->xn; g.b_rows = Bp; g.b_ld = d; g.in_dtype = dt;
         g.m_rows_per_batch = c.vocab; g.n = Bp; g.k = d; g.taps = 1; g.bn = Bp; g.splits = 1;
         g.mode = GEMM_OUT_PARTIAL_T; g.out = s->logits; g.ld_out = c.vocab; g.out_rows_per_batch = c.vocab; g.partial_cols = B;
@@ -200,6 +228,16 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
         WK_CHECK(gemm_wgmma(g, m->num_sms, st));
     }
     return WK_OK;
+}
+
+// one forward of the model's decoder for every row of the step.  explicit_pos == nullptr: loop mode
+static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* explicit_pos, bool check_done = true) {
+    const bool loop = !explicit_pos;
+    // loop mode: the window's G rows share one cross K/V block; beam rows and draft verification rows read the self K/V through the
+    // cache ancestry
+    DecPass P{s->m->main_decoder(), s->max_batch, s->self_k, s->self_v, s->cross_kv, s->cross_scale, s->st, s->batch, s->bp,
+              loop ? std::max(1, s->bs.group) : 1, loop && s->bs.use_anc ? s->bs.anc : nullptr, loop && s->draft_k > 0, loop && s->align_on};
+    return decoder_pass(s, P, ts_begin, explicit_pos, check_done);
 }
 
 static SamplerParams loop_sampler_params(wk_session* s, const wk_special_tokens* st) {
@@ -213,6 +251,7 @@ static SamplerParams loop_sampler_params(wk_session* s, const wk_special_tokens*
     p.max_ctx = kKvMaxLen;
     p.detect_tokens = s->lang_dev;
     p.beam = s->bs;
+    p.rng_div = s->draft_k > 0 ? s->bs.group : 1;
     return p;
 }
 
@@ -324,11 +363,32 @@ static void build_prompt(const wk_model* m, const wk_special_tokens* st, const w
 }
 
 // ---------------------------------------------------------------------------------------------- the step and its graph
+// A draft call's step is a round (kernels.h, DraftRound): k + 1 draft steps over the window slots - each catches the draft up on a
+// committed token or makes a proposal - then the verification rows are set up; the model's step over every row and the acceptance follow
+static wk_status enqueue_draft_steps(wk_session* s, const wk_special_tokens* st) {
+    wk_model* m = s->m;
+    const int slots = s->dr.slots;
+    WK_CHECK(draft_round_begin(s->st, s->dst, s->drp, s->dr, s->stream));
+    DecPass P{m->draft->view(), draft_slots(s), s->dr_self_k, s->dr_self_v, s->dr_cross_kv, s->dr_cross_scale, s->dst, slots, round_up(slots, 16), 1, nullptr, false, false};
+    SamplerParams sp = loop_sampler_params(s, st);
+    sp.beam = BeamState();
+    sp.rng_div = 1;
+    for (int i = 0; i <= s->draft_k; ++i) {
+        WK_CHECK(draft_feed(s->st, s->dst, s->dr, 0, s->stream));
+        WK_CHECK(decoder_pass(s, P, st->time_token_begin, nullptr, true));
+        WK_CHECK(sampler_filter_sample(s->logits, m->cfg.vocab, sp, s->dst, nullptr, 0, nullptr, nullptr, nullptr, nullptr, slots, s->stream));
+    }
+    WK_CHECK(draft_feed(s->st, s->dst, s->dr, 1, s->stream));
+    return draft_verify_setup(s->st, s->rp_dev, s->bs.anc, s->dr, s->stream);
+}
+
 static wk_status enqueue_step(wk_session* s, const wk_special_tokens* st, bool check_done) {
     wk_model* m = s->m;
+    if (s->draft_k > 0) WK_CHECK(enqueue_draft_steps(s, st));
     WK_CHECK(decoder_forward(s, st->time_token_begin, nullptr, check_done));
     WK_CHECK(sampler_filter_sample(s->logits, m->cfg.vocab, loop_sampler_params(s, st), s->st, nullptr, 0, nullptr, nullptr, nullptr, nullptr, s->batch, s->stream));
     if (s->bs.beam > 1) WK_CHECK(beam_update(s->st, s->bs, *st, kKvMaxLen, s->batch / s->bs.group, s->stream));
+    if (s->draft_k > 0) WK_CHECK(draft_accept(s->st, s->bs.anc, s->dr, s->stream));
     if (s->align_on)
         WK_CHECK(decoder_align_mean(s->align_scratch, m->n_align_slots, s->st.steps, s->st.done, s->st.lang_state, s->align_w, s->batch, m->cfg.n_audio_ctx,
                                     kKvMaxLen, s->stream));
@@ -349,10 +409,10 @@ static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bo
     // the step's shape depends on the rows per window (cross K/V sharing) and on whether the call has beam rows (ancestry, beam_update)
     const int beam_key = (std::max(1, s->bs.group) * 16 + std::max(1, s->bs.beam)) * 16 + s->bs.max_candidates;
     const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_beam != beam_key ||
-                       memcmp(&s->graph_st, st, sizeof(*st)) != 0;
+                       s->graph_draft != s->draft_k || memcmp(&s->graph_st, st, sizeof(*st)) != 0;
     if (stale) {
         drop_graphs(s);
-        s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_st = *st; s->graph_beam = beam_key;
+        s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_st = *st; s->graph_beam = beam_key; s->graph_draft = s->draft_k;
     }
     cudaGraphExec_t& exec = check_done ? s->graph_exec : s->graph_exec_live;
     if (!exec) {
@@ -392,6 +452,7 @@ struct CoreArgs {
     const wk_special_tokens* st; const wk_batch_opts* bo; wk_decode_result* results;
     bool ladder;
     const StopRule* stop = nullptr;   // stream stop rule (transcribe_windows_stop); nullptr: windows end on their own or by callback
+    int draft = 0;                    // speculative decoding: proposals per round, 0 = none
 };
 
 static const wk_decode_opts& opts_of(const wk_batch_opts* bo, int64_t w) { return bo->n_opts == 1 ? bo->opts[0] : bo->opts[w]; }
@@ -438,13 +499,48 @@ static wk_status ensure_beam(wk_session* s) {
     return WK_OK;
 }
 
+// the draft decoder's buffers (speculative decoding), for draft_slots(s) windows: self K/V and cross K/V, decode state, the rounds'
+// bookkeeping
+static wk_status ensure_draft(wk_session* s) {
+    if (s->draft_ready) return WK_OK;
+    const wk_model_config& c = s->m->cfg;
+    const int S = draft_slots(s), H = c.n_heads, T = c.n_audio_ctx, Ld = (int)s->m->draft->dec.size();
+    Buffers& b = s->mem;
+    if (s->ckv_fp8) {
+        uint8_t* codes = nullptr;
+        WK_CHECK(b.dmalloc(&codes, (size_t)2 * Ld * S * H * T * 64));
+        s->dr_cross_kv = codes;
+        WK_CHECK(b.dmalloc(&s->dr_cross_scale, (size_t)2 * Ld * S * H * T));
+    } else {
+        WK_CHECK(b.alloc16(&s->dr_cross_kv, (size_t)2 * Ld * S * H * T * 64));
+    }
+    WK_CHECK(b.alloc16(&s->dr_self_k, (size_t)Ld * S * H * kKvMaxLen * 64));
+    WK_CHECK(b.alloc16(&s->dr_self_v, (size_t)Ld * S * H * kKvMaxLen * 64));
+    DecodeState& d = s->dst;
+    WK_CHECK(b.dmalloc(&d.tokens, (size_t)S * kKvMaxLen));
+    WK_CHECK(b.dmalloc(&d.logprobs, (size_t)S * kKvMaxLen));
+    for (int32_t** p : {&d.n_tokens, &d.next_token, &d.done, &d.first_low, &d.steps, &d.input_ids, &d.error, &d.lang_token, &d.lang_state})
+        WK_CHECK(b.dmalloc(p, S));
+    WK_CHECK(b.dmalloc(&d.lang_logprob, S));
+    WK_CHECK(b.dmalloc(&d.no_speech, S));
+    WK_CHECK(b.dmalloc(&s->drp, S));
+    d.rp = s->drp;
+    DraftRound& R = s->dr;
+    for (int32_t** p : {&R.fed, &R.p0, &R.verify, &R.nprop, &R.rows, &R.cur}) WK_CHECK(b.dmalloc(p, S));
+    WK_CHECK(b.dmalloc(&R.prop, (size_t)S * 8));
+    WK_CHECK(b.dmalloc(&R.counters, 3));
+    s->draft_ready = true;
+    return WK_OK;
+}
+
 // One window as the call decodes it: its prompt, the index of the prompt's first <|startoftranscript|> (-1: none) and whether the window
 // detects its language in the loop
 struct WindowPlan { const int32_t* p = nullptr; int np = 0, sot = -1; bool detects = false; };
 
 // What a call decodes, worked out on the host before any CUDA work
 struct CallPlan {
-    int beam = 1, best_of = 0, G = 1, max_cand = 0;   // G = max(beam, best_of): decode rows per window
+    int beam = 1, best_of = 0, G = 1, max_cand = 0;   // G = max(beam, best_of), or draft + 1: decode rows per window
+    int draft = 0;                                    // proposals per round (wk_transcribe_windows_draft), 0 = no draft
     std::vector<WindowPlan> win;
     std::vector<std::vector<int32_t>> built;          // the prompts built from the options, when the call passes none
     std::vector<int32_t> sup_pool;                    // suppress ids of every option set: set i's at [sup_off[i], sup_off[i] + sup_n[i])
@@ -477,9 +573,19 @@ static wk_status plan_call(wk_session* s, const CoreArgs& a, CallPlan& p) {
             set_error("beam size / patience must be the same for every window of a call"); return WK_ERR_INVALID_ARGUMENT;
         }
     if (best_of < 0 || best_of > kMaxBeam) { set_error("best_of %d outside [0, %d]", best_of, kMaxBeam); return WK_ERR_INVALID_ARGUMENT; }
-    const int G = p.G = std::max(beam, std::max(best_of, 1));
+    // speculative decoding: greedy single-row windows only; the window's rows verify the draft's proposals
+    const int draft = p.draft = a.draft;
+    if (draft != 0) {
+        if (draft < 1 || draft > kMaxDraftTokens) { set_error("draft_tokens %d outside [1, %d]", draft, kMaxDraftTokens); return WK_ERR_INVALID_ARGUMENT; }
+        if (!s->m->draft) { set_error("draft_tokens %d: the model has no draft decoder", draft); return WK_ERR_INVALID_ARGUMENT; }
+        if (beam > 1 || best_of != 0) { set_error("draft_tokens does not combine with beam search or best_of"); return WK_ERR_INVALID_ARGUMENT; }
+        if (a.stop) { set_error("draft_tokens is not supported in streams"); return WK_ERR_INVALID_ARGUMENT; }
+        for (int i = 0; i < bo->n_opts; ++i)
+            if (bo->opts[i].word_timestamps) { set_error("draft_tokens does not combine with word timestamps"); return WK_ERR_INVALID_ARGUMENT; }
+    }
+    const int G = p.G = draft > 0 ? draft + 1 : std::max(beam, std::max(best_of, 1));
     if (G > s->max_batch) {
-        set_error("%d rows per window (beam size %d, best_of %d) exceed the session's %d rows", G, beam, best_of, s->max_batch);
+        set_error("%d rows per window (beam size %d, best_of %d, draft_tokens %d) exceed the session's %d rows", G, beam, best_of, draft, s->max_batch);
         return WK_ERR_INVALID_ARGUMENT;
     }
     if (a.stop && (G != 1 || a.stop->window < 1)) { set_error("the stream stop rule needs single-row windows and a check window >= 1"); return WK_ERR_INVALID_ARGUMENT; }
@@ -740,6 +846,8 @@ struct EncoderFeed {
             if (first && !ckv_timing) WK_CUDA_CHECK(cudaEventRecord(s->ev_t[4], s->stream));
             first = false;
             WK_CHECK(gemm_wgmma(cross_kv_gemm(s, (const char*)s->ws.enc_out + run0 * win_bytes, q - q0, q0), s->m->num_sms, s->stream));
+            if (s->draft_k > 0)   // the draft's cross K/V from the same encoder output
+                WK_CHECK(gemm_wgmma(cross_kv_gemm(s, (const char*)s->ws.enc_out + run0 * win_bytes, q - q0, q0, true), s->m->num_sms, s->stream));
         }
         if (!first && !ckv_timing) { WK_CUDA_CHECK(cudaEventRecord(s->ev_t[5], s->stream)); ckv_timing = true; }
         if (adm == n) WK_CUDA_CHECK(cudaEventRecord(s->ev_adm, s->stream));
@@ -853,8 +961,10 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     CallPlan p;
     WK_CHECK(plan_call(s, a, p));
     const int beam = p.beam, best_of = p.best_of, G = p.G;
-    if (beam > 1) WK_CHECK(ensure_beam(s));
-    s->bs.beam = beam; s->bs.max_candidates = p.max_cand; s->bs.group = G;
+    if (beam > 1 || p.draft > 0) WK_CHECK(ensure_beam(s));
+    if (p.draft > 0) WK_CHECK(ensure_draft(s));
+    s->bs.beam = beam; s->bs.max_candidates = p.max_cand; s->bs.group = G; s->bs.use_anc = beam > 1 || p.draft > 0;
+    s->draft_k = p.draft;
     WK_CHECK(upload_plan(s, p));
     s->align_on = p.any_words;
     s->win_align_lp.clear();   // the log-probs belong to the last align call only
@@ -870,8 +980,14 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     {   // every slot starts free: done = 1 keeps its rows out of the step until a window is admitted
         std::vector<int32_t> ones(s->max_batch, 1);
         WK_CUDA_CHECK(cudaMemcpyAsync(s->st.done, ones.data(), s->max_batch * 4, cudaMemcpyHostToDevice, s->stream));
+        if (p.draft > 0) {
+            s->dr.k = p.draft; s->dr.group = G; s->dr.slots = Brun;
+            WK_CUDA_CHECK(cudaMemsetAsync(s->dr.fed, 0, draft_slots(s) * 4, s->stream));
+            WK_CUDA_CHECK(cudaMemsetAsync(s->dr.counters, 0, 3 * sizeof(unsigned long long), s->stream));
+        }
         WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
     }
+    memset(s->draft_stats, 0, sizeof(s->draft_stats));
     const int Ec = bound ? 0 : std::max(1, std::min(bo->encoder_chunk > 0 ? bo->encoder_chunk : m->cfg.max_batch, m->cfg.max_batch));
     EncoderFeed feed{s, a, p.status, Ec};
     if (!bound) WK_CHECK(enc_ws_ensure(m, &s->ws, m->cfg.max_batch));
@@ -894,7 +1010,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         }
         // (C) a burst of decode steps, then the state comes back in one go
         WK_CUDA_CHECK(cudaEventRecord(s->ev_t[6], s->stream));
-        WK_CHECK(run_steps(s, a.st, poll, slots.live == Brun));
+        WK_CHECK(run_steps(s, a.st, poll, slots.live == Brun && p.draft == 0));   // a draft call's rows 1..G-1 end every round
         s->stats[0] += poll; s->stats[1] += (int64_t)poll * slots.live;
         WK_CUDA_CHECK(cudaEventRecord(s->ev_t[7], s->stream));
         WK_CHECK(read_back(s, p));
@@ -968,6 +1084,12 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             ++finished;
         }
         WK_CHECK(slots.flush());   // ladder re-admissions
+    }
+    if (p.draft > 0) {
+        unsigned long long c[3];
+        WK_CUDA_CHECK(cudaMemcpyAsync(c, s->dr.counters, sizeof(c), cudaMemcpyDeviceToHost, s->stream));
+        WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
+        for (int i = 0; i < 3; ++i) s->draft_stats[i] = (int64_t)c[i];
     }
     WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
     if (!bound) {
@@ -1265,6 +1387,12 @@ wk_status wk_session_set_encoder_output(wk_session* s, const wk_tensor* enc) {
     std::lock_guard<std::mutex> lock(m->api_mu);
     for (cudaEvent_t e : enc->events) WK_CUDA_CHECK(cudaStreamWaitEvent(s->stream, e, 0));
     WK_CHECK(gemm_wgmma(cross_kv_gemm(s, enc->data, s->batch, 0), m->num_sms, s->stream));
+    // a model with a draft decoder binds the draft's cross K/V too (wk_decode_text_draft), when the windows fit a draft call: the session
+    // does not keep the encoder output, so binding is the one time it can be projected
+    if (m->draft && s->batch <= draft_slots(s)) {
+        WK_CHECK(ensure_draft(s));
+        WK_CHECK(gemm_wgmma(cross_kv_gemm(s, enc->data, s->batch, 0, true), m->num_sms, s->stream));
+    }
     cudaEvent_t ev;
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventRecord(ev, s->stream));
@@ -1347,11 +1475,15 @@ wk_status wk_detect_language(wk_session* s, const wk_special_tokens* st, const i
 }
 
 wk_status wk_decode_text_ex(wk_session* s, const wk_special_tokens* st, const wk_batch_opts* bo, wk_decode_result* results) {
+    return wk_decode_text_draft(s, st, bo, 0, results);
+}
+
+wk_status wk_decode_text_draft(wk_session* s, const wk_special_tokens* st, const wk_batch_opts* bo, int32_t draft_tokens, wk_decode_result* results) {
     if (!s || !st || !bo || !bo->opts || bo->n_opts < 1 || !results) { set_error("wk_decode_text: null argument"); return WK_ERR_INVALID_ARGUMENT; }
     if (s->bound_windows < 1) { set_error("wk_decode_text: no encoder output bound"); return WK_ERR_PREPARE_DECODER_INPUTS; }
     if (bo->n_opts != 1 && bo->n_opts != s->bound_windows) { set_error("wk_decode_text: %d option sets for %d windows", bo->n_opts, s->bound_windows); return WK_ERR_INVALID_ARGUMENT; }
     WK_CUDA_CHECK(cudaSetDevice(s->m->device));
-    CoreArgs a{nullptr, s->bound_windows, 0, nullptr, st, bo, results, false};
+    CoreArgs a{nullptr, s->bound_windows, 0, nullptr, st, bo, results, false, nullptr, draft_tokens};
     return transcribe_core(s, a);
 }
 
@@ -1370,18 +1502,24 @@ wk_status wk_transcribe_windows_ex(wk_model* m, wk_session* s, const float* pcm_
     return wk::transcribe_windows_stop(m, s, pcm_host, n_windows, stride, samples_per_window, st, bo, results, nullptr);
 }
 
+wk_status wk_transcribe_windows_draft(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
+                                      const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
+                                      int32_t draft_tokens, wk_decode_result* results) {
+    return wk::transcribe_windows_stop(m, s, pcm_host, n_windows, stride, samples_per_window, st, bo, results, nullptr, draft_tokens);
+}
+
 }  // extern "C"
 
 wk_status wk::transcribe_windows_stop(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
                                       const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
-                                      wk_decode_result* results, const StopRule* stop) {
+                                      wk_decode_result* results, const StopRule* stop, int draft) {
     if (!m || !s || !pcm_host || !st || !bo || !bo->opts || bo->n_opts < 1 || !results || n_windows < 1) { set_error("wk_transcribe_windows: null argument"); return WK_ERR_INVALID_ARGUMENT; }
     if (s->m != m) { set_error("wk_transcribe_windows: session belongs to another model"); return WK_ERR_INVALID_ARGUMENT; }
     if (bo->n_opts != 1 && bo->n_opts != n_windows) { set_error("wk_transcribe_windows: %d option sets for %lld windows", bo->n_opts, (long long)n_windows); return WK_ERR_INVALID_ARGUMENT; }
     if (bo->prompts && !bo->prompt_lens) { set_error("wk_transcribe_windows: prompts without prompt_lens"); return WK_ERR_INVALID_ARGUMENT; }
     if (!m->finalized) { set_error("wk_transcribe_windows: model weights not finalized"); return WK_ERR_MODELS_UNAVAILABLE; }
     WK_CUDA_CHECK(cudaSetDevice(m->device));
-    CoreArgs a{pcm_host, n_windows, stride, samples_per_window, st, bo, results, true, stop};
+    CoreArgs a{pcm_host, n_windows, stride, samples_per_window, st, bo, results, true, stop, draft};
     return transcribe_core(s, a);
 }
 
@@ -1400,6 +1538,12 @@ wk_status wk_transcribe_windows(wk_model* m, wk_session* s, const float* pcm_hos
 wk_status wk_session_stats(const wk_session* s, int64_t* out4) {
     if (!s || !out4) return WK_ERR_INVALID_ARGUMENT;
     memcpy(out4, s->stats, sizeof(s->stats));
+    return WK_OK;
+}
+
+wk_status wk_session_draft_stats(const wk_session* s, int64_t* out3) {
+    if (!s || !out3) return WK_ERR_INVALID_ARGUMENT;
+    memcpy(out3, s->draft_stats, sizeof(s->draft_stats));
     return WK_OK;
 }
 

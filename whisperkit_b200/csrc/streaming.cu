@@ -281,7 +281,7 @@ wk_status wk_streamer_round(wk_streamer* t, int32_t* ids, int32_t cap, int32_t* 
         stop.logprob_threshold = t->opts.logprob_threshold;
         wk_transcription* T = nullptr;
         wk_status rc = seek_loop_units(t->m, t->s, units, (int)ready.size(), &t->st, &t->opts, t->prompt.data(), (int32_t)t->prompt.size(), 1.0f, -1,
-                                       t->has_hooks ? &t->hooks : nullptr, 0, &stop, false, &T);
+                                       t->has_hooks ? &t->hooks : nullptr, 0, 0, &stop, false, &T);
         if (rc != WK_OK) return rc;
         std::vector<size_t> local(T->segments.size());   // index of each result segment inside its stream's list
         for (size_t g = 0; g < T->segments.size(); ++g) {

@@ -41,7 +41,7 @@ def _same(a: StreamState, b: StreamState) -> bool:
 
 
 class AudioStreamTranscriber:
-    """One streamer per DecodingOptions.  Beam search and bestOf are not supported in streams (WK_ERR_INVALID_ARGUMENT)."""
+    """One streamer per DecodingOptions.  Beam search, bestOf and draftTokens are not supported in streams (WK_ERR_INVALID_ARGUMENT)."""
 
     def __init__(self, kit, decodingOptions: Optional[DecodingOptions] = None, requiredSegmentsForConfirmation: int = 2,
                  silenceThreshold: float = 0.3, compressionCheckWindow: int = 60, useVAD: bool = True,
@@ -49,6 +49,8 @@ class AudioStreamTranscriber:
         opts = kit.resolveLanguage(decodingOptions or DecodingOptions())
         if opts.bestOf:
             raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"bestOf={opts.bestOf} is not supported in streams")
+        if opts.draftTokens:
+            raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"draftTokens={opts.draftTokens} is not supported in streams")
         self.kit, self.options, self.lib = kit, opts, kit.model.lib
         self.stateChangeCallback = stateChangeCallback
         prompt = kit.textDecoder.prefillDecoderInputs(opts if opts.usePrefillPrompt else None, kit.specialTokens)

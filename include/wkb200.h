@@ -402,6 +402,26 @@ wk_status wk_transcribe_windows_draft(wk_model* m, wk_session* s, const float* p
 wk_status wk_decode_text_draft(wk_session* s, const wk_special_tokens* st, const wk_batch_opts* bo, int32_t draft_tokens,
                                wk_decode_result* results);
 
+/* ---- contextual biasing (DecodingOptions.biasPhrases): boost caller-given token phrases inside the fused decode loop ----
+ * A set is P phrases (1..256) of 1..16 text token ids each (ids below special_token_begin), 1024 ids in all, and one boost λ >= 0.
+ * Every decode row keeps a KMP match length m_p per phrase, 0 at its first sampled position (forced prompt tokens and detection steps
+ * leave it alone; every window and every ladder rung starts over).  With G = max_p m_p and g(v) = max_p δ_p(m_p, v) (the match length
+ * token v leads to, a completion counting as the phrase's length), token v gets b(v) = λ·(g(v) - G) on top of the filtered logits:
+ * a partial match earns λ per token, breaking it takes that back, and completing a phrase keeps it.  Suppressed tokens stay
+ * suppressed.  The choice (argmax, the top-k draw, beam ranking, the finished list and the best-of pick) follows the biased scores;
+ * every reported value (token log-probs, avgLogProb, the fallback thresholds, compressionRatio, noSpeechProb, word timings) stays the
+ * model's own.  λ = 0 decodes byte-identically to no set. */
+typedef struct wk_bias wk_bias;
+/* host only: validates the phrases (tokens: the phrases back to back, phrase_lens: their lengths) and builds the match tables */
+wk_status wk_bias_create(const int32_t* tokens, const int32_t* phrase_lens, int32_t n_phrases, float boost, int32_t special_token_begin,
+                         wk_bias** out);
+void wk_bias_free(wk_bias* b);
+/* Attaches sets to the session's following calls (copied: the sets may be freed afterwards); n_sets = 0 detaches.  n_sets = 1: every
+ * window; else one per window (wk_transcribe_windows*, wk_decode_text*) or per stream (wk_transcribe_streams*), a call of another size
+ * failing with WK_ERR_INVALID_ARGUMENT.  A NULL entry leaves its window unbiased; a set passed twice is stored once.  While a set is
+ * attached the draft entry points and wk_streamer_round return WK_ERR_INVALID_ARGUMENT. */
+wk_status wk_session_set_bias(wk_session* s, const wk_bias* const* sets, int64_t n_sets);
+
 /* ---- multi-GPU edges (SURVEY section 8e): one process per GPU, windows sharded, weights replicated; NCCL only moves PCM out and
  * results back (grouped ncclSend / ncclRecv over NVLink).  NCCL is resolved at run time from the process; wk_comm_unique_id fails with
  * WK_ERR_MODELS_UNAVAILABLE if it is not there.  The 128-byte id from rank 0 reaches the other ranks by whatever the host uses for

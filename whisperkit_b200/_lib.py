@@ -192,6 +192,9 @@ SYMBOLS = [
     ("wk_transcribe_windows_draft", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts), I32,
                                           C.POINTER(wk_decode_result)]),
     ("wk_decode_text_draft", I32, [P, C.POINTER(wk_special_tokens), C.POINTER(wk_batch_opts), I32, C.POINTER(wk_decode_result)]),
+    ("wk_bias_create", I32, [PI32, PI32, I32, F32, I32, C.POINTER(P)]),
+    ("wk_bias_free", None, [P]),
+    ("wk_session_set_bias", I32, [P, C.POINTER(P), I64]),
     ("wk_transcribe_windows", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts),
                                     PI32, I32, C.POINTER(wk_decode_result)]),
     ("wk_comm_shard_bounds", None, [I64, I32, I32, PI64, PI64]),

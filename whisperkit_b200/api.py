@@ -14,11 +14,12 @@ All arithmetic happens in libwkb200.so (sm_90a kernels); this module only marsha
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 import os
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Union
 
 import numpy as np
 
@@ -128,6 +129,12 @@ class DecodingOptions:
     # a window takes effect at a round boundary.  One value per call; refused with beamSize > 1, bestOf, wordTimestamps and streams
     # (C: wk_transcribe_windows_draft, wk_decode_text_draft, wk_transcribe_streams_draft)
     draftTokens: int = 0
+    # contextual biasing inside the fused decode loop (C: wk_bias_create / wk_session_set_bias): phrases whose tokens earn biasBoost per
+    # matched token while a partial match lasts, kept once the phrase completes.  A string is tokenized twice through the kit's tokenizer,
+    # as encode(" " + s) and encode(s); a list of ints is taken as given.  Reported log-probs and thresholds stay the model's own.  The
+    # 2.0 default is not tuned on a real checkpoint.  Refused with draftTokens and in AudioStreamTranscriber
+    biasPhrases: Optional[List[Union[str, List[int]]]] = None
+    biasBoost: float = 2.0
 
     @property
     def detectsLanguage(self) -> bool:
@@ -552,10 +559,11 @@ class TextDecoder:
         bo, keep = make_batch_opts(n, opts, prompt, callback, callbackEvery, None)
         res = (wk_decode_result * n)()
         draft = draft_tokens_of(opts)
-        if draft:
-            check(self.lib.wk_decode_text_draft(self.handle, C.byref(st), C.byref(bo), draft, res))
-        else:
-            check(self.lib.wk_decode_text_ex(self.handle, C.byref(st), C.byref(bo), res))
+        with attached_bias(self.lib, self.handle, opts, specialTokens):
+            if draft:
+                check(self.lib.wk_decode_text_draft(self.handle, C.byref(st), C.byref(bo), draft, res))
+            else:
+                check(self.lib.wk_decode_text_ex(self.handle, C.byref(st), C.byref(bo), res))
         out = [DecodingResult.from_c(r) for r in res]
         attach_languages(out, *session_languages(self.lib, self.handle, n))
         attach_no_speech_probs(out, session_no_speech_probs(self.lib, self.handle, n))
@@ -676,6 +684,58 @@ def draft_tokens_of(options) -> int:
     if len(draft) != 1:
         raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"draftTokens must be the same for every window of a call (got {sorted(draft)})")
     return draft.pop()
+
+
+def bias_phrase_tokens(phrases, tokenizer=None) -> List[List[int]]:
+    """DecodingOptions.biasPhrases as token phrases: a string gives encode(" " + s) and encode(s) (distinct spellings once each), a list
+    of ints is taken as given."""
+    out: List[List[int]] = []
+    for ph in phrases:
+        if isinstance(ph, str):
+            if tokenizer is None:
+                raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"biasPhrases entry {ph!r} needs a tokenizer (or pass token ids)")
+            for t in (tokenizer.encode(" " + ph), tokenizer.encode(ph)):
+                if list(t) not in out:
+                    out.append([int(v) for v in t])
+        else:
+            out.append([int(v) for v in ph])
+    return out
+
+
+@contextlib.contextmanager
+def attached_bias(lib, session, options, specialTokens: "SpecialTokens", tokenizer=None):
+    """Attaches the bias sets of `options` (one DecodingOptions, or one per window / stream) to the session for the duration of one call
+    and detaches them after it.  Options with the same phrases and boost share one set; options without phrases leave their windows
+    unbiased.  Does nothing when no option carries phrases."""
+    opt_list = list(options) if isinstance(options, (list, tuple)) else [options]
+    if all(o.biasPhrases is None for o in opt_list):
+        yield
+        return
+    handles, by_key = [], {}
+    try:
+        for o in opt_list:
+            if o.biasPhrases is None:
+                handles.append(None)
+                continue
+            phrases = bias_phrase_tokens(o.biasPhrases, tokenizer)
+            key = (tuple(tuple(p) for p in phrases), float(o.biasBoost))
+            if key not in by_key:
+                flat = [t for p in phrases for t in p]
+                toks = (C.c_int32 * max(1, len(flat)))(*flat)
+                lens = (C.c_int32 * max(1, len(phrases)))(*[len(p) for p in phrases])
+                h = C.c_void_p()
+                check(lib.wk_bias_create(toks, lens, len(phrases), float(o.biasBoost), int(specialTokens.specialTokenBegin), C.byref(h)))
+                by_key[key] = h
+            handles.append(by_key[key])
+        arr = (C.c_void_p * len(handles))(*[h.value if h is not None else None for h in handles])
+        check(lib.wk_session_set_bias(session, arr, len(handles)))
+        try:
+            yield
+        finally:
+            check(lib.wk_session_set_bias(session, None, 0))
+    finally:
+        for h in by_key.values():
+            lib.wk_bias_free(h)
 
 
 def make_batch_opts(n: int, options, prompt, callback=None, callbackEvery: int = 0, status=None, encoderChunk: int = 0):
@@ -873,12 +933,13 @@ class WhisperKit:
         # the prompt of every window is built inside the library from that window's options (prefillDecoderInputs); decodeWithFallback
         # (TranscribeTask.swift:316-411) runs there too: a window whose DecodingFallback asks for it is decoded again at the next temperature
         draft = draft_tokens_of(opts)
-        if draft:
-            check(self.model.lib.wk_transcribe_windows_draft(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw, C.byref(st),
-                                                             C.byref(bo), draft, res))
-        else:
-            check(self.model.lib.wk_transcribe_windows_ex(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw, C.byref(st),
-                                                          C.byref(bo), res))
+        with attached_bias(self.model.lib, self.textDecoder.handle, opts, self.specialTokens, self.tokenizer):
+            if draft:
+                check(self.model.lib.wk_transcribe_windows_draft(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw,
+                                                                 C.byref(st), C.byref(bo), draft, res))
+            else:
+                check(self.model.lib.wk_transcribe_windows_ex(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw,
+                                                              C.byref(st), C.byref(bo), res))
         self.textDecoder.batch = min(n, self.config.maxBatch)
         out = []
         for i, r in enumerate(res):

@@ -54,7 +54,10 @@ __global__ void decode_slots_init_kernel(DecodeState st, RowParams* __restrict__
         // sample rung) must read its own cache rows.  beam_update_kernel rewrites the entries of beam rows before they are read
         if (bs.use_anc) bs.anc[b * kMaxCtx + t] = b;
     }
+    if (st.bias_pool)   // every phrase match starts over with the window and with each ladder rung
+        for (int t = threadIdx.x; t < kMaxBiasPhrases; t += blockDim.x) st.bias_m[b * kMaxBiasPhrases + t] = 0;
     if (threadIdx.x == 0) {
+        if (st.bias_pool) st.bias_acc[b] = 0;
         rp_dev[b] = R;
         st.n_tokens[b] = n_prompt;
         st.next_token[b] = n_prompt > 0 ? prompts[i * kMaxCtx + n_prompt - 1] : 0;
@@ -801,6 +804,17 @@ __device__ __forceinline__ ArgMax block_argmax_row(const float* srow, int lo, in
     return best;
 }
 
+// the softmax at temperature 1 / inv_t over srow[lo, V) whose scaled max is zmax: its normaliser, and the probability of a value x
+__device__ __forceinline__ float tempered_sum(const float* srow, int lo, int V, float inv_t, float zmax, float* scratch) {
+    float z = 0.f;
+    for (int i = lo + threadIdx.x; i < V; i += kSamplerThreads) {
+        const float x = srow[i];
+        if (x != -INFINITY) z += __expf(x * inv_t - zmax);
+    }
+    return block_sum(z, scratch);
+}
+__device__ __forceinline__ float tempered_prob(float x, float inv_t, float zmax, float z) { return __expf(x * inv_t - zmax) / z; }
+
 // GreedyTokenSampler.update on a filtered row staged in smem, restricted to [lo, V) whose max is `m` and log-sum-exp `lse`:
 // temperature 0 = argmax; > 0 = logits / T, softmax over the whole (filtered) range, top-k, multinomial draw inside the top-k mass,
 // logprob = log softmax prob of the draw (TokenSampler.swift:57-73 / :140-180).  The reference draws with Float.random
@@ -817,12 +831,7 @@ __device__ __forceinline__ ArgMax sample_row(float* srow, int lo, int V, float m
     }
     const float inv_t = 1.f / temperature;
     const float zmax = m * inv_t;
-    float z = 0.f;
-    for (int i = lo + tid; i < V; i += kSamplerThreads) {
-        const float x = srow[i];
-        if (x != -INFINITY) z += __expf(x * inv_t - zmax);
-    }
-    z = block_sum(z, scratch);
+    const float z = tempered_sum(srow, lo, V, inv_t, zmax, scratch);
     __shared__ float topv[32];
     __shared__ int topi[32];
     const int k = top_k < 1 ? 1 : (top_k > 32 ? 32 : top_k);
@@ -830,7 +839,7 @@ __device__ __forceinline__ ArgMax sample_row(float* srow, int lo, int V, float m
     for (; kk < k; ++kk) {
         const ArgMax a = block_argmax_row(srow, lo, V, sarg);
         if (a.v == -INFINITY) break;
-        if (tid == 0) { topv[kk] = __expf(a.v * inv_t - zmax) / z; topi[kk] = a.i; srow[a.i] = -INFINITY; }
+        if (tid == 0) { topv[kk] = tempered_prob(a.v, inv_t, zmax, z); topi[kk] = a.i; srow[a.i] = -INFINITY; }
         __syncthreads();
     }
     __syncthreads();
@@ -855,6 +864,81 @@ __device__ __forceinline__ ArgMax sample_row(float* srow, int lo, int V, float m
 // (subsequence b), so that detecting moves no token draw of the decode
 static constexpr unsigned long long kDetectSubsequence = 1ull << 32;
 
+// ---- DecodingOptions.biasPhrases (tests/bias_ref.py is the specification).  A row keeps one KMP match length m_p per phrase; a token v
+// earns b(v) = λ·(g(v) - G) with G = max_p m_p and g(v) = max_p δ_p(m_p, v).  Only the tokens on some phrase's failure chain from m_p
+// have g > 0: at most Σ L_p = 1024 of them, one per thread of the sampler's CTA.
+struct BiasSet {
+    const int32_t* desc; const int32_t* tok; const int32_t* fail; int n;
+    __device__ BiasSet(const int32_t* pool, const RowParams& R)
+        : desc(pool + R.bias_off), tok(pool + R.bias_off + R.bias_n), fail(pool + R.bias_off + R.bias_n + R.bias_len), n(R.bias_n) {}
+};
+
+// δ_p(k, v), a completion counting as L_p; *stored: the state the row keeps (f_p(L_p) after a completion)
+__device__ __forceinline__ int bias_step(const BiasSet& B, int p, int k, int v, int* stored) {
+    const int d = B.desc[p], start = d & 0xffff, len = d >> 16;
+    const int32_t* w = B.tok + start;
+    const int32_t* f = B.fail + start;
+    while (k > 0 && w[k] != v) k = f[k - 1];
+    k = w[k] == v ? k + 1 : 0;
+    *stored = k == len ? f[len - 1] : k;
+    return k;
+}
+
+// adds b(v) to srow[lo, V) in place (−inf stays −inf); returns G.  cand: kMaxBiasTotal packed (token | g << 20) entries of shared memory
+__device__ int bias_apply(float* srow, int lo, int V, const BiasSet& B, const uint8_t* m, float boost, float* scratch, int* cand, int* ncand) {
+    const int tid = threadIdx.x;
+    const int mp = tid < B.n ? m[tid] : 0;
+    if (tid == 0) *ncand = 0;
+    const int G = (int)block_max((float)mp, scratch);   // (its barriers also publish *ncand = 0)
+    if (tid < B.n) {   // the failure chain mp, f(mp), ..., 0: token w[k] continues the match to k + 1 (the first such k is δ, the largest)
+        const int d = B.desc[tid], start = d & 0xffff;
+        const int32_t* w = B.tok + start;
+        const int32_t* f = B.fail + start;
+        for (int k = mp;; k = f[k - 1]) {
+            cand[atomicAdd(ncand, 1)] = w[k] | (k + 1) << 20;
+            if (k == 0) break;
+        }
+    }
+    __syncthreads();
+    const int nc = *ncand;
+    int tok = -1;
+    float val = 0.f;
+    if (tid < nc) {   // one owner per token (its first entry) applies the maximum over the phrases
+        const int c = cand[tid];
+        tok = c & 0xfffff;
+        int g = c >> 20;
+        for (int j = 0; j < nc && tok >= 0; ++j) {
+            const int o = cand[j];
+            if ((o & 0xfffff) != tok) continue;
+            if (j < tid) tok = -1;
+            else g = max(g, o >> 20);
+        }
+        if (tok < lo || tok >= V) tok = -1;
+        if (tok >= 0) val = srow[tok] + boost * (float)(g - G);
+    }
+    const float base = boost * (float)(0 - G);   // b of every token outside the chains
+    if (base != 0.f) {
+        __syncthreads();
+        for (int i = lo + tid; i < V; i += kSamplerThreads) srow[i] += base;
+        __syncthreads();
+    }
+    if (tok >= 0) srow[tok] = val;
+    __syncthreads();
+    return G;
+}
+
+// the row's states after token v; returns g(v) (block-uniform)
+__device__ int bias_advance(const BiasSet& B, uint8_t* m, int v, float* scratch) {
+    const int tid = threadIdx.x;
+    int g = 0;
+    if (tid < B.n) {
+        int stored;
+        g = bias_step(B, tid, m[tid], v, &stored);
+        m[tid] = (uint8_t)stored;
+    }
+    return (int)block_max((float)g, scratch);
+}
+
 __global__ void __launch_bounds__(kSamplerThreads)
 sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerParams p, DecodeState st,
                const int32_t* __restrict__ tokens_in, int ld_tokens, const int32_t* __restrict__ n_tokens_in,
@@ -863,6 +947,8 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
     __shared__ float scratch[32];
     __shared__ int sflag[8];     // 0: ts filter active, 1: lo0, 2: hi0 (interval A), 3: lo1, 4: hi1 (interval B), 5: blank active
     __shared__ ArgMax sarg[32];
+    __shared__ int s_cand[kMaxBiasTotal];   // biasPhrases: the row's (token, g) candidates, then the appended token (s_adv)
+    __shared__ int s_ncand, s_adv;
     const int b = blockIdx.x, tid = threadIdx.x;
     const int V = p.vocab;
     const bool loop_mode = p.loop_mode != 0;
@@ -1053,6 +1139,22 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         for (int i = tid; i < V; i += kSamplerThreads) filtered_out[(long long)b * V + i] = srow[i];
         __syncthreads();
     }
+    // DecodingOptions.biasPhrases: from the row's first sampled position on (prompt forcing and detection steps are left alone), the
+    // phrase bonus joins the filtered row after every filter.  The choice sees it; the reported log-probs stay the model's: a chosen
+    // token's filtered value is its raw logit, so they come from `row`, against the unbiased normaliser
+    const bool biased = loop_mode && st.bias_pool != nullptr && R.bias_n > 0 && st.steps[b] >= R.prompt_len - 1;
+    float m_draw = ts_wins ? mts : mall;
+    float z_unbiased = 0.f;
+    int bias_G = 0;
+    if (biased) {
+        if (R.mode != kRowBeam && R.temperature != 0.f) z_unbiased = tempered_sum(srow, lo, V, 1.f / R.temperature, m_draw * (1.f / R.temperature), scratch);
+        const BiasSet B(st.bias_pool, R);
+        bias_G = bias_apply(srow, lo, V, B, st.bias_m + b * kMaxBiasPhrases, R.bias_boost, scratch, s_cand, &s_ncand);
+        float mx = -INFINITY;
+        for (int i = lo + tid; i < V; i += kSamplerThreads) mx = fmaxf(mx, srow[i]);
+        mx = block_max(mx, scratch);
+        if (R.temperature != 0.f) m_draw = mx;
+    }
     if (loop_mode && R.mode == kRowBeam) {
         // beam search: rank the row's (beam + 1) best tokens of the filtered log-softmax, best first (whisper BeamSearchDecoder.update step 1);
         // the per-window merge and every state update happen in beam_update_kernel
@@ -1062,7 +1164,8 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
             const bool ok = a.v != -INFINITY && a.i >= 0 && a.i < V;   // (a NaN row yields the initial index: no candidate)
             if (tid == 0) {
                 p.beam.cand_tok[b * (kMaxBeam + 1) + kk] = ok ? a.i : -1;
-                p.beam.cand_lp[b * (kMaxBeam + 1) + kk] = ok ? a.v - lse : -INFINITY;
+                p.beam.cand_lp[b * (kMaxBeam + 1) + kk] = ok ? (biased ? row[a.i] : a.v) - lse : -INFINITY;
+                p.beam.cand_sc[b * (kMaxBeam + 1) + kk] = ok ? a.v - lse : -INFINITY;
                 if (ok) srow[a.i] = -INFINITY;
             }
             __syncthreads();
@@ -1070,9 +1173,13 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         return;
     }
     // the row's draw: Philox(seed, row, step) at temperature > 0 (row: the slot in a draft call, whose windows sample on row 0 only)
-    const ArgMax best = sample_row(srow, lo, V, ts_wins ? mts : mall, lse, R.temperature, R.top_k, R.seed, (unsigned long long)(b / max(1, p.rng_div)),
+    const ArgMax best = sample_row(srow, lo, V, m_draw, lse, R.temperature, R.top_k, R.seed, (unsigned long long)(b / max(1, p.rng_div)),
                                    (unsigned long long)(loop_mode ? st.steps[b] : n_tok), scratch, sarg);
-    const float lp_sampled = best.v;
+    float lp_sampled = best.v;
+    if (biased && best.i >= 0 && best.i < V)
+        lp_sampled = R.temperature == 0.f ? row[best.i] - lse
+                                          : logf(tempered_prob(row[best.i], 1.f / R.temperature, (ts_wins ? mts : mall) * (1.f / R.temperature), z_unbiased));
+    if (tid == 0) s_adv = -1;
     if (tid == 0) {
         int tok = best.i;
         float lp = lp_sampled;
@@ -1098,9 +1205,17 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
                     st.tokens[b * kMaxCtx + n_tok] = tok;
                     st.logprobs[b * kMaxCtx + n_tok] = lp;
                     st.n_tokens[b] = n_tok + 1;
+                    if (biased) s_adv = tok;
                 }
                 if (step + 1 >= R.max_steps) st.done[b] = 1;   // loop bound min(sampleLength, 223) reached (TextDecoder.swift:566)
             }
+        }
+    }
+    if (biased) {   // the appended token moves the row's matches on; the bonus it earned is banked for the best-of ranking
+        __syncthreads();
+        if (s_adv >= 0) {
+            const int g = bias_advance(BiasSet(st.bias_pool, R), st.bias_m + b * kMaxBiasPhrases, s_adv, scratch);
+            if (tid == 0) st.bias_acc[b] += g - bias_G;
         }
     }
 }
@@ -1152,7 +1267,7 @@ beam_update_kernel(DecodeState st, BeamState bs, wk_special_tokens S, int max_ct
                     const int t = bs.cand_tok[(r0 + j) * C1 + k];
                     if (t < 0) continue;
                     const float v = bs.cand_lp[(r0 + j) * C1 + k];
-                    c_score[nc] = bs.sum_lp[r0 + j] + v; c_lp[nc] = v; c_src[nc] = j; c_tok[nc] = t; c_ord[nc] = nc; ++nc;
+                    c_score[nc] = bs.sum_lp[r0 + j] + bs.cand_sc[(r0 + j) * C1 + k]; c_lp[nc] = v; c_src[nc] = j; c_tok[nc] = t; c_ord[nc] = nc; ++nc;
                 }
             for (int i = 1; i < nc; ++i) {             // stable insertion sort, best score first
                 const int o = c_ord[i];
@@ -1220,6 +1335,18 @@ beam_update_kernel(DecodeState st, BeamState bs, wk_special_tokens S, int max_ct
         st.n_tokens[r] = n_tok + 1;
         st.next_token[r] = n_tokv[tid];
         bs.sum_lp[r] = n_score[tid];
+    }
+    if (st.bias_pool && R.bias_n > 0) {   // biasPhrases: each surviving beam takes its source beam's matches, moved on by its new token
+        __shared__ uint8_t s_m[kMaxBeam][kMaxBiasPhrases];
+        const BiasSet B(st.bias_pool, R);
+        for (int i = tid; i < beam * B.n; i += kBeamThreads) s_m[i / B.n][i % B.n] = st.bias_m[(r0 + i / B.n) * kMaxBiasPhrases + i % B.n];
+        __syncthreads();
+        for (int i = tid; i < beam * B.n; i += kBeamThreads) {
+            const int j = i / B.n, ph = i % B.n;
+            int stored;
+            bias_step(B, ph, s_m[n_src[j]][ph], n_tokv[j], &stored);
+            st.bias_m[(r0 + j) * kMaxBiasPhrases + ph] = (uint8_t)stored;
+        }
     }
 }
 

@@ -186,6 +186,10 @@ struct RowParams {
     // DecodingResult.noSpeechProb: the step (= index of the prompt's first SOT) whose raw logits give it, <0 = off
     int32_t no_speech_pos;
     int32_t mode;                // kRowSingle / kRowBeam / kRowSample: how the row's rung decodes (one step mixes groups at different rungs)
+    // DecodingOptions.biasPhrases: the window's phrase set in the session's bias pool (DecodeState.bias_pool + bias_off), bias_n phrases
+    // of bias_len tokens in all (0 = no bias), boost λ
+    int32_t bias_off, bias_n, bias_len;
+    float bias_boost;
 };
 // RowParams.mode.  Single and sample rows run the per-row sampler and bookkeeping (a sample row is one of best_of independent draws of its
 // group); beam rows only rank candidates, and beam_update_kernel does their bookkeeping per group
@@ -207,8 +211,16 @@ struct DecodeState {
     float* lang_logprob;  // [Bmax]
     int32_t* lang_state;  // [Bmax] kLangLead: the leading detection step is next; kLangLeadRan: it was this step's; 0 otherwise
     float* no_speech;     // [Bmax] softmax(raw logits)[no_speech_token] at step RowParams.no_speech_pos; NaN = not computed
+    // contextual biasing: the phrase pool of the call's sets (nullptr = no set attached: the loop never reads the two arrays below),
+    // each row's KMP match length per phrase and the sum of g(v) - G over its appended tokens (the bonus it banked, in units of λ)
+    const int32_t* bias_pool;
+    uint8_t* bias_m;      // [Bmax][kMaxBiasPhrases]
+    int32_t* bias_acc;    // [Bmax]
 };
 constexpr int kLangLead = 2, kLangLeadRan = 3;
+// A bias set: up to 256 phrases of 1..16 token ids each, 1024 tokens in all.  Its pool record is [n] descriptors (start | len << 16),
+// [total] phrase tokens, [total] failure links (f(k) for k = 1..len of a phrase at its start + k - 1)
+constexpr int kMaxBiasPhrases = 256, kMaxBiasLen = 16, kMaxBiasTotal = 1024;
 
 // Beam search (SURVEY 8f row 2; semantics restated from openai/whisper BeamSearchDecoder in oracle/beam_ref.py - the reference's
 // BeamSearchTokenSampler is a fatalError stub, TokenSampler.swift:254-290).  Decode rows come in groups of `group` consecutive rows per
@@ -221,6 +233,7 @@ struct BeamState {
     int group;                     // decode rows per window (<= 1: one)
     float* sum_lp;                 // [rows] cumulative log-prob of the sampled tokens of the beam
     int32_t* cand_tok; float* cand_lp;   // [rows][kMaxBeam + 1] best tokens of the step's filtered log-softmax, best first (-1 = none)
+    float* cand_sc;                // [rows][kMaxBeam + 1] the candidates' score increments: cand_lp plus the phrase bonus (= cand_lp unbiased)
     int32_t* anc;                  // [rows][224] physical cache row that holds position t of this beam's self K/V
     int32_t* fin_tokens; float* fin_lps;   // [groups][kMaxCand][224] finished sequences (EOT included), per-token log-probs (EOT -> 0)
     int32_t* fin_len; float* fin_score;    // [groups][kMaxCand]
@@ -363,5 +376,9 @@ struct StopRule {
 wk_status transcribe_windows_stop(wk_model* m, wk_session* s, const float* pcm_host, int64_t n_windows, int64_t stride,
                                   const int32_t* samples_per_window, const wk_special_tokens* st, const wk_batch_opts* bo,
                                   wk_decode_result* results, const StopRule* stop, int draft = 0);
+// bias sets attached with wk_session_set_bias (0 = none), and the set each window of the session's next calls uses (empty: the plain
+// rule, set i for window i or set 0 for every window)
+int64_t session_bias_sets(const wk_session* s);
+void session_bias_map(wk_session* s, std::vector<int> map);
 
 }  // namespace wk

@@ -336,6 +336,10 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
     if (rc != WK_OK) return rc;
     const int max_batch = info.max_batch;
     const int64_t window_padding = (int64_t)(window_clip_time * (float)kSampleRate);
+    // contextual biasing: one set for every stream or one per stream
+    const int64_t n_bias = session_bias_sets(s);
+    if (n_bias > 1 && n_bias != n_streams) { set_error("%lld bias sets attached for %d streams (1 or one per stream)", (long long)n_bias, n_streams); return WK_ERR_INVALID_ARGUMENT; }
+    const bool per_stream_bias = n_bias > 1;
     for (Unit& u : units) {
         // a clip is live while seek < clipEnd - windowPadding (TranscribeTask.swift:118) and, as a guard the reference lacks (it would
         // pad a negative-length window), while the seek is still inside the audio
@@ -381,7 +385,13 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         wk_batch_opts bo;
         memset(&bo, 0, sizeof(bo));
         bo.opts = o; bo.n_opts = 1; bo.prompt = prompt; bo.n_prompt = n_prompt; bo.best_of = best_of;
+        if (per_stream_bias) {   // each window decodes with its stream's set
+            std::vector<int> map(active.size());
+            for (size_t k = 0; k < active.size(); ++k) map[k] = units[active[k]].stream;
+            session_bias_map(s, std::move(map));
+        }
         rc = transcribe_windows_stop(m, s, batch, (int64_t)active.size(), kWindow, valid.data(), st, &bo, res.data(), stop, draft_tokens);
+        if (per_stream_bias) session_bias_map(s, {});
         if (rc != WK_OK) return rc;
         T->windows += (int)active.size();
         if (o->detect_language) {   // TranscriptionResult.language: the stream keeps the language of its last detecting window

@@ -93,6 +93,21 @@ struct wk_session {
     DraftRound dr = DraftRound();
     int64_t draft_stats[3] = {0, 0, 0};   // of the last batched call: rounds that verified, proposals verified, proposals accepted
     int graph_draft = 0;
+    // contextual biasing (wk_session_set_bias): the attached sets' records in one device pool, where each set sits in it (n = 0: a
+    // window without bias), and the per-window set indices a long-form round uses (empty: set i for window i, or set 0 for all)
+    struct BiasSlot { int off = 0, n = 0, len = 0; float boost = 0.f; };
+    int32_t* bias_pool = nullptr; size_t bias_cap = 0;
+    std::vector<BiasSlot> bias_sets;
+    std::vector<int> bias_map;
+    int32_t* h_bias_acc = nullptr;
+    const int32_t* graph_bias = nullptr;
+};
+
+// a phrase set as wk_bias_create validated it: its pool record (kernels.h) and boost
+struct wk_bias {
+    std::vector<int32_t> rec;
+    int n = 0, len = 0;
+    float boost = 0.f;
 };
 
 // The cached step graphs bake in the call's shape and the session's buffer pointers: dropped, they are captured again on the next step
@@ -117,6 +132,8 @@ namespace wk {
 AudioWs** session_audio_ws(wk_session* s) { return &s->audio; }
 cudaStream_t session_stream(wk_session* s) { return s->stream; }
 int session_device(wk_session* s) { return s->m->device; }
+int64_t session_bias_sets(const wk_session* s) { return (int64_t)s->bias_sets.size(); }
+void session_bias_map(wk_session* s, std::vector<int> map) { s->bias_map = std::move(map); }
 
 // ---------------------------------------------------------------------------------------------- decoder schedule
 static wk_status dec_gemm(wk_session* s, const void* w, int N, int K, const void* act, int* splits_out, int bp = 0) {
@@ -407,12 +424,14 @@ static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bo
     }
     if (done >= n) return WK_OK;
     // the step's shape depends on the rows per window (cross K/V sharing) and on whether the call has beam rows (ancestry, beam_update)
+    // and on the bias pool the sampler reads (nullptr: no set attached)
     const int beam_key = (std::max(1, s->bs.group) * 16 + std::max(1, s->bs.beam)) * 16 + s->bs.max_candidates;
     const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_beam != beam_key ||
-                       s->graph_draft != s->draft_k || memcmp(&s->graph_st, st, sizeof(*st)) != 0;
+                       s->graph_draft != s->draft_k || s->graph_bias != s->st.bias_pool || memcmp(&s->graph_st, st, sizeof(*st)) != 0;
     if (stale) {
         drop_graphs(s);
         s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_st = *st; s->graph_beam = beam_key; s->graph_draft = s->draft_k;
+        s->graph_bias = s->st.bias_pool;
     }
     cudaGraphExec_t& exec = check_done ? s->graph_exec : s->graph_exec_live;
     if (!exec) {
@@ -483,6 +502,7 @@ static wk_status ensure_beam(wk_session* s) {
     WK_CHECK(b.dmalloc(&s->bs.sum_lp, S));
     WK_CHECK(b.dmalloc(&s->bs.cand_tok, (size_t)S * (kMaxBeam + 1)));
     WK_CHECK(b.dmalloc(&s->bs.cand_lp, (size_t)S * (kMaxBeam + 1)));
+    WK_CHECK(b.dmalloc(&s->bs.cand_sc, (size_t)S * (kMaxBeam + 1)));
     WK_CHECK(b.dmalloc(&s->bs.anc, (size_t)S * kKvMaxLen));
     WK_CHECK(b.dmalloc(&s->bs.fin_tokens, (size_t)G * kMaxCand * kKvMaxLen));
     WK_CHECK(b.dmalloc(&s->bs.fin_lps, (size_t)G * kMaxCand * kKvMaxLen));
@@ -549,6 +569,7 @@ struct CallPlan {
     std::vector<wk_status> st_local;
     wk_status* status = nullptr;                      // per window: bo->status, or st_local
     std::string first_err;                            // the message of the first window that failed
+    std::vector<int> bias_of;                         // per window: its entry of the session's bias sets (empty: no set attached)
     bool any_words = false, any_detect = false, any_nsp = false;
     void fail(int64_t w, wk_status code, wk_decode_result* results) {
         status[w] = code;
@@ -582,6 +603,17 @@ static wk_status plan_call(wk_session* s, const CoreArgs& a, CallPlan& p) {
         if (a.stop) { set_error("draft_tokens is not supported in streams"); return WK_ERR_INVALID_ARGUMENT; }
         for (int i = 0; i < bo->n_opts; ++i)
             if (bo->opts[i].word_timestamps) { set_error("draft_tokens does not combine with word timestamps"); return WK_ERR_INVALID_ARGUMENT; }
+    }
+    // contextual biasing: one attached set for every window, one per window, or the long-form round's per-window choice
+    if (!s->bias_sets.empty()) {
+        const int64_t ns = (int64_t)s->bias_sets.size();
+        if (draft != 0) { set_error("a bias set does not combine with draft_tokens"); return WK_ERR_INVALID_ARGUMENT; }
+        if (!s->bias_map.empty() ? (int64_t)s->bias_map.size() != n : (ns != 1 && ns != n)) {
+            set_error("%lld bias sets attached for a call of %lld windows (1 or one per window)", (long long)ns, (long long)n);
+            return WK_ERR_INVALID_ARGUMENT;
+        }
+        p.bias_of.resize((size_t)n);
+        for (int64_t w = 0; w < n; ++w) p.bias_of[w] = !s->bias_map.empty() ? s->bias_map[w] : (ns == 1 ? 0 : (int)w);
     }
     const int G = p.G = draft > 0 ? draft + 1 : std::max(beam, std::max(best_of, 1));
     if (G > s->max_batch) {
@@ -751,6 +783,13 @@ static RowParams row_params(const CallPlan& p, const wk_batch_opts* bo, const wk
     return R;
 }
 
+// the bias set of window w (RowParams.bias_*), none when the call has no set attached
+static void row_bias(const wk_session* s, const CallPlan& p, int64_t w, RowParams& R) {
+    if (p.bias_of.empty()) return;
+    const wk_session::BiasSlot& b = s->bias_sets[p.bias_of[w]];
+    R.bias_off = b.off; R.bias_n = b.n; R.bias_len = b.len; R.bias_boost = b.boost;
+}
+
 // The decode slots of a call: the window each holds (-1: free), its ladder rung, and the stream stop rule's progress through the window's
 // history (entries checked, their log-prob sum).  admit() stages the window's rows in the session's pinned buffers, flush() sends what
 // is staged to the device in one go
@@ -764,7 +803,8 @@ struct Slots {
     // window w into free slot q at rung 0, or back into its slot at the next rung
     wk_status admit(int q, int64_t w, int r) {
         int active = 1;
-        const RowParams R = row_params(p, a.bo, a.st, w, r, &active);
+        RowParams R = row_params(p, a.bo, a.st, w, r, &active);
+        row_bias(s, p, w, R);
         if (staged == 0) WK_CUDA_CHECK(cudaEventSynchronize(s->ev_stage));   // the previous round's copies out of the pinned staging have landed
         for (int j = 0; j < active; ++j) {                                     // beam search / best-of: `active` identical rows start the window
             s->h_adm_slots[staged] = q * p.G + j;
@@ -884,6 +924,7 @@ static wk_status read_back(wk_session* s, const CallPlan& p) {
         WK_CUDA_CHECK(cudaMemcpyAsync(s->h_lang_logprob, s->st.lang_logprob, rows * 4, cudaMemcpyDeviceToHost, s->stream));
     }
     if (p.any_nsp) WK_CUDA_CHECK(cudaMemcpyAsync(s->h_no_speech, s->st.no_speech, rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    if (!p.bias_of.empty() && p.best_of > 1) WK_CUDA_CHECK(cudaMemcpyAsync(s->h_bias_acc, s->st.bias_acc, rows * 4, cudaMemcpyDeviceToHost, s->stream));
     if (p.beam > 1) {
         WK_CUDA_CHECK(cudaMemcpyAsync(s->h_sum_lp, s->bs.sum_lp, rows * 4, cudaMemcpyDeviceToHost, s->stream));
         WK_CUDA_CHECK(cudaMemcpyAsync(s->h_n_fin, s->bs.n_fin, slots * 4, cudaMemcpyDeviceToHost, s->stream));
@@ -901,18 +942,20 @@ static wk_status read_back(wk_session* s, const CallPlan& p) {
 // history, the best-ranked best-of sample or the beam search winner (P: prompt length); cut after the token the stream stop rule stops
 // at when stop_at >= 0.  Points into the session's pinned readback buffers
 struct Choice { int row; const int32_t* tok; const float* lp; int n; };
-static Choice select_result(const wk_session* s, int q, int G, int mode, int beam, int best_of, int P, int stop_at) {
+static Choice select_result(const wk_session* s, int q, int G, int mode, int beam, int best_of, int P, int stop_at, float bias_boost) {
     const int r0 = q * G;
     int rc = r0;                              // the row whose result the window returns
     if (mode == kRowSample) {
         // best-of: MaximumLikelihoodRanker without length penalty over the samples (oracle/best_of_ref.py rank_best_of) - the sum of
-        // the row's recorded log-probs over max(sampled tokens, 1); ties go to the lowest row
+        // the row's recorded log-probs over max(sampled tokens, 1); ties go to the lowest row.  With a bias set the sum carries the
+        // bonus the row banked (bias_boost > 0)
         float best_rank = -INFINITY;
         for (int j = 0; j < best_of; ++j) {
             const int rr = r0 + j;
             const float* lp = s->h_logprobs + (size_t)rr * kKvMaxLen;
             float sum = 0.f;
             for (int i = 0; i < s->h_n_tokens[rr]; ++i) sum += lp[i];
+            if (bias_boost != 0.f) sum += bias_boost * (float)s->h_bias_acc[rr];
             const float rk = sum / (float)std::max(s->h_n_tokens[rr] - P, 1);
             if (j == 0 || rk > best_rank) { rc = rr; best_rank = rk; }
         }
@@ -965,6 +1008,7 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     if (p.draft > 0) WK_CHECK(ensure_draft(s));
     s->bs.beam = beam; s->bs.max_candidates = p.max_cand; s->bs.group = G; s->bs.use_anc = beam > 1 || p.draft > 0;
     s->draft_k = p.draft;
+    s->st.bias_pool = p.bias_of.empty() ? nullptr : s->bias_pool;
     WK_CHECK(upload_plan(s, p));
     s->align_on = p.any_words;
     s->win_align_lp.clear();   // the log-probs belong to the last align call only
@@ -1053,7 +1097,8 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             if (!ended) continue;
             const float temperature = rung_temperature(o, slots.rung[q]);
             int active = 1;
-            const Choice ch = select_result(s, q, G, rung_mode(beam, best_of, temperature, &active), beam, best_of, p.win[w].np, stop_at);
+            const float boost = p.bias_of.empty() ? 0.f : s->bias_sets[p.bias_of[w]].boost;
+            const Choice ch = select_result(s, q, G, rung_mode(beam, best_of, temperature, &active), beam, best_of, p.win[w].np, stop_at, boost);
             // beam search: every beam of the window is the same forced copy through the prefill, so row r0 holds the value
             const float nsp = o.compute_no_speech_prob ? s->h_no_speech[r0] : NAN;
             wk_decode_result r;
@@ -1346,6 +1391,9 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
     WK_CHECK(b.pinned(&s->h_lang_token, S));
     WK_CHECK(b.pinned(&s->h_lang_logprob, S));
     WK_CHECK(b.pinned(&s->h_no_speech, S));
+    WK_CHECK(b.dmalloc(&s->st.bias_m, (size_t)S * kMaxBiasPhrases));
+    WK_CHECK(b.dmalloc(&s->st.bias_acc, S));
+    WK_CHECK(b.pinned(&s->h_bias_acc, S));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_enc, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_adm, cudaEventDisableTiming));
     WK_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_stage, cudaEventDisableTiming));
@@ -1370,6 +1418,76 @@ wk_status wk_session_reset(wk_session* s) {
     const size_t n = (size_t)c.dec_layers * s->max_batch * c.n_heads * kKvMaxLen * 64 * 2;
     WK_CUDA_CHECK(cudaMemsetAsync(s->self_k, 0, n, s->stream));
     WK_CUDA_CHECK(cudaMemsetAsync(s->self_v, 0, n, s->stream));
+    return WK_OK;
+}
+
+wk_status wk_bias_create(const int32_t* tokens, const int32_t* phrase_lens, int32_t n_phrases, float boost, int32_t special_token_begin, wk_bias** out) {
+    if (!out || !phrase_lens || !tokens) { set_error("wk_bias_create: null argument"); return WK_ERR_INVALID_ARGUMENT; }
+    *out = nullptr;
+    if (n_phrases < 1 || n_phrases > kMaxBiasPhrases) { set_error("wk_bias_create: %d phrases outside [1, %d]", n_phrases, kMaxBiasPhrases); return WK_ERR_INVALID_ARGUMENT; }
+    if (!(boost >= 0.f) || !isfinite(boost)) { set_error("wk_bias_create: boost %g is not a finite value >= 0", boost); return WK_ERR_INVALID_ARGUMENT; }
+    if (special_token_begin < 1) { set_error("wk_bias_create: special_token_begin %d", special_token_begin); return WK_ERR_INVALID_ARGUMENT; }
+    int total = 0;
+    for (int p = 0; p < n_phrases; ++p) {
+        if (phrase_lens[p] < 1 || phrase_lens[p] > kMaxBiasLen) { set_error("wk_bias_create: phrase %d has %d tokens (1..%d)", p, phrase_lens[p], kMaxBiasLen); return WK_ERR_INVALID_ARGUMENT; }
+        total += phrase_lens[p];
+        if (total > kMaxBiasTotal) { set_error("wk_bias_create: more than %d phrase tokens in all", kMaxBiasTotal); return WK_ERR_INVALID_ARGUMENT; }
+    }
+    for (int i = 0; i < total; ++i)
+        if (tokens[i] < 0 || tokens[i] >= special_token_begin) {
+            set_error("wk_bias_create: token %d is not a text token (ids below %d)", tokens[i], special_token_begin);
+            return WK_ERR_INVALID_ARGUMENT;
+        }
+    std::unique_ptr<wk_bias> B(new wk_bias());
+    B->n = n_phrases; B->len = total; B->boost = boost;
+    B->rec.assign((size_t)n_phrases + 2 * total, 0);
+    int32_t* tok = B->rec.data() + n_phrases;
+    int32_t* fail = tok + total;
+    for (int p = 0, start = 0; p < n_phrases; start += phrase_lens[p], ++p) {
+        const int L = phrase_lens[p];
+        B->rec[p] = start | L << 16;
+        memcpy(tok + start, tokens + start, (size_t)L * 4);
+        // KMP failure links: fail[k - 1] = the longest proper border of w[0..k)
+        const int32_t* w = tokens + start;
+        int32_t* f = fail + start;
+        f[0] = 0;
+        for (int k = 1, b = 0; k < L; ++k) {
+            while (b > 0 && w[k] != w[b]) b = f[b - 1];
+            if (w[k] == w[b]) ++b;
+            f[k] = b;
+        }
+    }
+    *out = B.release();
+    return WK_OK;
+}
+
+void wk_bias_free(wk_bias* b) { delete b; }
+
+wk_status wk_session_set_bias(wk_session* s, const wk_bias* const* sets, int64_t n_sets) {
+    if (!s || n_sets < 0 || (n_sets > 0 && !sets)) { set_error("wk_session_set_bias: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
+    std::vector<wk_session::BiasSlot> slots((size_t)n_sets);
+    std::vector<int32_t> pool;
+    for (int64_t i = 0; i < n_sets; ++i) {
+        const wk_bias* b = sets[i];
+        if (!b) continue;                                 // a window without bias
+        int64_t same = -1;                                // a set passed again shares its record
+        for (int64_t j = 0; j < i && same < 0; ++j) if (sets[j] == b) same = j;
+        if (same >= 0) { slots[i] = slots[same]; continue; }
+        slots[i].off = (int)pool.size(); slots[i].n = b->n; slots[i].len = b->len; slots[i].boost = b->boost;
+        pool.insert(pool.end(), b->rec.begin(), b->rec.end());
+    }
+    WK_CUDA_CHECK(cudaSetDevice(s->m->device));
+    if (pool.size() > s->bias_cap) {
+        const size_t cap = std::max<size_t>(4096, pool.size());
+        WK_CHECK(s->mem.grow(&s->bias_pool, cap, s->stream));   // a new pointer makes the next step capture its graph again
+        s->bias_cap = cap;
+    }
+    if (!pool.empty()) {
+        WK_CUDA_CHECK(cudaMemcpyAsync(s->bias_pool, pool.data(), pool.size() * 4, cudaMemcpyHostToDevice, s->stream));
+        WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));   // the host record is pageable
+    }
+    s->bias_sets = std::move(slots);
+    s->bias_map.clear();
     return WK_OK;
 }
 

@@ -225,6 +225,7 @@ wk_status wk_streamer_push(wk_streamer* t, int32_t id, const float* pcm, int64_t
 
 wk_status wk_streamer_round(wk_streamer* t, int32_t* ids, int32_t cap, int32_t* n_out) {
     if (!t || !n_out || cap < 0 || (cap > 0 && !ids)) { set_error("wk_streamer_round: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
+    if (session_bias_sets(t->s) > 0) { set_error("wk_streamer_round: the session has a bias set attached"); return WK_ERR_INVALID_ARGUMENT; }
     std::lock_guard<std::mutex> round_lock(t->round_mu);
     struct Ready { int32_t id; std::shared_ptr<Stream> stream; int64_t n; std::vector<float> audio; int64_t base; std::vector<const float*> src; };
     std::vector<Ready> ready;

@@ -11,7 +11,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import check, wk_segment
-from .api import DecodingOptions, SpecialTokens, language_code
+from .api import DecodingOptions, SpecialTokens, attached_bias, language_code
 
 
 @dataclass
@@ -162,10 +162,12 @@ def transcribe_streams(kit, audioArrays: Sequence[np.ndarray], options: Optional
     native = hooks                      # a wk_tokenizer_hooks struct (WhisperTokenizer.hooks()): the library's own tokenizer, no host callbacks
     if native is None:
         hooks, keep_hooks = make_hooks(split_to_word_tokens, decode)
-    check(lib.wk_transcribe_streams_draft(kit.model.handle, kit.textDecoder.handle, ptrs, lens, len(arrs), C.byref(st), C.byref(o), p, len(prompt),
-                                       ts, n, windowClipTime, -1 if maxWindowSeek is None else maxWindowSeek,
-                                       1 if chunkingStrategy == "vad" else 0, C.byref(hooks) if (split_to_word_tokens is not None or native is not None) else None,
-                                       int(opts.bestOf or 0), int(opts.draftTokens or 0), C.byref(h)))
+    with attached_bias(lib, kit.textDecoder.handle, opts, kit.specialTokens, kit.tokenizer):
+        check(lib.wk_transcribe_streams_draft(kit.model.handle, kit.textDecoder.handle, ptrs, lens, len(arrs), C.byref(st), C.byref(o), p,
+                                              len(prompt), ts, n, windowClipTime, -1 if maxWindowSeek is None else maxWindowSeek,
+                                              1 if chunkingStrategy == "vad" else 0,
+                                              C.byref(hooks) if (split_to_word_tokens is not None or native is not None) else None,
+                                              int(opts.bestOf or 0), int(opts.draftTokens or 0), C.byref(h)))
     try:
         ns, nt = lib.wk_transcription_segment_count(h), lib.wk_transcription_token_count(h)
         raw = (wk_segment * max(1, ns))()

@@ -51,6 +51,8 @@ class AudioStreamTranscriber:
             raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"bestOf={opts.bestOf} is not supported in streams")
         if opts.draftTokens:
             raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"draftTokens={opts.draftTokens} is not supported in streams")
+        if opts.biasPhrases is not None:
+            raise WhisperError(WK_ERR_INVALID_ARGUMENT, "biasPhrases is not supported in streams")
         self.kit, self.options, self.lib = kit, opts, kit.model.lib
         self.stateChangeCallback = stateChangeCallback
         prompt = kit.textDecoder.prefillDecoderInputs(opts if opts.usePrefillPrompt else None, kit.specialTokens)

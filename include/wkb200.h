@@ -422,6 +422,21 @@ void wk_bias_free(wk_bias* b);
  * attached the draft entry points and wk_streamer_round return WK_ERR_INVALID_ARGUMENT. */
 wk_status wk_session_set_bias(wk_session* s, const wk_bias* const* sets, int64_t n_sets);
 
+/* ---- top log-probs (DecodingOptions.topLogProbs): the k most likely tokens at every sampled position ----
+ * k in [0, 20] applies to the session's following calls; 0 (the default) turns it off.  At every position the loop sampled and
+ * appended, the sampler ranks the candidates its choice was made from: the filtered row over the range the draw uses (only the
+ * timestamp tokens when the timestamp rule wins), larger value first, ties to the lower id.  Each carries the log-prob its token would
+ * have been reported with: the filtered log-softmax at temperature 0, the log of the tempered probability before the top-k cut at
+ * temperature > 0, and with a bias set the model's unbiased values and ranking.  At temperature 0 without bias, entry 0 is the
+ * sampled token and its log-prob.  Forced prompt positions and the closing EOT (whose token log-prob is the 0 that finalize appends)
+ * get none.  Calls with beam_size > 1, draft_tokens, the stream stop rule and wk_streamer_create return WK_ERR_INVALID_ARGUMENT while
+ * k > 0, as does k outside [0, 20]. */
+wk_status wk_session_set_top_logprobs(wk_session* s, int32_t k);
+/* The pairs of one window of the session's last batched call (wk_transcribe_windows*, wk_decode_text*) for its result tokens [0, n):
+ * tokens / logprobs [n][k] with k the setting the call ran with, best first, padded with -1 / -inf (positions without candidates,
+ * fewer finite candidates than k, positions >= the result's n_tokens).  Nothing is written when the call ran with k = 0. */
+wk_status wk_session_top_logprobs(const wk_session* s, int32_t window, int32_t n, int32_t* tokens, float* logprobs);
+
 /* ---- multi-GPU edges (SURVEY section 8e): one process per GPU, windows sharded, weights replicated; NCCL only moves PCM out and
  * results back (grouped ncclSend / ncclRecv over NVLink).  NCCL is resolved at run time from the process; wk_comm_unique_id fails with
  * WK_ERR_MODELS_UNAVAILABLE if it is not there.  The 128-byte id from rank 0 reaches the other ranks by whatever the host uses for
@@ -498,6 +513,9 @@ int32_t wk_transcription_window_count(const wk_transcription* t);
 int64_t wk_transcription_token_count(const wk_transcription* t);
 wk_status wk_transcription_segments(const wk_transcription* t, wk_segment* segs, int32_t cap);
 wk_status wk_transcription_tokens(const wk_transcription* t, int32_t* tokens, float* logprobs, int64_t cap);
+/* wk_session_top_logprobs for every entry of wk_transcription_tokens: [token_count][k] pairs, k the session's topLogProbs setting when
+ * the call ran (cap: pairs the arrays hold, at least token_count * k); nothing when k was 0.  Refused with beam_size > 1 or draft_tokens. */
+wk_status wk_transcription_top_logprobs(const wk_transcription* t, int32_t* tokens, float* logprobs, int64_t cap);
 int32_t wk_transcription_word_count(const wk_transcription* t);
 wk_status wk_transcription_word(const wk_transcription* t, int32_t i, wk_word* out);   /* .segment indexes wk_transcription_segments */
 /* TranscriptionResult.language of one stream (TranscribeTask.swift:71,292,352): the language of the stream's last window (in stream time)

@@ -195,6 +195,8 @@ SYMBOLS = [
     ("wk_bias_create", I32, [PI32, PI32, I32, F32, I32, C.POINTER(P)]),
     ("wk_bias_free", None, [P]),
     ("wk_session_set_bias", I32, [P, C.POINTER(P), I64]),
+    ("wk_session_set_top_logprobs", I32, [P, I32]),
+    ("wk_session_top_logprobs", I32, [P, I32, I32, PI32, PF32]),
     ("wk_transcribe_windows", I32, [P, P, P, I64, I64, PI32, C.POINTER(wk_special_tokens), C.POINTER(wk_decode_opts),
                                     PI32, I32, C.POINTER(wk_decode_result)]),
     ("wk_comm_shard_bounds", None, [I64, I32, I32, PI64, PI64]),
@@ -224,6 +226,7 @@ SYMBOLS = [
     ("wk_transcription_token_count", I64, [P]),
     ("wk_transcription_segments", I32, [P, C.POINTER(wk_segment), I32]),
     ("wk_transcription_tokens", I32, [P, PI32, PF32, I64]),
+    ("wk_transcription_top_logprobs", I32, [P, PI32, PF32, I64]),
     ("wk_transcription_word_count", I32, [P]),
     ("wk_transcription_word", I32, [P, I32, C.POINTER(wk_word)]),
     ("wk_transcription_language", I32, [P, I32, PI32, PF32]),

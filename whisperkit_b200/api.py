@@ -28,6 +28,7 @@ from ._lib import (PROGRESS_FN, WK_DTYPE_BF16, WK_DTYPE_F16, WK_DTYPE_F32, WK_ER
                    wk_decode_result, wk_model_config, wk_model_info, wk_special_tokens)
 
 MAX_TOKEN_CONTEXT = 224  # Constants.maxTokenContext (Models.swift:1334)
+MAX_TOP_LOGPROBS = 20    # DecodingOptions.topLogProbs limit (OpenAI's top_logprobs)
 WINDOW_SAMPLES = 480000  # Constants.defaultWindowSamples (Models.swift:1457)
 FALLBACK_REASONS = {0: None, 1: "firstTokenLogProbThreshold", 2: "silence", 3: "compressionRatioThreshold",
                     4: "logProbThreshold"}
@@ -135,6 +136,11 @@ class DecodingOptions:
     # 2.0 default is not tuned on a real checkpoint.  Refused with draftTokens and in AudioStreamTranscriber
     biasPhrases: Optional[List[Union[str, List[int]]]] = None
     biasBoost: float = 2.0
+    # the k most likely tokens and their log-probs at every sampled position (DecodingResult.topLogProbs, TranscriptionSegment.topLogProbs):
+    # k in 0..20, 0 = off.  Ranked on the filtered row the choice was made from, with the normaliser of tokenLogProbs (the tempered one
+    # at temperature > 0; the model's own values under biasPhrases).  One value per call; refused with beamSize > 1, draftTokens and in
+    # AudioStreamTranscriber (C: wk_session_set_top_logprobs)
+    topLogProbs: int = 0
 
     @property
     def detectsLanguage(self) -> bool:
@@ -210,6 +216,9 @@ class DecodingResult:
     languageLogProb: Optional[float] = None
     language: Optional[str] = None
     noSpeechProb: float = 0.0   # DecodingOptions.computeNoSpeechProb; 0 where it was not computed, as in the reference
+    # DecodingOptions.topLogProbs: one {token: logprob} per tokenLogProbs entry, best first; empty for forced prompt positions and the
+    # closing EOT, and an empty list when the option is 0
+    topLogProbs: List[Dict[int, float]] = field(default_factory=list)
 
     @staticmethod
     def from_c(r: wk_decode_result) -> "DecodingResult":
@@ -247,6 +256,33 @@ def attach_no_speech_probs(results: List["DecodingResult"], probs: Sequence[floa
     for r, p in zip(results, probs):
         if isinstance(r, DecodingResult):
             r.noSpeechProb = 0.0 if math.isnan(p) else p
+
+
+def top_logprob_dicts(tokens: Sequence[int], logprobs: Sequence[float], n: int, k: int) -> List[Dict[int, float]]:
+    """The flat [n][k] pairs of wk_session_top_logprobs / wk_transcription_top_logprobs as one dict per position, best first; the -1
+    padding is dropped."""
+    out = []
+    for i in range(n):
+        d: Dict[int, float] = {}
+        for j in range(i * k, i * k + k):
+            if int(tokens[j]) >= 0:
+                d[int(tokens[j])] = float(logprobs[j])
+        out.append(d)
+    return out
+
+
+def attach_top_logprobs(lib, session, results: List["DecodingResult"], k: int) -> None:
+    """DecodingResult.topLogProbs of every result of the session's last batched call that ran with topLogProbs = k."""
+    if k == 0:
+        return
+    for w, r in enumerate(results):
+        if not isinstance(r, DecodingResult):
+            continue
+        n = len(r.tokens)
+        tok = (C.c_int32 * max(1, n * k))()
+        lp = (C.c_float * max(1, n * k))()
+        check(lib.wk_session_top_logprobs(session, w, n, tok, lp))
+        r.topLogProbs = top_logprob_dicts(tok, lp, n, k)
 
 
 def attach_languages(results: List["DecodingResult"], tokens: Sequence[int], logprobs: Sequence[float], tokenizer=None) -> None:
@@ -559,7 +595,8 @@ class TextDecoder:
         bo, keep = make_batch_opts(n, opts, prompt, callback, callbackEvery, None)
         res = (wk_decode_result * n)()
         draft = draft_tokens_of(opts)
-        with attached_bias(self.lib, self.handle, opts, specialTokens):
+        top = top_logprobs_of(opts)
+        with attached_bias(self.lib, self.handle, opts, specialTokens), top_logprobs_set(self.lib, self.handle, top):
             if draft:
                 check(self.lib.wk_decode_text_draft(self.handle, C.byref(st), C.byref(bo), draft, res))
             else:
@@ -567,6 +604,7 @@ class TextDecoder:
         out = [DecodingResult.from_c(r) for r in res]
         attach_languages(out, *session_languages(self.lib, self.handle, n))
         attach_no_speech_probs(out, session_no_speech_probs(self.lib, self.handle, n))
+        attach_top_logprobs(self.lib, self.handle, out, top)
         return out
 
     def detectLanguage(self, encoderOutput: Optional[DeviceTensor], specialTokens: SpecialTokens, allLanguageTokens: Sequence[int],
@@ -684,6 +722,31 @@ def draft_tokens_of(options) -> int:
     if len(draft) != 1:
         raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"draftTokens must be the same for every window of a call (got {sorted(draft)})")
     return draft.pop()
+
+
+def top_logprobs_of(options) -> int:
+    """The call's DecodingOptions.topLogProbs: one value in [0, 20] for every window."""
+    opt_list = list(options) if isinstance(options, (list, tuple)) else [options]
+    ks = {int(o.topLogProbs or 0) for o in opt_list}
+    if len(ks) != 1:
+        raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"topLogProbs must be the same for every window of a call (got {sorted(ks)})")
+    k = ks.pop()
+    if not 0 <= k <= MAX_TOP_LOGPROBS:
+        raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"topLogProbs {k} outside [0, {MAX_TOP_LOGPROBS}]")
+    return k
+
+
+@contextlib.contextmanager
+def top_logprobs_set(lib, session, k: int):
+    """Sets the session's topLogProbs to k for one call and back to 0 after it."""
+    if k == 0:
+        yield
+        return
+    check(lib.wk_session_set_top_logprobs(session, k))
+    try:
+        yield
+    finally:
+        check(lib.wk_session_set_top_logprobs(session, 0))
 
 
 def bias_phrase_tokens(phrases, tokenizer=None) -> List[List[int]]:
@@ -933,7 +996,9 @@ class WhisperKit:
         # the prompt of every window is built inside the library from that window's options (prefillDecoderInputs); decodeWithFallback
         # (TranscribeTask.swift:316-411) runs there too: a window whose DecodingFallback asks for it is decoded again at the next temperature
         draft = draft_tokens_of(opts)
-        with attached_bias(self.model.lib, self.textDecoder.handle, opts, self.specialTokens, self.tokenizer):
+        top = top_logprobs_of(opts)
+        with attached_bias(self.model.lib, self.textDecoder.handle, opts, self.specialTokens, self.tokenizer), \
+                top_logprobs_set(self.model.lib, self.textDecoder.handle, top):
             if draft:
                 check(self.model.lib.wk_transcribe_windows_draft(self.model.handle, self.textDecoder.handle, _ptr(a), n, stride, spw,
                                                                  C.byref(st), C.byref(bo), draft, res))
@@ -949,6 +1014,7 @@ class WhisperKit:
                 out.append(DecodingResult.from_c(r))
         attach_languages(out, *session_languages(self.model.lib, self.textDecoder.handle, n), tokenizer=self.tokenizer)
         attach_no_speech_probs(out, session_no_speech_probs(self.model.lib, self.textDecoder.handle, n))
+        attach_top_logprobs(self.model.lib, self.textDecoder.handle, out, top)
         return out
 
     def _transcribe_paths(self, paths: Sequence[str], decodeOptions, chunkingStrategy: Optional[str]):

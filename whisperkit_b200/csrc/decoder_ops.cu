@@ -819,9 +819,10 @@ __device__ __forceinline__ float tempered_prob(float x, float inv_t, float zmax,
 // temperature 0 = argmax; > 0 = logits / T, softmax over the whole (filtered) range, top-k, multinomial draw inside the top-k mass,
 // logprob = log softmax prob of the draw (TokenSampler.swift:57-73 / :140-180).  The reference draws with Float.random
 // (non-deterministic); here the draw is Philox(seed, subsequence, offset).  Returns the token in .i (out of [0, V) if the row has no
-// finite logit) and its log-prob in .v; srow is modified at T > 0.
+// finite logit) and its log-prob in .v; srow is modified at T > 0.  z_out (T > 0, may be nullptr): the tempered normaliser
 __device__ __forceinline__ ArgMax sample_row(float* srow, int lo, int V, float m, float lse, float temperature, int top_k, uint64_t seed,
-                                             unsigned long long subsequence, unsigned long long offset, float* scratch, ArgMax* sarg) {
+                                             unsigned long long subsequence, unsigned long long offset, float* scratch, ArgMax* sarg,
+                                             float* z_out = nullptr) {
     const int tid = threadIdx.x;
     ArgMax best;
     if (temperature == 0.f) {
@@ -832,6 +833,7 @@ __device__ __forceinline__ ArgMax sample_row(float* srow, int lo, int V, float m
     const float inv_t = 1.f / temperature;
     const float zmax = m * inv_t;
     const float z = tempered_sum(srow, lo, V, inv_t, zmax, scratch);
+    if (z_out) *z_out = z;
     __shared__ float topv[32];
     __shared__ int topi[32];
     const int k = top_k < 1 ? 1 : (top_k > 32 ? 32 : top_k);
@@ -939,11 +941,62 @@ __device__ int bias_advance(const BiasSet& B, uint8_t* m, int v, float* scratch)
     return (int)block_max((float)g, scratch);
 }
 
+// ---- DecodingOptions.topLogProbs (tests/top_logprobs_ref.py is the specification): the k best candidates of the filtered row, ordered
+// like block_argmax_row (larger value first, ties to the lower index), in one pass over the row.  Each warp keeps a register top-k of
+// its threads' strided slices, entry j in lane j, and warp 0 then merges the 32 warp lists with the same insertion.  (A list per
+// thread would need 2k registers of the 64 that a 1024-thread CTA allows.)
+__device__ __forceinline__ bool top_better(float av, int ai, float bv, int bi) { return av > bv || (av == bv && ai < bi); }
+
+// offers every lane's (x, i) to the warp's list (lv, li) of k entries; only finite values enter.  Called by whole warps
+__device__ __forceinline__ void warp_top_offer(float x, int i, int k, float& lv, int& li) {
+    const int lane = threadIdx.x & 31;
+    const float tv = __shfl_sync(0xffffffffu, lv, k - 1);
+    const int ti = __shfl_sync(0xffffffffu, li, k - 1);
+    unsigned cand = __ballot_sync(0xffffffffu, x > -INFINITY && top_better(x, i, tv, ti));
+    while (cand) {
+        const int src = __ffs(cand) - 1;
+        cand &= cand - 1;
+        const float cv = __shfl_sync(0xffffffffu, x, src);
+        const int ci = __shfl_sync(0xffffffffu, i, src);
+        // the entries better than the candidate keep their lanes, the others move down one lane and the last falls off
+        const int pos = __popc(__ballot_sync(0xffffffffu, lane < k && top_better(lv, li, cv, ci)));
+        const float uv = __shfl_up_sync(0xffffffffu, lv, 1);
+        const int ui = __shfl_up_sync(0xffffffffu, li, 1);
+        if (pos < k) {
+            if (lane == pos) { lv = cv; li = ci; }
+            else if (lane > pos) { lv = uv; li = ui; }
+        }
+    }
+}
+
+// the k best entries of srow[lo, V) (only read) into tv / ti [0, k), padded with (-inf, INT_MAX); tv / ti: 32 * k entries of shared
+// memory.  Thread j < k (lane j of warp 0) writes entry j
+__device__ void block_top_row(const float* srow, int lo, int V, int k, float* tv, int* ti) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    float lv = -INFINITY;
+    int li = 0x7fffffff;
+    for (int i0 = lo + (tid & ~31); i0 < V; i0 += kSamplerThreads) {   // thread tid sees srow[lo + tid + j * kSamplerThreads]
+        const int i = i0 + lane;
+        warp_top_offer(i < V ? srow[i] : -INFINITY, i, k, lv, li);
+    }
+    if (lane < k) { tv[warp * k + lane] = lv; ti[warp * k + lane] = li; }
+    __syncthreads();
+    if (warp != 0) return;
+    lv = -INFINITY;
+    li = 0x7fffffff;
+    const int n = (kSamplerThreads / 32) * k;
+    for (int c = 0; c < n; c += 32) warp_top_offer(c + lane < n ? tv[c + lane] : -INFINITY, c + lane < n ? ti[c + lane] : 0, k, lv, li);
+    __syncwarp();
+    if (lane < k) { tv[lane] = lv; ti[lane] = li; }
+}
+
+// kTop: the variant with the DecodingOptions.topLogProbs pass (SamplerParams.top_n > 0); the other one is the sampler without it
+template <bool kTop>
 __global__ void __launch_bounds__(kSamplerThreads)
 sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerParams p, DecodeState st,
                const int32_t* __restrict__ tokens_in, int ld_tokens, const int32_t* __restrict__ n_tokens_in,
                int32_t* __restrict__ token_out, float* __restrict__ logprob_out, float* __restrict__ filtered_out) {
-    extern __shared__ __align__(16) float srow[];  // [V]
+    extern __shared__ __align__(16) float srow[];  // [V]; kTop: then the candidate lists [32 * 20] values, [32 * 20] ids, the position
     __shared__ float scratch[32];
     __shared__ int sflag[8];     // 0: ts filter active, 1: lo0, 2: hi0 (interval A), 3: lo1, 4: hi1 (interval B), 5: blank active
     __shared__ ArgMax sarg[32];
@@ -1143,6 +1196,16 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
     // phrase bonus joins the filtered row after every filter.  The choice sees it; the reported log-probs stay the model's: a chosen
     // token's filtered value is its raw logit, so they come from `row`, against the unbiased normaliser
     const bool biased = loop_mode && st.bias_pool != nullptr && R.bias_n > 0 && st.steps[b] >= R.prompt_len - 1;
+    // DecodingOptions.topLogProbs: a position the row may record ranks its candidates here, on the filtered row before the bonus or the
+    // draw change it.  The values are raw logits until they are written, against the normaliser of the position's reported log-prob
+    float* top_v = srow + V;
+    int* top_i = (int*)(top_v + 32 * kMaxTopLogprobs);
+    int* top_pos = top_i + 32 * kMaxTopLogprobs;
+    bool top = false;
+    if constexpr (kTop) {
+        top = loop_mode && R.mode != kRowBeam && st.steps[b] >= R.prompt_len - 1;
+        if (top) block_top_row(srow, lo, V, p.top_n, top_v, top_i);
+    }
     float m_draw = ts_wins ? mts : mall;
     float z_unbiased = 0.f;
     int bias_G = 0;
@@ -1173,14 +1236,16 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
         return;
     }
     // the row's draw: Philox(seed, row, step) at temperature > 0 (row: the slot in a draft call, whose windows sample on row 0 only)
+    float z_draw = 0.f;
     const ArgMax best = sample_row(srow, lo, V, m_draw, lse, R.temperature, R.top_k, R.seed, (unsigned long long)(b / max(1, p.rng_div)),
-                                   (unsigned long long)(loop_mode ? st.steps[b] : n_tok), scratch, sarg);
+                                   (unsigned long long)(loop_mode ? st.steps[b] : n_tok), scratch, sarg, kTop && top ? &z_draw : nullptr);
     float lp_sampled = best.v;
     if (biased && best.i >= 0 && best.i < V)
         lp_sampled = R.temperature == 0.f ? row[best.i] - lse
                                           : logf(tempered_prob(row[best.i], 1.f / R.temperature, (ts_wins ? mts : mall) * (1.f / R.temperature), z_unbiased));
     if (tid == 0) s_adv = -1;
     if (tid == 0) {
+        if constexpr (kTop) *top_pos = -1;
         int tok = best.i;
         float lp = lp_sampled;
         // a row with no finite logit (every token masked, or a NaN from upstream) has no argmax: end the window there and flag it instead
@@ -1206,8 +1271,25 @@ sampler_kernel(const float* __restrict__ logits, long long ld_logits, SamplerPar
                     st.logprobs[b * kMaxCtx + n_tok] = lp;
                     st.n_tokens[b] = n_tok + 1;
                     if (biased) s_adv = tok;
+                    if constexpr (kTop) *top_pos = n_tok;
                 }
                 if (step + 1 >= R.max_steps) st.done[b] = 1;   // loop bound min(sampleLength, 223) reached (TextDecoder.swift:566)
+            }
+        }
+    }
+    if constexpr (kTop) {   // the candidates of an appended token at its position, with the normaliser of its log-prob (unbiased)
+        if (top) {
+            __syncthreads();
+            const int pos = *top_pos;
+            if (pos >= 0 && tid < p.top_n) {
+                const float v = top_v[tid];
+                const bool ok = v > -INFINITY;
+                const float lp = R.temperature == 0.f ? v - lse
+                                                      : logf(tempered_prob(v, 1.f / R.temperature, (ts_wins ? mts : mall) * (1.f / R.temperature),
+                                                                           biased ? z_unbiased : z_draw));
+                const long long at = ((long long)b * kMaxCtx + pos) * p.top_n + tid;
+                p.top_tok[at] = ok ? top_i[tid] : -1;
+                p.top_lp[at] = ok ? lp : -INFINITY;
             }
         }
     }
@@ -1532,15 +1614,21 @@ wk_status draft_accept(DecodeState st, int32_t* anc, DraftRound R, cudaStream_t 
 wk_status sampler_filter_sample(const float* logits, int64_t ld_logits, SamplerParams p, DecodeState st, const int32_t* tokens,
                                 int ld_tokens, const int32_t* n_tokens, int32_t* token_out, float* logprob_out,
                                 float* filtered_out, int B, cudaStream_t stream) {
-    const size_t smem = (size_t)p.vocab * sizeof(float);
-    if (smem > 220 * 1024) { set_error("sampler: vocab %d too large for the shared-memory row", p.vocab); return WK_ERR_INVALID_ARGUMENT; }
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(sampler_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(sampler): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
-        attr_set = true;
+    const bool top = p.top_n > 0;
+    if (top && (p.top_n > kMaxTopLogprobs || !p.loop_mode || !p.top_tok || !p.top_lp)) {
+        set_error("sampler: top_n %d needs the decode loop, its buffers and top_n <= %d", p.top_n, kMaxTopLogprobs);
+        return WK_ERR_INVALID_ARGUMENT;
     }
-    launch_k(sampler_kernel, dim3(B), dim3(kSamplerThreads), smem, stream, 8, logits, (long long)ld_logits, p, st, tokens, ld_tokens,
+    const size_t smem = (size_t)p.vocab * sizeof(float) + (top ? (2 * 32 * kMaxTopLogprobs + 1) * sizeof(float) : 0);
+    if (smem > 220 * 1024) { set_error("sampler: vocab %d too large for the shared-memory row", p.vocab); return WK_ERR_INVALID_ARGUMENT; }
+    static bool attr_set[2] = {false, false};
+    auto kernel = top ? sampler_kernel<true> : sampler_kernel<false>;
+    if (!attr_set[top]) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(sampler): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
+        attr_set[top] = true;
+    }
+    launch_k(kernel, dim3(B), dim3(kSamplerThreads), smem, stream, 8, logits, (long long)ld_logits, p, st, tokens, ld_tokens,
              n_tokens, token_out, logprob_out, filtered_out);
     count_launch();
     cudaError_t e = cudaGetLastError();

@@ -221,6 +221,8 @@ constexpr int kLangLead = 2, kLangLeadRan = 3;
 // A bias set: up to 256 phrases of 1..16 token ids each, 1024 tokens in all.  Its pool record is [n] descriptors (start | len << 16),
 // [total] phrase tokens, [total] failure links (f(k) for k = 1..len of a phrase at its start + k - 1)
 constexpr int kMaxBiasPhrases = 256, kMaxBiasLen = 16, kMaxBiasTotal = 1024;
+// DecodingOptions.topLogProbs: k in [0, 20] (OpenAI's top_logprobs limit)
+constexpr int kMaxTopLogprobs = 20;
 
 // Beam search (SURVEY 8f row 2; semantics restated from openai/whisper BeamSearchDecoder in oracle/beam_ref.py - the reference's
 // BeamSearchTokenSampler is a fatalError stub, TokenSampler.swift:254-290).  Decode rows come in groups of `group` consecutive rows per
@@ -253,6 +255,9 @@ struct SamplerParams {
     BeamState beam;         // loop mode: rows with RowParams.mode == kRowBeam only rank candidates; beam_update() does their bookkeeping
     int rng_div;            // loop mode: decode rows per Philox subsequence (a draft call's G, so that row 0 of slot q draws as row q of a
                             // draft-less call); 0 or 1 = every row its own
+    // loop mode, DecodingOptions.topLogProbs: the top_n best (token, log-prob) candidates of every sampled position, [rows][224][top_n]
+    // at the position DecodeState.logprobs uses, best first, padded with (-1, -inf); top_n = 0: off, the sampler has no top-k pass
+    int32_t* top_tok; float* top_lp; int top_n;
     // stateless mode only
     int sample_begin_ts, sample_begin_blank, n_suppress;
     float temperature; int top_k; uint64_t seed;
@@ -380,5 +385,6 @@ wk_status transcribe_windows_stop(wk_model* m, wk_session* s, const float* pcm_h
 // rule, set i for window i or set 0 for every window)
 int64_t session_bias_sets(const wk_session* s);
 void session_bias_map(wk_session* s, std::vector<int> map);
+int session_top_logprobs(const wk_session* s);   // the k of wk_session_set_top_logprobs
 
 }  // namespace wk

@@ -340,6 +340,11 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
     const int64_t n_bias = session_bias_sets(s);
     if (n_bias > 1 && n_bias != n_streams) { set_error("%lld bias sets attached for %d streams (1 or one per stream)", (long long)n_bias, n_streams); return WK_ERR_INVALID_ARGUMENT; }
     const bool per_stream_bias = n_bias > 1;
+    const int top_k = session_top_logprobs(s);
+    if (top_k > 0 && (o->beam_size > 1 || draft_tokens > 0 || stop)) {
+        set_error("topLogProbs %d does not combine with beam search, draft_tokens or streams", top_k);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
     for (Unit& u : units) {
         // a clip is live while seek < clipEnd - windowPadding (TranscribeTask.swift:118) and, as a guard the reference lacks (it would
         // pad a negative-length window), while the seek is still inside the audio
@@ -351,6 +356,7 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         if (!u.done && u.seek < u.base) { set_error("seek loop: stream %d seeks to sample %lld before its first held sample %lld", u.stream, (long long)u.seek, (long long)u.base); return WK_ERR_INVALID_ARGUMENT; }
     }
     std::unique_ptr<wk_transcription> T(new wk_transcription());
+    T->top_k = top_k;
     T->lang.assign(n_streams, -1); T->lang_logprob.assign(n_streams, 0.f); T->lang_at.assign(n_streams, -1);
     // One round = the next window of EVERY unfinished unit (up to kRoundCap): the window scheduler behind wk_transcribe_windows keeps the
     // session's decode slots full and runs the mel + encoder pass of the following windows under the running decode, so a round is not
@@ -366,6 +372,8 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
     std::vector<int> active;
     std::vector<std::vector<int32_t>> unit_tokens(units.size());
     std::vector<std::vector<float>> unit_lps(units.size());
+    std::vector<std::vector<int32_t>> unit_top_tok(units.size());
+    std::vector<std::vector<float>> unit_top_lp(units.size());
     const int n_threads = (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
     for (;;) {
         active.clear();
@@ -411,6 +419,15 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
             rc = wk_session_no_speech_probs(s, 0, (int32_t)active.size(), nsp.data());
             if (rc != WK_OK) return rc;
             for (float& v : nsp) if (isnan(v)) v = 0.f;
+        }
+        // top log-probs per window: [n_tokens][top_k], beside the result's tokens
+        std::vector<std::vector<int32_t>> top_tok(top_k > 0 ? active.size() : 0);
+        std::vector<std::vector<float>> top_lp(top_tok.size());
+        for (size_t k = 0; k < top_tok.size(); ++k) {
+            top_tok[k].resize((size_t)std::max(res[k].n_tokens, 1) * top_k);
+            top_lp[k].resize(top_tok[k].size());
+            rc = wk_session_top_logprobs(s, (int32_t)k, res[k].n_tokens, top_tok[k].data(), top_lp[k].data());
+            if (rc != WK_OK) return rc;
         }
         const int cols = info.n_audio_ctx;
         if (o->word_timestamps) {   // every window's alignment rows back in one burst (Float16, as the reference's alignmentWeights)
@@ -479,6 +496,11 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
                     unit_tokens[active[k]].push_back(r.tokens[sg.token_offset + t]);
                     unit_lps[active[k]].push_back(r.token_logprobs[sg.token_offset + t]);
                 }
+                if (top_k > 0) {
+                    const size_t a = (size_t)sg.token_offset * top_k, b = a + (size_t)sg.n_tokens * top_k;
+                    unit_top_tok[active[k]].insert(unit_top_tok[active[k]].end(), top_tok[k].begin() + a, top_tok[k].begin() + b);
+                    unit_top_lp[active[k]].insert(unit_top_lp[active[k]].end(), top_lp[k].begin() + a, top_lp[k].begin() + b);
+                }
                 sg.token_offset = base;
                 sg.stream = u.stream;
                 u.segs.push_back(sg);
@@ -501,6 +523,8 @@ wk_status wk::seek_loop_units(wk_model* m, wk_session* s, std::vector<Unit>& uni
         const int64_t base = (int64_t)T->tokens.size();
         T->tokens.insert(T->tokens.end(), unit_tokens[i].begin(), unit_tokens[i].end());
         T->logprobs.insert(T->logprobs.end(), unit_lps[i].begin(), unit_lps[i].end());
+        T->top_tok.insert(T->top_tok.end(), unit_top_tok[i].begin(), unit_top_tok[i].end());
+        T->top_lp.insert(T->top_lp.end(), unit_top_lp[i].begin(), unit_top_lp[i].end());
         const int seg_base = (int)T->segments.size();
         for (OutWord w : u.words) {
             w.start += seek_time; w.end += seek_time; w.segment += seg_base;
@@ -533,6 +557,17 @@ wk_status wk_transcription_tokens(const wk_transcription* t, int32_t* tokens, fl
     if (!t || cap < (int64_t)t->tokens.size()) { set_error("wk_transcription_tokens: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (tokens && !t->tokens.empty()) memcpy(tokens, t->tokens.data(), t->tokens.size() * 4);
     if (logprobs && !t->logprobs.empty()) memcpy(logprobs, t->logprobs.data(), t->logprobs.size() * 4);
+    return WK_OK;
+}
+wk_status wk_transcription_top_logprobs(const wk_transcription* t, int32_t* tokens, float* logprobs, int64_t cap) {
+    if (!t || cap < (int64_t)t->top_tok.size() || (!t->top_tok.empty() && (!tokens || !logprobs))) {
+        set_error("wk_transcription_top_logprobs: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    if (!t->top_tok.empty()) {
+        memcpy(tokens, t->top_tok.data(), t->top_tok.size() * 4);
+        memcpy(logprobs, t->top_lp.data(), t->top_lp.size() * 4);
+    }
     return WK_OK;
 }
 int32_t wk_transcription_word_count(const wk_transcription* t) { return t ? (int32_t)t->words.size() : 0; }

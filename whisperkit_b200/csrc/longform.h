@@ -19,6 +19,10 @@ struct wk_transcription {
     std::vector<OutWord> words;   // .segment indexes `segments`
     std::vector<int32_t> tokens;
     std::vector<float> logprobs;
+    // DecodingOptions.topLogProbs: top_k pairs per entry of `tokens` (padded with -1 / -inf), empty when top_k = 0
+    int top_k = 0;
+    std::vector<int32_t> top_tok;
+    std::vector<float> top_lp;
     int windows = 0;
     // per stream: the detected language of its latest window (in stream time) that detected one, and where that window started
     std::vector<int32_t> lang; std::vector<float> lang_logprob; std::vector<int64_t> lang_at;

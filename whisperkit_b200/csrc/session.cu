@@ -101,6 +101,13 @@ struct wk_session {
     std::vector<int> bias_map;
     int32_t* h_bias_acc = nullptr;
     const int32_t* graph_bias = nullptr;
+    // DecodingOptions.topLogProbs (wk_session_set_top_logprobs): the setting for the next calls and the k of the running call; the
+    // sampler's pairs [S][224][k] on the device (allocated for k = 20 on first use) and their pinned readback; per window of the last
+    // call, the pairs of its result tokens [n_tokens][k] (top_store_k = the call's k)
+    int top_k = 0, top_n = 0, graph_top = 0, top_store_k = 0;
+    int32_t *top_tok = nullptr, *h_top_tok = nullptr; float *top_lp = nullptr, *h_top_lp = nullptr;
+    std::vector<std::vector<int32_t>> win_top_tok;
+    std::vector<std::vector<float>> win_top_lp;
 };
 
 // a phrase set as wk_bias_create validated it: its pool record (kernels.h) and boost
@@ -133,6 +140,7 @@ AudioWs** session_audio_ws(wk_session* s) { return &s->audio; }
 cudaStream_t session_stream(wk_session* s) { return s->stream; }
 int session_device(wk_session* s) { return s->m->device; }
 int64_t session_bias_sets(const wk_session* s) { return (int64_t)s->bias_sets.size(); }
+int session_top_logprobs(const wk_session* s) { return s->top_k; }
 void session_bias_map(wk_session* s, std::vector<int> map) { s->bias_map = std::move(map); }
 
 // ---------------------------------------------------------------------------------------------- decoder schedule
@@ -269,6 +277,7 @@ static SamplerParams loop_sampler_params(wk_session* s, const wk_special_tokens*
     p.detect_tokens = s->lang_dev;
     p.beam = s->bs;
     p.rng_div = s->draft_k > 0 ? s->bs.group : 1;
+    p.top_tok = s->top_tok; p.top_lp = s->top_lp; p.top_n = s->top_n;
     return p;
 }
 
@@ -312,9 +321,10 @@ static int stop_rule_index(const StopRule& rule, Deflater& z, const int32_t* tok
     return -1;
 }
 
-// finalisation of one window on the host: finalize + slicing + averages (TextDecoder.swift:776-853)
-static void finalize_result(wk_decode_result& r, const int32_t* tokens, const float* lps, int n_tok, int steps, int first_low,
-                            const wk_special_tokens* st, const wk_decode_opts* o, float temperature, float no_speech_prob, Deflater& z) {
+// finalisation of one window on the host: finalize + slicing + averages (TextDecoder.swift:776-853).  Returns the history index of the
+// result's first token
+static size_t finalize_result(wk_decode_result& r, const int32_t* tokens, const float* lps, int n_tok, int steps, int first_low,
+                              const wk_special_tokens* st, const wk_decode_opts* o, float temperature, float no_speech_prob, Deflater& z) {
     memset(&r, 0, sizeof(r));
     std::vector<int32_t> seg(tokens, tokens + n_tok);
     std::vector<float> slp(lps, lps + n_tok);
@@ -347,6 +357,7 @@ static void finalize_result(wk_decode_result& r, const int32_t* tokens, const fl
     else if (o->has_no_speech_threshold && no_speech_prob > o->no_speech_threshold) { r.needs_fallback = 0; r.fallback_reason = 2; }
     else if (o->has_compression_ratio_threshold && r.compression_ratio > o->compression_ratio_threshold) { r.needs_fallback = 1; r.fallback_reason = 3; }
     else if (o->has_logprob_threshold && r.avg_logprob < o->logprob_threshold) { r.needs_fallback = 1; r.fallback_reason = 4; }
+    return start;
 }
 
 // prefillDecoderInputs (TextDecoder.swift:163-216)
@@ -427,11 +438,12 @@ static wk_status run_steps(wk_session* s, const wk_special_tokens* st, int n, bo
     // and on the bias pool the sampler reads (nullptr: no set attached)
     const int beam_key = (std::max(1, s->bs.group) * 16 + std::max(1, s->bs.beam)) * 16 + s->bs.max_candidates;
     const bool stale = s->graph_batch != s->batch || s->graph_align != s->align_on || s->graph_beam != beam_key ||
-                       s->graph_draft != s->draft_k || s->graph_bias != s->st.bias_pool || memcmp(&s->graph_st, st, sizeof(*st)) != 0;
+                       s->graph_draft != s->draft_k || s->graph_bias != s->st.bias_pool || s->graph_top != s->top_n ||
+                       memcmp(&s->graph_st, st, sizeof(*st)) != 0;
     if (stale) {
         drop_graphs(s);
         s->graph_batch = s->batch; s->graph_align = s->align_on; s->graph_st = *st; s->graph_beam = beam_key; s->graph_draft = s->draft_k;
-        s->graph_bias = s->st.bias_pool;
+        s->graph_bias = s->st.bias_pool; s->graph_top = s->top_n;
     }
     cudaGraphExec_t& exec = check_done ? s->graph_exec : s->graph_exec_live;
     if (!exec) {
@@ -553,6 +565,18 @@ static wk_status ensure_draft(wk_session* s) {
     return WK_OK;
 }
 
+// the sampler's top-k pairs and their readback (DecodingOptions.topLogProbs), sized for k = 20: their pointers never change
+static wk_status ensure_top(wk_session* s) {
+    if (s->top_tok) return WK_OK;
+    const size_t n = (size_t)s->max_batch * kKvMaxLen * kMaxTopLogprobs;
+    Buffers& b = s->mem;
+    WK_CHECK(b.dmalloc(&s->top_tok, n));
+    WK_CHECK(b.dmalloc(&s->top_lp, n));
+    WK_CHECK(b.pinned(&s->h_top_tok, n));
+    WK_CHECK(b.pinned(&s->h_top_lp, n));
+    return WK_OK;
+}
+
 // One window as the call decodes it: its prompt, the index of the prompt's first <|startoftranscript|> (-1: none) and whether the window
 // detects its language in the loop
 struct WindowPlan { const int32_t* p = nullptr; int np = 0, sot = -1; bool detects = false; };
@@ -621,6 +645,11 @@ static wk_status plan_call(wk_session* s, const CoreArgs& a, CallPlan& p) {
         return WK_ERR_INVALID_ARGUMENT;
     }
     if (a.stop && (G != 1 || a.stop->window < 1)) { set_error("the stream stop rule needs single-row windows and a check window >= 1"); return WK_ERR_INVALID_ARGUMENT; }
+    // top log-probs: the rows of greedy, sampling and best-of windows (a beam's history is reordered through its cache ancestry)
+    if (s->top_k > 0 && (beam > 1 || draft > 0 || a.stop)) {
+        set_error("topLogProbs %d does not combine with beam search, draft_tokens or streams", s->top_k);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
     if (beam > 1) {
         const float patience = bo->opts[0].beam_patience > 0.f ? bo->opts[0].beam_patience : 1.f;
         p.max_cand = (int)((float)beam * patience);                                  // TokenSampler.swift:266
@@ -713,6 +742,9 @@ static wk_status plan_call(wk_session* s, const CoreArgs& a, CallPlan& p) {
     s->win_lang.assign((size_t)n, -1);
     s->win_lang_logprob.assign((size_t)n, 0.f);
     s->win_no_speech.assign((size_t)n, NAN);
+    s->win_top_tok.assign((size_t)n, {});
+    s->win_top_lp.assign((size_t)n, {});
+    s->top_store_k = s->top_k;
     if (a.pcm && a.stride < kWindowSamples && !a.spw) { set_error("wk_transcribe_windows: stride < 480000 requires samples_per_window"); return WK_ERR_AUDIO_PROCESSING_FAILED; }
     if (!bo->status)
         for (int64_t w = 0; w < n; ++w) if (p.status[w] != WK_OK) { set_error("%s", p.first_err.c_str()); return p.status[w]; }
@@ -1009,6 +1041,8 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
     s->bs.beam = beam; s->bs.max_candidates = p.max_cand; s->bs.group = G; s->bs.use_anc = beam > 1 || p.draft > 0;
     s->draft_k = p.draft;
     s->st.bias_pool = p.bias_of.empty() ? nullptr : s->bias_pool;
+    s->top_n = s->top_k;
+    if (s->top_n > 0) WK_CHECK(ensure_top(s));
     WK_CHECK(upload_plan(s, p));
     s->align_on = p.any_words;
     s->win_align_lp.clear();   // the log-probs belong to the last align call only
@@ -1060,6 +1094,8 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
         WK_CHECK(read_back(s, p));
         feed.collect(true);
         // (D) retire ended windows; progress callback / early stop for the live ones
+        struct TopCopy { int64_t w; int row; size_t start; int np, n; };
+        std::vector<TopCopy> top_copies;   // returned windows whose top log-probs come back after the loop
         for (int q = 0; q < Brun; ++q) {
             const int w = slots.window[q];
             if (w < 0) continue;
@@ -1102,8 +1138,8 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             // beam search: every beam of the window is the same forced copy through the prefill, so row r0 holds the value
             const float nsp = o.compute_no_speech_prob ? s->h_no_speech[r0] : NAN;
             wk_decode_result r;
-            finalize_result(r, ch.tok, ch.lp, ch.n, stop_at >= 0 ? stop_at : s->h_steps[ch.row], s->h_first_low[ch.row], a.st, &o, temperature,
-                            isnan(nsp) ? 0.f : nsp, z);
+            const size_t start = finalize_result(r, ch.tok, ch.lp, ch.n, stop_at >= 0 ? stop_at : s->h_steps[ch.row], s->h_first_low[ch.row], a.st,
+                                                 &o, temperature, isnan(nsp) ? 0.f : nsp, z);
             int err_row = -1;                         // a row of the rung without a finite logit fails the window
             for (int j = 0; j < active && err_row < 0; ++j) if (s->h_error[r0 + j]) err_row = r0 + j;
             if (err_row >= 0) {
@@ -1117,6 +1153,13 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
                 a.results[w] = r;
                 if (p.any_detect) { s->win_lang[w] = s->h_lang_token[r0]; s->win_lang_logprob[w] = s->h_lang_logprob[r0]; }   // the returned rung's
                 s->win_no_speech[w] = nsp;
+                const int np = p.win[w].np;
+                if (s->top_n > 0 && ch.n > np) {   // the sampled positions [np, n) of the returned row, before a re-admission reuses it
+                    const size_t off = ((size_t)ch.row * kKvMaxLen + np) * s->top_n, cnt = (size_t)(ch.n - np) * s->top_n;
+                    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_top_tok + off, s->top_tok + off, cnt * 4, cudaMemcpyDeviceToHost, s->stream));
+                    WK_CUDA_CHECK(cudaMemcpyAsync(s->h_top_lp + off, s->top_lp + off, cnt * 4, cudaMemcpyDeviceToHost, s->stream));
+                }
+                if (s->top_n > 0) top_copies.push_back(TopCopy{w, ch.row, start, np, ch.n});
             }
             if (s->align_on && p.status[w] == WK_OK && stop_at >= 0)   // rows of the steps run past the stopping token: the reference never ran them
                 WK_CUDA_CHECK(cudaMemsetAsync((char*)s->align_w + ((size_t)ch.row * kKvMaxLen + stop_at + 1) * T * 2, 0,
@@ -1127,6 +1170,22 @@ static wk_status transcribe_core(wk_session* s, const CoreArgs& a) {
             slots.window[q] = -1;
             --slots.live;
             ++finished;
+        }
+        if (!top_copies.empty()) {
+            WK_CUDA_CHECK(cudaStreamSynchronize(s->stream));
+            const int k = s->top_n;
+            for (const TopCopy& c : top_copies) {   // result token i is history entry start + i; forced entries and the closing EOT stay padded
+                const int nr = a.results[c.w].n_tokens;
+                std::vector<int32_t>& tt = s->win_top_tok[c.w];
+                std::vector<float>& tl = s->win_top_lp[c.w];
+                tt.assign((size_t)nr * k, -1);
+                tl.assign((size_t)nr * k, -INFINITY);
+                for (int t = std::max<int>(c.np, (int)c.start); t < c.n && t - (int)c.start < nr; ++t) {
+                    const size_t src = ((size_t)c.row * kKvMaxLen + t) * k, dst = (size_t)(t - c.start) * k;
+                    memcpy(tt.data() + dst, s->h_top_tok + src, (size_t)k * 4);
+                    memcpy(tl.data() + dst, s->h_top_lp + src, (size_t)k * 4);
+                }
+            }
         }
         WK_CHECK(slots.flush());   // ladder re-admissions
     }
@@ -1488,6 +1547,27 @@ wk_status wk_session_set_bias(wk_session* s, const wk_bias* const* sets, int64_t
     }
     s->bias_sets = std::move(slots);
     s->bias_map.clear();
+    return WK_OK;
+}
+
+wk_status wk_session_set_top_logprobs(wk_session* s, int32_t k) {
+    if (!s || k < 0 || k > kMaxTopLogprobs) { set_error("wk_session_set_top_logprobs: k %d outside [0, %d]", k, kMaxTopLogprobs); return WK_ERR_INVALID_ARGUMENT; }
+    s->top_k = k;
+    return WK_OK;
+}
+
+wk_status wk_session_top_logprobs(const wk_session* s, int32_t window, int32_t n, int32_t* tokens, float* logprobs) {
+    if (!s || window < 0 || (size_t)window >= s->win_top_tok.size() || n < 0 || (n > 0 && s->top_store_k > 0 && (!tokens || !logprobs))) {
+        set_error("wk_session_top_logprobs: window %d / %d tokens outside the last call's %zu windows", window, n, s ? s->win_top_tok.size() : (size_t)0);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    const size_t want = (size_t)n * s->top_store_k;
+    const std::vector<int32_t>& tt = s->win_top_tok[window];
+    const std::vector<float>& tl = s->win_top_lp[window];
+    for (size_t i = 0; i < want; ++i) {
+        tokens[i] = i < tt.size() ? tt[i] : -1;
+        logprobs[i] = i < tl.size() ? tl[i] : -INFINITY;
+    }
     return WK_OK;
 }
 

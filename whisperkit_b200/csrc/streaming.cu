@@ -176,6 +176,7 @@ wk_status wk_streamer_create(wk_model* m, wk_session* s, const wk_special_tokens
                              int32_t n_prompt, const wk_stream_config* cfg, const wk_tokenizer_hooks* hooks, wk_streamer** out) {
     if (!m || !s || !st || !o || !prompt || n_prompt < 1 || !cfg || !out) { set_error("wk_streamer_create: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
     if (o->beam_size > 1) { set_error("wk_streamer_create: beam search is not supported in streams (beam_size %d)", o->beam_size); return WK_ERR_INVALID_ARGUMENT; }
+    if (session_top_logprobs(s) > 0) { set_error("wk_streamer_create: topLogProbs is not supported in streams"); return WK_ERR_INVALID_ARGUMENT; }
     if (o->word_timestamps && (!hooks || !hooks->split_to_word_tokens)) { set_error("wk_streamer_create: wordTimestamps needs the tokenizer's split_to_word_tokens hook"); return WK_ERR_INVALID_ARGUMENT; }
     if (cfg->required_segments_for_confirmation < 0 || cfg->compression_check_window < 1) {
         set_error("wk_streamer_create: required_segments_for_confirmation %d must be >= 0 and compression_check_window %d >= 1",

@@ -4,14 +4,14 @@ libwkb200.so (csrc/longform.cu); everything except `transcribe_streams` works wi
 from __future__ import annotations
 
 import ctypes as C
-from dataclasses import dataclass
-from typing import List, Optional, Sequence, Tuple
+from dataclasses import dataclass, field
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
 from ._lib import check, wk_segment
-from .api import DecodingOptions, SpecialTokens, attached_bias, language_code
+from .api import DecodingOptions, SpecialTokens, attached_bias, language_code, top_logprob_dicts, top_logprobs_of, top_logprobs_set
 
 
 @dataclass
@@ -30,15 +30,21 @@ class TranscriptionSegment:
     noSpeechProb: float
     words: Optional[list] = None
     text: str = ""
+    topLogProbs: List[Dict[int, float]] = field(default_factory=list)   # DecodingOptions.topLogProbs, sliced like tokenLogProbs
 
 
-def _segs(raw, n, tokens, lps, rel=0) -> List[TranscriptionSegment]:
+def _segs(raw, n, tokens, lps, rel=0, top=None) -> List[TranscriptionSegment]:
+    """top: (the flat [tokens][k] pairs of wk_transcription_top_logprobs, k) for DecodingOptions.topLogProbs, else None."""
     out = []
     for i in range(n):
         g = raw[i]
         a, b = g.token_offset - rel, g.token_offset - rel + g.n_tokens
-        out.append(TranscriptionSegment(g.stream, g.id, g.seek, g.start, g.end, [int(t) for t in tokens[a:b]], [float(v) for v in lps[a:b]],
-                                        g.temperature, g.avg_logprob, g.compression_ratio, g.no_speech_prob))
+        seg = TranscriptionSegment(g.stream, g.id, g.seek, g.start, g.end, [int(t) for t in tokens[a:b]], [float(v) for v in lps[a:b]],
+                                   g.temperature, g.avg_logprob, g.compression_ratio, g.no_speech_prob)
+        if top is not None:
+            (ttok, tlp), k = top
+            seg.topLogProbs = top_logprob_dicts(ttok[a * k:b * k], tlp[a * k:b * k], b - a, k)
+        out.append(seg)
     return out
 
 
@@ -162,7 +168,8 @@ def transcribe_streams(kit, audioArrays: Sequence[np.ndarray], options: Optional
     native = hooks                      # a wk_tokenizer_hooks struct (WhisperTokenizer.hooks()): the library's own tokenizer, no host callbacks
     if native is None:
         hooks, keep_hooks = make_hooks(split_to_word_tokens, decode)
-    with attached_bias(lib, kit.textDecoder.handle, opts, kit.specialTokens, kit.tokenizer):
+    k = top_logprobs_of(opts)
+    with attached_bias(lib, kit.textDecoder.handle, opts, kit.specialTokens, kit.tokenizer), top_logprobs_set(lib, kit.textDecoder.handle, k):
         check(lib.wk_transcribe_streams_draft(kit.model.handle, kit.textDecoder.handle, ptrs, lens, len(arrs), C.byref(st), C.byref(o), p,
                                               len(prompt), ts, n, windowClipTime, -1 if maxWindowSeek is None else maxWindowSeek,
                                               1 if chunkingStrategy == "vad" else 0,
@@ -175,7 +182,13 @@ def transcribe_streams(kit, audioArrays: Sequence[np.ndarray], options: Optional
         tk = (C.c_int32 * max(1, nt))()
         lp = (C.c_float * max(1, nt))()
         check(lib.wk_transcription_tokens(h, tk, lp, max(1, nt)))
-        segs = _segs(raw, ns, tk, lp)
+        top = None
+        if k > 0:
+            ttok = (C.c_int32 * max(1, nt * k))()
+            tlp = (C.c_float * max(1, nt * k))()
+            check(lib.wk_transcription_top_logprobs(h, ttok, tlp, max(1, nt * k)))
+            top = ((ttok, tlp), k)
+        segs = _segs(raw, ns, tk, lp, top=top)
         if opts.wordTimestamps:
             for g in segs:
                 g.words = []

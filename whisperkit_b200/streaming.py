@@ -41,7 +41,8 @@ def _same(a: StreamState, b: StreamState) -> bool:
 
 
 class AudioStreamTranscriber:
-    """One streamer per DecodingOptions.  Beam search, bestOf and draftTokens are not supported in streams (WK_ERR_INVALID_ARGUMENT)."""
+    """One streamer per DecodingOptions.  Beam search, bestOf, draftTokens and topLogProbs are not supported in streams
+    (WK_ERR_INVALID_ARGUMENT)."""
 
     def __init__(self, kit, decodingOptions: Optional[DecodingOptions] = None, requiredSegmentsForConfirmation: int = 2,
                  silenceThreshold: float = 0.3, compressionCheckWindow: int = 60, useVAD: bool = True,
@@ -53,6 +54,8 @@ class AudioStreamTranscriber:
             raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"draftTokens={opts.draftTokens} is not supported in streams")
         if opts.biasPhrases is not None:
             raise WhisperError(WK_ERR_INVALID_ARGUMENT, "biasPhrases is not supported in streams")
+        if opts.topLogProbs:
+            raise WhisperError(WK_ERR_INVALID_ARGUMENT, f"topLogProbs={opts.topLogProbs} is not supported in streams")
         self.kit, self.options, self.lib = kit, opts, kit.model.lib
         self.stateChangeCallback = stateChangeCallback
         prompt = kit.textDecoder.prefillDecoderInputs(opts if opts.usePrefillPrompt else None, kit.specialTokens)

@@ -729,6 +729,20 @@ wk_status wk_test_cross_attention_shared(wk_model* m, const float* q, const void
 wk_status wk_test_cross_attention_fp8(wk_model* m, const float* q, const uint8_t* kcodes, const uint8_t* vcodes, const float* kscale,
                                       const float* vscale, void* out, int32_t B, int32_t H, int32_t T, int32_t dtype, const int32_t* done,
                                       int32_t kv_div, float* align_out);
+/* Packed bf16 cross K/V cache (the default cache of a bf16 model).  wk_test_cross_kv_project: the cross-K/V projection GEMM alone,
+ * x [windows * T][d] times w [d][d] (+ bias [d], may be NULL) of one K or V, d = H * 64, bf16.  packed == 0: the 16-bit cache blocks
+ * out [windows][H][T][64]; packed != 0: the packed blocks (T x 128 bytes each) in out and the row headers [windows][H][round_up(T, 16)]
+ * in hdr. */
+wk_status wk_test_cross_kv_project(wk_model* m, const void* x, const void* w, const float* bias, int32_t windows, int32_t T, int32_t H,
+                                   int32_t packed, void* out, uint8_t* hdr);
+/* wk_test_cross_attention_fp8 on the packed cache (blocks and headers as wk_test_cross_kv_project writes them); out is bf16. */
+wk_status wk_test_cross_attention_packed(wk_model* m, const float* q, const void* kc, const void* vc, const uint8_t* khdr, const uint8_t* vhdr,
+                                         void* out, int32_t B, int32_t H, int32_t T, const int32_t* done, int32_t kv_div, float* align_out);
+/* The word-timestamp pass's cross-attention alone (bf16): q [nw * 224][H * 64] against the cache blocks of slots 0 .. nw - 1 (16-bit, or
+ * packed when khdr / vhdr are not NULL), seq_len [nw] device -> out [nw * 224][H * 64]; then the export of the heads in `mask` into
+ * acc [nw * 224][T] f32. */
+wk_status wk_test_align_cross_attention(wk_model* m, const void* q, const void* kc, const void* vc, const uint8_t* khdr, const uint8_t* vhdr,
+                                        const int32_t* seq_len, int32_t nw, int32_t H, int32_t T, uint32_t mask, void* out, float* acc);
 /* Decoder self-attention kernel alone: qkv [B][3*H*64] f32 of the new token, caches [B][H][224][64] 16-bit (positions < pos[b] valid;
  * row pos[b] is appended), pos [B] device -> out [B][H*64] 16-bit. */
 wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, void* vcache, const int32_t* pos, void* out, int32_t B,

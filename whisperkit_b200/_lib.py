@@ -284,6 +284,9 @@ SYMBOLS = [
     ("wk_test_cross_attention_shared", I32, [P, P, P, P, P, I32, I32, I32, I32, P, I32]),
     ("wk_test_cross_attention_fp8", I32, [P, P, P, P, P, P, P, I32, I32, I32, I32, P, I32, P]),
     ("wk_test_self_attention", I32, [P, P, P, P, P, P, I32, I32, I32, P]),
+    ("wk_test_cross_kv_project", I32, [P, P, P, P, I32, I32, I32, I32, P, P]),
+    ("wk_test_cross_attention_packed", I32, [P, P, P, P, P, P, P, I32, I32, I32, P, I32, P]),
+    ("wk_test_align_cross_attention", I32, [P, P, P, P, P, P, P, I32, I32, I32, C.c_uint32, P, P]),
     ("wk_test_gemm_residual", I32, [P, P, P, P, P, I32, I32, I32, I32]),
     ("wk_test_gemm_fp8", I32, [P, I32, P, P, P, P, P, P, P, I32, I32, I32, I32]),
     ("wk_test_gemm_splitk", I32, [P, P, P, P, I32, I32, I32, I32, I32]),

@@ -139,10 +139,44 @@ __device__ __forceinline__ void at_widen(const uint8_t* codes, T* dst, int tid) 
     }
 }
 
+// Packed bf16 cache: cp.async of the 96-byte primary slots of rows [key0, key0 + 64) of block `blk` and of their 64 header bytes (at
+// kAtKeys * 96); rows >= nkeys are zero-filled (header 0, value 0)
+__device__ __forceinline__ void at_issue_tile_packed(uint8_t* dst, const uint8_t* __restrict__ blk, const uint8_t* __restrict__ hdr, int key0,
+                                                     int nkeys, int tid) {
+    for (int i = tid; i < kAtKeys * 6 + 4; i += kAtThreads) {
+        if (i < kAtKeys * 6) {
+            const int r = i / 6, c = i % 6, key = key0 + r;
+            const bool ok = key < nkeys;
+            cp_async16(dst + r * kPackedRowBytes + c * 16, blk + (long long)(ok ? key : 0) * kPackedRowBytes + c * 16, ok);
+        } else {
+            const int c = i - kAtKeys * 6;
+            const bool ok = key0 + 16 * c < nkeys;   // the header vector is padded to 16 bytes
+            cp_async16(dst + kAtKeys * kPackedRowBytes + c * 16, hdr + (ok ? key0 + 16 * c : 0), ok);
+        }
+    }
+}
+// Packed: rebuild the exact bf16 tile in the 16-bit [64][kAtLd] layout (a raw row's last 32 bytes from global memory)
+template <typename T>
+__device__ __forceinline__ void at_widen_packed(const uint8_t* tile, T* dst, const uint8_t* __restrict__ blk, int Tlen, int key0, int tid) {
+    for (int i = tid; i < kAtKeys * 8; i += kAtThreads) {
+        const int r = i >> 3, c = i & 7;
+        const uint8_t h = tile[kAtKeys * kPackedRowBytes + r];
+        const uint8_t* pr = tile + r * kPackedRowBytes;
+        uint4 u;
+        if (h == kPackedRaw)
+            u = c < 6 ? *reinterpret_cast<const uint4*>(pr + 16 * c)
+                      : __ldg(reinterpret_cast<const uint4*>(blk + (long long)Tlen * kPackedRowBytes + (long long)(key0 + r) * 32 + 16 * (c - 6)));
+        else
+            u = unpack_bf16x8(*reinterpret_cast<const uint2*>(pr + 8 * c), *reinterpret_cast<const uint32_t*>(pr + 64 + 4 * c), h);
+        *reinterpret_cast<uint4*>(dst + r * kAtLd + c * 8) = u;
+    }
+}
+
 // =====================================================================================================
 // attention.  KIND 0: causal self-attention over the window's own rows of the QKV output (keys <= the query position);
 // KIND 1: cross-attention against the 16-bit cache block [T][64] of the window's slot; KIND 2: the same against the FP8 cache (codes widened
-// exactly to 16-bit in shared memory, the K row scale applied to the scores, the V row scale folded into p relative to the block's largest).
+// exactly to 16-bit in shared memory, the K row scale applied to the scores, the V row scale folded into p relative to the block's largest);
+// KIND 3: the same against the packed bf16 cache (rows rebuilt exactly in shared memory, at_widen_packed).
 // One CTA = (query tile of 128 rows, head, window); K / V stream through a double-buffered 64-key ring; each warp keeps its 16 rows' running
 // max / sum / output in registers.  Query tiles that start past the window's sequence exit at once; rows past it are computed but not stored.
 // stats != nullptr (cross only): each row's final (max, sum) of the head, [H][rows], for align_export_kernel.
@@ -151,11 +185,12 @@ template <typename T, int KIND>
 __global__ void __launch_bounds__(kAtThreads)
 align_attention_kernel(const T* __restrict__ q, long long ldq, const uint8_t* __restrict__ kb, const uint8_t* __restrict__ vb, long long ld_kv,
                        const float* __restrict__ kscale, const float* __restrict__ vscale, const int32_t* __restrict__ seq_len, int slot0,
-                       T* __restrict__ out, int H, int Tlen, float2* __restrict__ stats, long long stat_rows) {
-    constexpr bool FP8 = KIND == 2;
-    constexpr int kTileBytes = FP8 ? kAtKeys * 64 : kAtKeys * kAtLd * 2;
+                       T* __restrict__ out, int H, int Tlen, float2* __restrict__ stats, long long stat_rows, const uint8_t* __restrict__ khdr,
+                       const uint8_t* __restrict__ vhdr) {
+    constexpr bool FP8 = KIND == 2, PK = KIND == 3, WIDE = FP8 || PK;
+    constexpr int kTileBytes = FP8 ? kAtKeys * 64 : PK ? kAtKeys * (kPackedRowBytes + 1) : kAtKeys * kAtLd * 2;
     __shared__ __align__(128) uint8_t ring[2][2][kTileBytes];           // [stage][K|V]
-    __shared__ __align__(128) T wide[FP8 ? 2 : 1][FP8 ? kAtKeys * kAtLd : 8];   // FP8: the widened K and V tiles
+    __shared__ __align__(128) T wide[WIDE ? 2 : 1][WIDE ? kAtKeys * kAtLd : 8];   // FP8 / packed: the widened K and V tiles
     __shared__ float ksc_s[FP8 ? kAtKeys : 1], vsc_s[FP8 ? kAtKeys : 1], red[8];
     const int qt = blockIdx.x, h = blockIdx.y, w = blockIdx.z;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, tq = lane & 3;
@@ -173,6 +208,16 @@ align_attention_kernel(const T* __restrict__ q, long long ldq, const uint8_t* __
     const uint8_t* ksrc = KIND == 0 ? kb + (row_base * ld_kv + h * 64) * 2 : kb + blk * Tlen * ld_kv;
     const uint8_t* vsrc = KIND == 0 ? vb + (row_base * ld_kv + h * 64) * 2 : vb + blk * Tlen * ld_kv;
     const long long ld_bytes = KIND == 0 ? ld_kv * 2 : ld_kv;
+    const long long hoff = PK ? blk * packed_hdr_stride(Tlen) : 0;
+    auto issue = [&](uint8_t* kd, uint8_t* vd, int key0) {
+        if constexpr (PK) {
+            at_issue_tile_packed(kd, ksrc, khdr + hoff, key0, nkeys, tid);
+            at_issue_tile_packed(vd, vsrc, vhdr + hoff, key0, nkeys, tid);
+        } else {
+            at_issue_tile<FP8>(kd, ksrc, ld_bytes, key0, nkeys, tid);
+            at_issue_tile<FP8>(vd, vsrc, ld_bytes, key0, nkeys, tid);
+        }
+    };
     float vmax = 1.f;
     if constexpr (FP8) {   // V scales are used relative to the block's largest, so p * vsc / vmax stays <= 1
         float vm = 0.f;
@@ -194,14 +239,12 @@ align_attention_kernel(const T* __restrict__ q, long long ldq, const uint8_t* __
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
     const int pos0 = rw0 + g, pos1 = rw0 + g + 8;   // positions of the thread's two rows
 
-    at_issue_tile<FP8>(ring[0][0], ksrc, ld_bytes, 0, nkeys, tid);
-    at_issue_tile<FP8>(ring[0][1], vsrc, ld_bytes, 0, nkeys, tid);
+    issue(ring[0][0], ring[0][1], 0);
     cp_async_commit();
     for (int kt = 0; kt < ntiles; ++kt) {
         const int stg = kt & 1;
         if (kt + 1 < ntiles) {
-            at_issue_tile<FP8>(ring[stg ^ 1][0], ksrc, ld_bytes, (kt + 1) * kAtKeys, nkeys, tid);
-            at_issue_tile<FP8>(ring[stg ^ 1][1], vsrc, ld_bytes, (kt + 1) * kAtKeys, nkeys, tid);
+            issue(ring[stg ^ 1][0], ring[stg ^ 1][1], (kt + 1) * kAtKeys);
             cp_async_commit();
             cp_async_wait<1>();
         } else {
@@ -218,6 +261,13 @@ align_attention_kernel(const T* __restrict__ q, long long ldq, const uint8_t* __
                 ksc_s[tid] = key < Tlen ? kscale[blk * Tlen + key] : 0.f;
                 vsc_s[tid] = key < Tlen ? vscale[blk * Tlen + key] * inv_vmax : 0.f;
             }
+            __syncthreads();
+            kt16 = wide[0];
+            vt16 = wide[1];
+        }
+        if constexpr (PK) {
+            at_widen_packed<T>(ring[stg][0], wide[0], ksrc, Tlen, kt * kAtKeys, tid);
+            at_widen_packed<T>(ring[stg][1], wide[1], vsrc, Tlen, kt * kAtKeys, tid);
             __syncthreads();
             kt16 = wide[0];
             vt16 = wide[1];
@@ -311,9 +361,9 @@ align_attention_kernel(const T* __restrict__ q, long long ldq, const uint8_t* __
 template <typename T, int KIND>
 static void launch_attention(const void* q, long long ldq, const void* k, const void* v, long long ld_kv, const float* ks, const float* vs,
                              const int32_t* seq_len, int slot0, void* out, int nw, int H, int Tlen, float2* stats, long long stat_rows,
-                             cudaStream_t stream) {
+                             cudaStream_t stream, const uint8_t* kh = nullptr, const uint8_t* vh = nullptr) {
     launch_k(align_attention_kernel<T, KIND>, dim3((kAlignStride + kAtQ - 1) / kAtQ, H, nw), dim3(kAtThreads), 0, stream, 0, (const T*)q, ldq,
-             (const uint8_t*)k, (const uint8_t*)v, ld_kv, ks, vs, seq_len, slot0, (T*)out, H, Tlen, stats, stat_rows);
+             (const uint8_t*)k, (const uint8_t*)v, ld_kv, ks, vs, seq_len, slot0, (T*)out, H, Tlen, stats, stat_rows, kh, vh);
 }
 
 wk_status align_self_attention(const void* qkv, const int32_t* seq_len, void* out, int nw, int H, int dtype, cudaStream_t stream) {
@@ -331,11 +381,15 @@ wk_status align_self_attention(const void* qkv, const int32_t* seq_len, void* ou
 }
 
 wk_status align_cross_attention(const void* q, const void* kc, const void* vc, const float* kscale, const float* vscale, const int32_t* seq_len,
-                                int slot0, void* out, float* stats, int64_t stat_rows, int nw, int H, int Tlen, int dtype, cudaStream_t stream) {
+                                int slot0, void* out, float* stats, int64_t stat_rows, int nw, int H, int Tlen, int dtype, cudaStream_t stream,
+                                const uint8_t* khdr, const uint8_t* vhdr) {
     const bool fp8 = kscale != nullptr, f16 = dtype == WK_DTYPE_F16;
     const long long ldq = (long long)H * 64;
     float2* st2 = reinterpret_cast<float2*>(stats);
-    if (fp8) {
+    if (khdr) {
+        if (f16 || fp8 || !vhdr) { set_error("align_cross_attention: the packed cache is bf16 and needs both header vectors"); return WK_ERR_INVALID_ARGUMENT; }
+        launch_attention<__nv_bfloat16, 3>(q, ldq, kc, vc, 128, nullptr, nullptr, seq_len, slot0, out, nw, H, Tlen, st2, stat_rows, stream, khdr, vhdr);
+    } else if (fp8) {
         if (f16) launch_attention<__half, 2>(q, ldq, kc, vc, 64, kscale, vscale, seq_len, slot0, out, nw, H, Tlen, st2, stat_rows, stream);
         else launch_attention<__nv_bfloat16, 2>(q, ldq, kc, vc, 64, kscale, vscale, seq_len, slot0, out, nw, H, Tlen, st2, stat_rows, stream);
     } else {
@@ -355,14 +409,16 @@ wk_status align_cross_attention(const void* q, const void* kc, const void* vc, c
 // at 0).  Each accumulator element belongs to one thread of one CTA: the mean is deterministic, in the decode loop's order (layers, then
 // heads, decoder_align_mean_kernel).
 // =====================================================================================================
-template <typename T, bool FP8>
+// F: 0 the 16-bit cache, 1 FP8, 2 packed bf16
+template <typename T, int F>
 __global__ void __launch_bounds__(kAtThreads)
 align_export_kernel(const T* __restrict__ q, const uint8_t* __restrict__ kc, const float* __restrict__ kscale, const float2* __restrict__ stats,
                     long long stat_rows, const int32_t* __restrict__ seq_len, int slot0, uint32_t mask, int first, float* __restrict__ acc, int H,
-                    int Tlen) {
-    constexpr int kTileBytes = FP8 ? kAtKeys * 64 : kAtKeys * kAtLd * 2;
+                    int Tlen, const uint8_t* __restrict__ khdr) {
+    constexpr bool FP8 = F == 1, PK = F == 2;
+    constexpr int kTileBytes = FP8 ? kAtKeys * 64 : PK ? kAtKeys * (kPackedRowBytes + 1) : kAtKeys * kAtLd * 2;
     __shared__ __align__(128) uint8_t tile[kTileBytes];
-    __shared__ __align__(128) T wide[FP8 ? kAtKeys * kAtLd : 8];
+    __shared__ __align__(128) T wide[FP8 || PK ? kAtKeys * kAtLd : 8];
     __shared__ float ksc_s[FP8 ? kAtKeys : 1];
     const int kt = blockIdx.x, qt = blockIdx.y, w = blockIdx.z;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, tq = lane & 3;
@@ -373,7 +429,7 @@ align_export_kernel(const T* __restrict__ q, const uint8_t* __restrict__ kc, con
     const int rw0 = q0 + warp * 16;
     const bool active = rw0 < n;
     const int pos0 = rw0 + g, pos1 = rw0 + g + 8;
-    const long long ld_bytes = FP8 ? 64 : 128;
+    const long long ld_bytes = FP8 ? 64 : 128;   // packed: blocks of T x 128 bytes too
     float a[8][4];
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
@@ -385,7 +441,8 @@ align_export_kernel(const T* __restrict__ q, const uint8_t* __restrict__ kc, con
     for (uint32_t hm = mask; hm != 0; hm &= hm - 1) {
         const int h = __ffs(hm) - 1;
         const long long blk = (long long)(slot0 + w) * H + h;
-        at_issue_tile<FP8>(tile, kc + blk * Tlen * ld_bytes, ld_bytes, kt * kAtKeys, Tlen, tid);
+        if constexpr (PK) at_issue_tile_packed(tile, kc + blk * Tlen * ld_bytes, khdr + blk * packed_hdr_stride(Tlen), kt * kAtKeys, Tlen, tid);
+        else at_issue_tile<FP8>(tile, kc + blk * Tlen * ld_bytes, ld_bytes, kt * kAtKeys, Tlen, tid);
         cp_async_commit();
         cp_async_wait<0>();
         __syncthreads();
@@ -396,6 +453,11 @@ align_export_kernel(const T* __restrict__ q, const uint8_t* __restrict__ kc, con
                 const int key = kt * kAtKeys + tid;
                 ksc_s[tid] = key < Tlen ? kscale[blk * Tlen + key] : 0.f;
             }
+            __syncthreads();
+            k16 = wide;
+        }
+        if constexpr (PK) {
+            at_widen_packed<T>(tile, wide, kc + blk * Tlen * ld_bytes, Tlen, kt * kAtKeys, tid);
             __syncthreads();
             k16 = wide;
         }
@@ -429,14 +491,17 @@ align_export_kernel(const T* __restrict__ q, const uint8_t* __restrict__ kc, con
 }
 
 wk_status align_export(const void* q, const void* kc, const float* kscale, const float* stats, int64_t stat_rows, const int32_t* seq_len, int slot0,
-                       uint32_t mask, int first, float* acc, int nw, int H, int Tlen, int dtype, cudaStream_t stream) {
+                       uint32_t mask, int first, float* acc, int nw, int H, int Tlen, int dtype, cudaStream_t stream, const uint8_t* khdr) {
     const dim3 grid((Tlen + kAtKeys - 1) / kAtKeys, (kAlignStride + kAtQ - 1) / kAtQ, nw);
     const float2* st2 = reinterpret_cast<const float2*>(stats);
     const bool fp8 = kscale != nullptr, f16 = dtype == WK_DTYPE_F16;
 #define WK_EXPORT(TT, F) launch_k(align_export_kernel<TT, F>, grid, dim3(kAtThreads), 0, stream, 0, (const TT*)q, (const uint8_t*)kc, kscale, st2, \
-                                  (long long)stat_rows, seq_len, slot0, mask, first, acc, H, Tlen)
-    if (fp8) { if (f16) WK_EXPORT(__half, true); else WK_EXPORT(__nv_bfloat16, true); }
-    else { if (f16) WK_EXPORT(__half, false); else WK_EXPORT(__nv_bfloat16, false); }
+                                  (long long)stat_rows, seq_len, slot0, mask, first, acc, H, Tlen, khdr)
+    if (khdr) {
+        if (f16 || fp8) { set_error("align_export: the packed cache is bf16"); return WK_ERR_INVALID_ARGUMENT; }
+        WK_EXPORT(__nv_bfloat16, 2);
+    } else if (fp8) { if (f16) WK_EXPORT(__half, 1); else WK_EXPORT(__nv_bfloat16, 1); }
+    else { if (f16) WK_EXPORT(__half, 0); else WK_EXPORT(__nv_bfloat16, 0); }
 #undef WK_EXPORT
     count_launch();
     cudaError_t e = cudaGetLastError();

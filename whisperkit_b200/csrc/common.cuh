@@ -70,6 +70,36 @@ __device__ __forceinline__ void fp8x4_to_half2(uint32_t w, uint32_t& lo, uint32_
     hi = (uint32_t)b.x | ((uint32_t)b.y << 16);
 }
 
+// Packed bf16 cross K/V cache (12 bits per value, lossless).  Block (layer, K|V, slot, head) keeps its T x 128-byte region:
+//   primary slot of row t at t * 96: 64 sign|mantissa bytes (value i -> byte i: sign in bit 7, mantissa in bits 0..6), then 32 bytes of
+//     exponent offsets, 4 bytes per group of 8 values (group g at 64 + 4 g); value 8 g + j sits at bit 16 (j & 1) + 4 (j >> 1) of its word
+//   secondary slot of row t at T * 96 + t * 32: bytes 96..127 of a raw row
+//   header byte of row t (a separate [block][round_up(T, 16)] vector): the row's largest exponent field `base`, offset = base - field
+//   (0..15), or kPackedRaw: the row spans more than 16 binades or holds Inf/NaN and keeps its 128 raw bytes (0..95 primary, 96..127
+//   secondary).  Exponent fields are coded as bits, so zeros and subnormals (field 0) need no special case.
+static constexpr int kPackedRowBytes = 96;
+static constexpr uint8_t kPackedRaw = 255;
+__host__ __device__ inline int packed_hdr_stride(int T) { return (T + 15) & ~15; }
+// the bf16 bits of one group of 8 values of a packed row, as the uint4 the raw row holds there
+__device__ __forceinline__ uint4 unpack_bf16x8(uint2 sm, uint32_t nib, uint32_t base) {
+    const uint32_t b7 = (base << 7) | (base << 23);
+    const uint32_t nh = nib >> 8;
+    // prmt: sign|mantissa byte k into bits 0..7 of its 16-bit half and its sign replicated into bits 8..15; & 0x807f keeps sign and mantissa
+    uint4 u;
+    u.x = (__byte_perm(sm.x, 0, 0x9180) & 0x807f807fu) | (b7 - (nib & 0x000f000fu) * 128u);
+    u.y = (__byte_perm(sm.x, 0, 0xb3a2) & 0x807f807fu) | (b7 - (nib & 0x00f000f0u) * 8u);
+    u.z = (__byte_perm(sm.y, 0, 0x9180) & 0x807f807fu) | (b7 - (nh & 0x000f000fu) * 128u);
+    u.w = (__byte_perm(sm.y, 0, 0xb3a2) & 0x807f807fu) | (b7 - (nh & 0x00f000f0u) * 8u);
+    return u;
+}
+// 8 values (16 bytes) of row t of a packed block: group g of a coded row, or bytes 16 g .. 16 g + 15 of a raw row
+__device__ __forceinline__ uint4 packed_group(const uint8_t* blk, int T, int t, int g, uint8_t hdr) {
+    const uint8_t* row = blk + (long long)t * kPackedRowBytes;
+    if (hdr == kPackedRaw)
+        return *reinterpret_cast<const uint4*>(g < 6 ? row + 16 * g : blk + (long long)T * kPackedRowBytes + (long long)t * 32 + 16 * (g - 6));
+    return unpack_bf16x8(*reinterpret_cast<const uint2*>(row + 8 * g), *reinterpret_cast<const uint32_t*>(row + 64 + 4 * g), hdr);
+}
+
 __device__ __forceinline__ float gelu_erf(float x) {
     // exact (erf) GELU with erf from Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, far below the 16-bit storage step of the output):
     // ~13 instructions and 2 MUFU ops against libdevice erff's two divergent polynomial branches - the FC1 epilogue is bound by this
@@ -134,6 +164,10 @@ __device__ __forceinline__ void fence_proxy_async() {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                  : "memory");
+}
+// raise the transaction count of the current phase without arriving
+__device__ __forceinline__ void mbar_expect_tx_only(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");

@@ -11,6 +11,9 @@
 // Softmax is exact two-pass over the f32 scores in shared memory (one warp per beam row, no block barriers inside).
 // FP8 cache (FP8 = true): the TMA brings 64-byte rows of E4M3 codes, each consumer warp widens its rows exactly to 16-bit (mq_widen_fp8) and
 // the MMA path is unchanged; the K row scale multiplies the scores, p carries the V row scale relative to the block's largest one.
+// Packed bf16 cache (PK): the TMA brings the 96-byte primary slots, the consumers first copy the block's row headers to shared memory, and
+// each warp rebuilds its rows' exact bf16 values into the same 16-bit buffer (mq_widen_packed; a raw row's last 32 bytes come from global
+// memory - at most a few rows per tile).
 // 4 consumer warps (each owns a quarter of every tile's keys) + 1 TMA producer warp; the K tiles do not depend on the upstream kernel
 // (the cross K/V cache is written before the decode loop), so the producer starts before griddepcontrol.wait.
 // Reference counterpart: the cross-attention inside TextDecoder.mlmodelc (Sources/WhisperKit/Core/TextDecoder.swift:394-417); beam
@@ -79,13 +82,34 @@ __device__ __forceinline__ void mq_widen_fp8(const uint8_t* tile, uint8_t* wbuf,
     }
 }
 
-template <typename T, int NQ, int STAGES, bool FP8>
+// Packed cache: a warp rebuilds its 32 rows of the tile (headers hdr[row of the tile]) into its 4 KiB buffer, same layout as mq_widen_fp8
+__device__ __forceinline__ void mq_widen_packed(const uint8_t* tile, const uint8_t* hdr, const uint8_t* __restrict__ blk, int Tlen, int t0,
+                                                uint8_t* wbuf, int warp, int lane) {
+#pragma unroll 1
+    for (int it = 0; it < 8; ++it) {
+        const int idx = it * 32 + lane, row = idx >> 3, chunk = idx & 7, tr = warp * 32 + row;
+        const uint8_t h = hdr[tr];
+        const uint8_t* pr = tile + tr * kPackedRowBytes;
+        uint4 u;
+        if (h == kPackedRaw)
+            u = chunk < 6 ? *reinterpret_cast<const uint4*>(pr + 16 * chunk)
+                          : __ldg(reinterpret_cast<const uint4*>(blk + (long long)Tlen * kPackedRowBytes + (long long)(t0 + tr) * 32 + 16 * (chunk - 6)));
+        else
+            u = unpack_bf16x8(*reinterpret_cast<const uint2*>(pr + 8 * chunk), *reinterpret_cast<const uint32_t*>(pr + 64 + 4 * chunk), h);
+        *reinterpret_cast<uint4*>(wbuf + row * 128 + ((chunk ^ (row & 7)) << 4)) = u;
+    }
+}
+
+// F: 0 the 16-bit cache, 1 FP8, 2 packed bf16
+template <typename T, int NQ, int STAGES, int F>
 __global__ void __launch_bounds__(kMqThreads)
 decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
                                   const float* __restrict__ partial, int splits, int Bp, const float* __restrict__ bq, T* __restrict__ out, int H,
                                   int Tlen, int chunks, const int32_t* __restrict__ done, const float* __restrict__ kscale,
-                                  const float* __restrict__ vscale) {
-    constexpr int kStage = FP8 ? kMqRows * 64 : kMqStageBytes;   // bytes of one TMA tile
+                                  const float* __restrict__ vscale, const uint8_t* __restrict__ kcross, const uint8_t* __restrict__ vcross,
+                                  const uint8_t* __restrict__ khdr, const uint8_t* __restrict__ vhdr) {
+    constexpr bool FP8 = F == 1, PK = F == 2, WIDE = FP8 || PK;
+    constexpr int kStage = FP8 ? kMqRows * 64 : PK ? kMqRows * kPackedRowBytes : kMqStageBytes;   // bytes of one TMA tile
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));   // STAGES x kStage
     const int Tp = chunks * kMqRows;
@@ -99,7 +123,9 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
     float* ksc = reinterpret_cast<float*>(empty_bar + STAGES);
     float* vsc = ksc + Tp;
     float* vmax_s = vsc + Tp;
-    uint8_t* wbuf = reinterpret_cast<uint8_t*>(vmax_s + 8);
+    // packed: the widened tiles right after the barriers, then the K and V row headers [2][Tp] (rows past Tlen: 0)
+    uint8_t* wbuf = PK ? reinterpret_cast<uint8_t*>(empty_bar + STAGES) : reinterpret_cast<uint8_t*>(vmax_s + 8);
+    uint8_t* hdr_s = wbuf + 4 * 32 * 128;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int win = blockIdx.x / H, h = blockIdx.x % H;
@@ -150,6 +176,13 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
         vm = warp_max(vm);
         if (lane == 0) vmax_s[warp] = vm;
     }
+    if constexpr (PK) {
+        const long long hb = (long long)blockIdx.x * packed_hdr_stride(Tlen);
+        for (int t = tid; t < Tp; t += 128) {
+            hdr_s[t] = t < Tlen ? khdr[hb + t] : 0;
+            hdr_s[Tp + t] = t < Tlen ? vhdr[hb + t] : 0;
+        }
+    }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     // FP8: p carries vsc[t] / vmax (at most 1, so the hi + lo split of p keeps its range) and the output is scaled back by vmax
     const float vmax = FP8 ? fmaxf(fmaxf(vmax_s[0], vmax_s[1]), fmaxf(vmax_s[2], vmax_s[3])) : 1.f;
@@ -170,8 +203,10 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
         const int stage = c % STAGES;
         mbar_wait_bounded(&full_bar[stage], (c / STAGES) & 1);
         uint32_t tile = smem_u32(ring + stage * kStage);
-        if constexpr (FP8) {   // widen this warp's rows, release the stage, read the 16-bit copy (same row addressing)
-            mq_widen_fp8<T>(ring + stage * kStage, wbuf + warp * 4096, warp, lane);
+        if constexpr (WIDE) {   // widen this warp's rows, release the stage, read the 16-bit copy (same row addressing)
+            if constexpr (FP8) mq_widen_fp8<T>(ring + stage * kStage, wbuf + warp * 4096, warp, lane);
+            else mq_widen_packed(ring + stage * kStage, hdr_s + c * kMqRows, kcross + (long long)blockIdx.x * Tlen * 128, Tlen, c * kMqRows,
+                                 wbuf + warp * 4096, warp, lane);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[stage]);
             tile = smem_u32(wbuf + warp * 4096) - warp * 4096;
@@ -197,7 +232,7 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
             if (g < NQ) *reinterpret_cast<float2*>(scores + g * Tp + c * kMqRows + kg * 8 + 2 * tq) = make_float2(cacc[0], cacc[1]);
         }
         __syncwarp();
-        if (!FP8 && lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (!WIDE && lane == 0) mbar_arrive(&empty_bar[stage]);
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     // ---- exact two-pass softmax, one warp per beam row; keys past Tlen (zero-filled K rows) get probability 0
@@ -227,8 +262,10 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
         const int stage = c % STAGES;
         mbar_wait_bounded(&full_bar[stage], (c / STAGES) & 1);
         uint32_t tile = smem_u32(ring + stage * kStage);
-        if constexpr (FP8) {   // widen this warp's rows, release the stage, read the 16-bit copy (same row addressing)
-            mq_widen_fp8<T>(ring + stage * kStage, wbuf + warp * 4096, warp, lane);
+        if constexpr (WIDE) {   // widen this warp's rows, release the stage, read the 16-bit copy (same row addressing)
+            if constexpr (FP8) mq_widen_fp8<T>(ring + stage * kStage, wbuf + warp * 4096, warp, lane);
+            else mq_widen_packed(ring + stage * kStage, hdr_s + Tp + (c - chunks) * kMqRows, vcross + (long long)blockIdx.x * Tlen * 128, Tlen,
+                                 (c - chunks) * kMqRows, wbuf + warp * 4096, warp, lane);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[stage]);
             tile = smem_u32(wbuf + warp * 4096) - warp * 4096;
@@ -258,7 +295,7 @@ decoder_cross_attention_mq_kernel(const __grid_constant__ CUtensorMap tm_k, cons
             }
         }
         __syncwarp();
-        if (!FP8 && lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (!WIDE && lane == 0) mbar_arrive(&empty_bar[stage]);
     }
     if (g < NQ) {
 #pragma unroll
@@ -278,32 +315,35 @@ typedef CUresult (*PFN_encodeTiledMq)(CUtensorMap*, CUtensorMapDataType, cuuint3
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 template <int NQ> static constexpr int mq_stages() { return NQ <= 5 ? 4 : 3; }
-template <int NQ, bool FP8> static size_t mq_smem_bytes(int chunks) {
-    const size_t fp8_extra = FP8 ? (size_t)2 * chunks * kMqRows * 4 + 8 * 4 + 4 * 32 * 128 : 0;   // row scales, V-scale maximum, widened tiles
-    return 1024 + (size_t)mq_stages<NQ>() * (FP8 ? kMqRows * 64 : kMqStageBytes) + (size_t)NQ * chunks * kMqRows * 4 + (size_t)NQ * 64 * 4 +
-           (size_t)4 * NQ * 64 * 4 + 8 * 4 + 2 * mq_stages<NQ>() * 8 + fp8_extra + 64;
+template <int NQ, int F> static size_t mq_smem_bytes(int chunks) {
+    const size_t fp8_extra = F == 1 ? (size_t)2 * chunks * kMqRows * 4 + 8 * 4 + 4 * 32 * 128 : 0;   // row scales, V-scale maximum, widened tiles
+    const size_t pk_extra = F == 2 ? (size_t)4 * 32 * 128 + 2 * chunks * kMqRows : 0;                // widened tiles, row headers
+    const int stage = F == 1 ? kMqRows * 64 : F == 2 ? kMqRows * kPackedRowBytes : kMqStageBytes;
+    return 1024 + (size_t)mq_stages<NQ>() * stage + (size_t)NQ * chunks * kMqRows * 4 + (size_t)NQ * 64 * 4 +
+           (size_t)4 * NQ * 64 * 4 + 8 * 4 + 2 * mq_stages<NQ>() * 8 + fp8_extra + pk_extra + 64;
 }
 
-template <typename T, int NQ, bool FP8>
+template <typename T, int NQ, int F>
 static wk_status launch_mq(const CUtensorMap& tmk, const CUtensorMap& tmv, const float* partial, int splits, int Bp, const float* bq, void* out, int B, int H,
-                           int Tlen, int chunks, const int32_t* done, const float* kscale, const float* vscale, cudaStream_t stream) {
+                           int Tlen, int chunks, const int32_t* done, const float* kscale, const float* vscale, const void* kcross, const void* vcross,
+                           const uint8_t* khdr, const uint8_t* vhdr, cudaStream_t stream) {
     constexpr int ST = mq_stages<NQ>();
-    const size_t smem = mq_smem_bytes<NQ, FP8>(chunks);
+    const size_t smem = mq_smem_bytes<NQ, F>(chunks);
     if (smem > 227 * 1024) { set_error("decoder_cross_attention (beam): %d encoder positions do not fit shared memory", Tlen); return WK_ERR_INVALID_ARGUMENT; }
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_mq_kernel<T, NQ, ST, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_mq_kernel<T, NQ, ST, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(cross mq): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
         attr_set = true;
     }
-    launch_k(decoder_cross_attention_mq_kernel<T, NQ, ST, FP8>, dim3((B / NQ) * H), dim3(kMqThreads), smem, stream, 4, tmk, tmv, partial, splits, Bp, bq, (T*)out, H,
-             Tlen, chunks, done, kscale, vscale);
+    launch_k(decoder_cross_attention_mq_kernel<T, NQ, ST, F>, dim3((B / NQ) * H), dim3(kMqThreads), smem, stream, 4, tmk, tmv, partial, splits, Bp, bq, (T*)out, H,
+             Tlen, chunks, done, kscale, vscale, (const uint8_t*)kcross, (const uint8_t*)vcross, khdr, vhdr);
     return WK_OK;
 }
 
 wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, void* out, int B, int H,
                                      int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq, const float* kscale,
-                                     const float* vscale) {
+                                     const float* vscale, const uint8_t* khdr, const uint8_t* vhdr) {
     if (nq < 2 || nq > 8 || B % nq != 0) { set_error("decoder_cross_attention (beam): %d rows, groups of %d", B, nq); return WK_ERR_INVALID_ARGUMENT; }
     static PFN_encodeTiledMq enc = nullptr;
     if (!enc) {
@@ -316,15 +356,17 @@ wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, c
         enc = reinterpret_cast<PFN_encodeTiledMq>(fp);
     }
     const int chunks = (Tlen + kMqRows - 1) / kMqRows;
-    const bool fp8 = kscale != nullptr;
+    const bool fp8 = kscale != nullptr, pk = khdr != nullptr;
+    if (pk && (fp8 || dtype != WK_DTYPE_BF16 || !vhdr)) { set_error("decoder_cross_attention (beam): the packed cache is bf16 and needs both header vectors"); return WK_ERR_INVALID_ARGUMENT; }
     CUtensorMap tmk, tmv;
-    const cuuint64_t row_bytes = fp8 ? 64 : 128;   // FP8: unswizzled 64-byte rows of codes, widened by the consumers
-    cuuint64_t gdim[3] = {64, (cuuint64_t)Tlen, (cuuint64_t)(B / nq) * H};
-    cuuint64_t gstr[2] = {row_bytes, (cuuint64_t)Tlen * row_bytes};
-    cuuint32_t box[3] = {64, (cuuint32_t)kMqRows, 1};
+    // FP8: unswizzled 64-byte rows of codes; packed: unswizzled 96-byte primary slots in blocks of T x 128 bytes; both widened by the consumers
+    const cuuint64_t row_bytes = fp8 ? 64 : pk ? kPackedRowBytes : 128;
+    cuuint64_t gdim[3] = {pk ? (cuuint64_t)kPackedRowBytes : 64, (cuuint64_t)Tlen, (cuuint64_t)(B / nq) * H};
+    cuuint64_t gstr[2] = {row_bytes, (cuuint64_t)Tlen * (pk ? 128 : row_bytes)};
+    cuuint32_t box[3] = {pk ? (cuuint32_t)kPackedRowBytes : 64, (cuuint32_t)kMqRows, 1};
     cuuint32_t es[3] = {1, 1, 1};
-    const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    const CUtensorMapSwizzle sw = fp8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
+    const CUtensorMapDataType dt = fp8 || pk ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : dtype == WK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const CUtensorMapSwizzle sw = fp8 || pk ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
     CUresult r = enc(&tmk, dt, 3, const_cast<void*>(kcross), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r == CUDA_SUCCESS)
@@ -332,12 +374,13 @@ wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, c
                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cross-attention tensor map encode failed: %d", (int)r); return WK_ERR_CUDA; }
     wk_status st = WK_OK;
-#define WK_MQ_T(N, F) (dtype == WK_DTYPE_F16 ? launch_mq<__half, N, F>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, kscale, vscale, stream) \
-                                           : launch_mq<__nv_bfloat16, N, F>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, kscale, vscale, stream))
-#define WK_MQ(N) case N: st = fp8 ? WK_MQ_T(N, true) : WK_MQ_T(N, false); break;
+#define WK_MQ_A(TT, N, F) launch_mq<TT, N, F>(tmk, tmv, partial, splits, Bp, bq, out, B, H, Tlen, chunks, done, kscale, vscale, kcross, vcross, khdr, vhdr, stream)
+#define WK_MQ_T(N, F) (dtype == WK_DTYPE_F16 ? WK_MQ_A(__half, N, F) : WK_MQ_A(__nv_bfloat16, N, F))
+#define WK_MQ(N) case N: st = pk ? WK_MQ_A(__nv_bfloat16, N, 2) : fp8 ? WK_MQ_T(N, 1) : WK_MQ_T(N, 0); break;
     switch (nq) { WK_MQ(2) WK_MQ(3) WK_MQ(4) WK_MQ(5) WK_MQ(6) WK_MQ(7) WK_MQ(8) default: break; }
 #undef WK_MQ
 #undef WK_MQ_T
+#undef WK_MQ_A
     if (st != WK_OK) return st;
     count_launch();
     cudaError_t e = cudaGetLastError();

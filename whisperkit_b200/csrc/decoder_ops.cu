@@ -472,15 +472,22 @@ wk_status decoder_kv_append(const float* partial, int splits, int Bp, const floa
 // contiguous K block then V block through a ring of 16000-byte bulk-copy stages (cp.async.bulk + mbarrier), a dedicated producer warp
 // keeps the ring full while 4 consumer warps compute.  K/V layout [B][H][T][64] (written head-major by the cross-KV GEMM epilogue).
 //   16-bit cache: 128-byte rows, 125 rows per stage, 2 stages (5 CTAs per SM); a lane takes 8 values (16 bytes) of a row.
+//   packed bf16 cache (common.cuh): the producer bulk-loads the block's K and V header vectors, then per stage the 12000 bytes of primary
+//   slots and, on the same barrier, one 32-byte copy of each raw row's secondary slot into the stage's side area; a lane rebuilds the exact
+//   uint4 the 16-bit row holds (cross_piece), so the dot products, the row-to-lane mapping and the reduction order are the 16-bit ones.
 //   FP8 cache (FP8 = true): 64-byte rows of E4M3 codes with one f32 scale per row ([B][H][T], see fp8_row_scale), 250 rows per stage,
 //   2 stages (4 CTAs per SM); the producer first bulk-loads the block's two scale vectors, a lane widens 16
 //   codes exactly to f32, the K scale multiplies each key's dot product before the softmax and the V scale is folded into p for the P.V
 //   phase - the alignment export stays the normalised softmax row.
 // =====================================================================================================
-template <bool FP8> struct CrossCfg {
+enum CrossFmt { kCrossRaw16 = 0, kCrossFp8 = 1, kCrossPacked = 2 };
+template <int F> struct CrossCfg {
+    static constexpr bool FP8 = F == kCrossFp8;
     static constexpr int kRowBytes = FP8 ? 64 : 128;
     static constexpr int kRows = FP8 ? 250 : 125;             // rows per stage: kRows * kRowBytes = 16000 B (multiple of 16)
+    // bytes a stage occupies in the ring: packed, the 12000-byte primary slots, then one 32-byte secondary slot per row (filled for raw rows)
     static constexpr int kStageBytes = kRows * kRowBytes;
+    static constexpr int kLoadBytes = F == kCrossPacked ? kRows * kPackedRowBytes : kStageBytes;   // bytes of a stage's bulk copy
     // 2 stages: 38.6 KB of shared memory per 16-bit CTA (5 per SM), 50.3 KB per FP8 CTA (4 per SM).  More, smaller CTAs per SM keep
     // more K/V streams in flight and shorten the last wave: a deeper ring (4 stages, 3 CTAs per SM) moved the same bytes more slowly
     static constexpr int kStages = 2;
@@ -488,7 +495,7 @@ template <bool FP8> struct CrossCfg {
     static constexpr int kRowsPerWarp = 32 / kLanesPerRow;    // rows per warp instruction
     static constexpr int kDims = 64 / kLanesPerRow;           // values per lane
 };
-static constexpr int kCrossRows = CrossCfg<false>::kRows;
+static constexpr int kCrossRows = CrossCfg<kCrossRaw16>::kRows;
 static constexpr int kCrossThreads = 160;           // 4 consumer warps + 1 producer warp
 
 __device__ __forceinline__ void fp8x16_to_f32(const uint4 u, float (&x)[16]) {
@@ -502,10 +509,9 @@ __device__ __forceinline__ void fp8x16_to_f32(const uint4 u, float (&x)[16]) {
     }
 }
 // q . (this lane's 16 bytes of a K row)
-template <typename T, bool FP8>
-__device__ __forceinline__ float cross_row_dot(const uint8_t* piece, const float (&qv)[CrossCfg<FP8>::kDims]) {
-    const uint4 u = *reinterpret_cast<const uint4*>(piece);
-    if constexpr (FP8) {
+template <typename T, int F>
+__device__ __forceinline__ float cross_row_dot(const uint4 u, const float (&qv)[CrossCfg<F>::kDims]) {
+    if constexpr (CrossCfg<F>::FP8) {
         float x[16];
         fp8x16_to_f32(u, x);
         float acc = 0.f;
@@ -518,10 +524,9 @@ __device__ __forceinline__ float cross_row_dot(const uint8_t* piece, const float
     }
 }
 // acc += p * (this lane's 16 bytes of a V row)
-template <typename T, bool FP8>
-__device__ __forceinline__ void cross_row_axpy(const uint8_t* piece, float p, float (&acc)[CrossCfg<FP8>::kDims]) {
-    const uint4 u = *reinterpret_cast<const uint4*>(piece);
-    if constexpr (FP8) {
+template <typename T, int F>
+__device__ __forceinline__ void cross_row_axpy(const uint4 u, float p, float (&acc)[CrossCfg<F>::kDims]) {
+    if constexpr (CrossCfg<F>::FP8) {
         float x[16];
         fp8x16_to_f32(u, x);
 #pragma unroll
@@ -533,24 +538,41 @@ __device__ __forceinline__ void cross_row_axpy(const uint8_t* piece, float p, fl
     }
 }
 
-template <typename T, bool FP8>
+// this lane's 16 bytes (8 16-bit values, or 16 FP8 codes) of row r of a stage; packed: rebuilt from the row's slots (header byte h)
+template <int F>
+__device__ __forceinline__ uint4 cross_piece(const uint8_t* tile, int r, int sub, uint8_t h) {
+    using C = CrossCfg<F>;
+    if constexpr (F == kCrossPacked) {
+        const uint8_t* row = tile + r * kPackedRowBytes;
+        if (h == kPackedRaw) return *reinterpret_cast<const uint4*>(sub < 6 ? row + 16 * sub : tile + C::kLoadBytes + r * 32 + 16 * (sub - 6));
+        return unpack_bf16x8(*reinterpret_cast<const uint2*>(row + 8 * sub), *reinterpret_cast<const uint32_t*>(row + 64 + 4 * sub), h);
+    } else {
+        return *reinterpret_cast<const uint4*>(tile + r * C::kRowBytes + sub * 16);
+    }
+}
+
+template <typename T, int F>
 __global__ void __launch_bounds__(kCrossThreads)
 decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, int Bp, const float* __restrict__ bq,
                                const uint8_t* __restrict__ kcross, const uint8_t* __restrict__ vcross, const float* __restrict__ kscale,
                                const float* __restrict__ vscale, T* __restrict__ out, int B, int H, int Tlen, const int32_t* __restrict__ done,
-                               float* __restrict__ align_scratch, uint32_t align_mask, int kv_div) {
-    using C = CrossCfg<FP8>;
+                               float* __restrict__ align_scratch, uint32_t align_mask, int kv_div, const uint8_t* __restrict__ khdr,
+                               const uint8_t* __restrict__ vhdr) {
+    using C = CrossCfg<F>;
+    constexpr bool FP8 = C::FP8, PACKED = F == kCrossPacked;
     extern __shared__ __align__(128) uint8_t smem[];
     const int Tp = (Tlen + 3) & ~3;
     uint8_t* ring = smem;                                                   // C::kStages * 16000
     float* scores = reinterpret_cast<float*>(smem + C::kStages * C::kStageBytes);   // [Tlen]
     float* ksc = scores + Tp;                                               // FP8: [Tlen] K row scales
     float* vsc = ksc + Tp;                                                  // FP8: [Tlen] V row scales
-    float* sq = FP8 ? vsc + Tp : scores + Tp;                               // [64]
+    const int hs = packed_hdr_stride(Tlen);
+    uint8_t* hdr = reinterpret_cast<uint8_t*>(scores + Tp);                 // packed: [2][hs] K then V row headers
+    float* sq = FP8 ? vsc + Tp : PACKED ? reinterpret_cast<float*>(hdr + 2 * hs) : scores + Tp;   // [64]
     float* red = sq + 64;                                                   // [4][64] + scratch
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(red + 4 * 64 + 32);
     uint64_t* empty_bar = full_bar + C::kStages;
-    uint64_t* scale_bar = empty_bar + C::kStages;                           // FP8 only
+    uint64_t* scale_bar = empty_bar + C::kStages;                           // FP8: the row scales, packed: the row headers
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // grid order: (window, head, beam) - the kv_div rows that share one K/V block are adjacent, so their streams meet in L2
@@ -566,7 +588,7 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
     const int ended = done != nullptr ? done[b] : 0;
     if (tid == 0) {
         for (int i = 0; i < C::kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
-        if constexpr (FP8) mbar_init(scale_bar, 1);
+        if constexpr (FP8 || PACKED) mbar_init(scale_bar, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -576,6 +598,43 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
         // ---------------- producer ----------------
         // no griddepcontrol.wait here: the cross K/V cache is written once before the decode loop starts, so when this kernel is
         // launched as a programmatic dependent the first K chunks are already in flight while the upstream GEMM drains
+        if constexpr (PACKED) {
+            // packed: the two header vectors, then per stage the primary slots and a 32-byte copy of the secondary slot of each raw row
+            // into the stage's side area, all on the stage's barrier.  The primary copy is issued before the headers are read, so only
+            // the first stage's raw copies wait for the header load
+            const uint8_t* kb = kcross + (long long)kvh * Tlen * 128;
+            const uint8_t* vb = vcross + (long long)kvh * Tlen * 128;
+            if (lane == 0) {
+                mbar_expect_tx(scale_bar, 2u * hs);
+                bulk_load_1d(hdr, khdr + (long long)kvh * hs, hs, scale_bar);
+                bulk_load_1d(hdr + hs, vhdr + (long long)kvh * hs, hs, scale_bar);
+            }
+            for (int c = 0; c < 2 * chunks; ++c) {
+                const int stage = c % C::kStages;
+                const uint32_t ph = (c / C::kStages) & 1;
+                const int cc = c < chunks ? c : c - chunks;
+                const uint8_t* blk = c < chunks ? kb : vb;
+                uint8_t* dst = ring + stage * C::kStageBytes;
+                mbar_wait(&empty_bar[stage], ph ^ 1);
+                if (lane == 0) {
+                    mbar_expect_tx_only(&full_bar[stage], C::kLoadBytes);
+                    bulk_load_1d(dst, blk + (long long)cc * C::kLoadBytes, C::kLoadBytes, &full_bar[stage]);
+                }
+                mbar_wait(scale_bar, 0);
+                const uint8_t* h = hdr + (c < chunks ? 0 : hs) + cc * C::kRows;
+                int raw = 0;
+                for (int r = lane; r < C::kRows; r += 32)
+                    if (h[r] == kPackedRaw) {
+                        bulk_load_1d(dst + C::kLoadBytes + r * 32, blk + (long long)Tlen * kPackedRowBytes + (long long)(cc * C::kRows + r) * 32, 32,
+                                     &full_bar[stage]);
+                        ++raw;
+                    }
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) raw += __shfl_xor_sync(0xffffffffu, raw, o);
+                if (lane == 0) mbar_expect_tx(&full_bar[stage], 32u * raw);   // the stage's one arrival
+            }
+            return;
+        }
         if (lane == 0) {
             if constexpr (FP8) {
                 mbar_expect_tx(scale_bar, 2u * Tlen * 4);
@@ -608,7 +667,7 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
     float qv[C::kDims];
 #pragma unroll
     for (int j = 0; j < C::kDims; ++j) qv[j] = sq[sub * C::kDims + j];
-    if constexpr (FP8) mbar_wait(scale_bar, 0);
+    if constexpr (FP8 || PACKED) mbar_wait(scale_bar, 0);
 
     // K phase: scores[t] = q . K[t]  (FP8: ksc[t] * (q . code[t]))
     for (int c = 0; c < chunks; ++c) {
@@ -620,7 +679,7 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
         for (int i = 0; i < 8; ++i) {
             const int r = warp * C::kRowsPerWarp + rsel + 4 * C::kRowsPerWarp * i;
             float acc = 0.f;
-            if (r < C::kRows) acc = cross_row_dot<T, FP8>(tile + r * C::kRowBytes + sub * 16, qv);
+            if (r < C::kRows) acc = cross_row_dot<T, F>(cross_piece<F>(tile, r, sub, PACKED ? hdr[c * C::kRows + r] : 0), qv);
 #pragma unroll
             for (int o = 1; o < C::kLanesPerRow; o <<= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
             if (sub == 0 && r < C::kRows) scores[c * C::kRows + r] = FP8 ? acc * ksc[c * C::kRows + r] : acc;
@@ -669,7 +728,7 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
             if (r < C::kRows) {
                 const int t = (c - chunks) * C::kRows + r;
                 const float p = FP8 ? scores[t] * vsc[t] : scores[t];
-                cross_row_axpy<T, FP8>(tile + r * C::kRowBytes + sub * 16, p, acc);
+                cross_row_axpy<T, F>(cross_piece<F>(tile, r, sub, PACKED ? hdr[hs + t] : 0), p, acc);
             }
         }
         __syncwarp();
@@ -692,24 +751,42 @@ decoder_cross_attention_kernel(const float* __restrict__ partial, int splits, in
     }
 }
 
-template <bool FP8> static size_t cross_smem_bytes(int T) {
-    using C = CrossCfg<FP8>;
-    return (size_t)C::kStages * C::kStageBytes + (size_t)((T + 3) & ~3) * 4 * (FP8 ? 3 : 1) + 64 * 4 + (4 * 64 + 32) * 4 +
-           (2 * C::kStages + (FP8 ? 1 : 0)) * 8 + 64;
+template <int F> static size_t cross_smem_bytes(int T) {
+    using C = CrossCfg<F>;
+    return (size_t)C::kStages * C::kStageBytes + (size_t)((T + 3) & ~3) * 4 * (C::FP8 ? 3 : 1) + (F == kCrossPacked ? 2 * packed_hdr_stride(T) : 0) +
+           64 * 4 + (4 * 64 + 32) * 4 + (2 * C::kStages + (F != kCrossRaw16 ? 1 : 0)) * 8 + 64;
 }
 
-template <typename T, bool FP8>
+template <typename T, int F>
 static wk_status launch_cross(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, const float* kscale,
                               const float* vscale, void* out, int B, int H, int Tlen, cudaStream_t stream, const int32_t* done, float* align_scratch,
-                              uint32_t align_mask, int kv_div) {
+                              uint32_t align_mask, int kv_div, const uint8_t* khdr, const uint8_t* vhdr) {
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_kernel<T, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(decoder_cross_attention_kernel<T, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(cross): %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
         attr_set = true;
     }
-    launch_k(decoder_cross_attention_kernel<T, FP8>, dim3(B * H), dim3(kCrossThreads), cross_smem_bytes<FP8>(Tlen), stream, 4, partial, splits, Bp, bq,
-             (const uint8_t*)kcross, (const uint8_t*)vcross, kscale, vscale, (T*)out, B, H, Tlen, done, align_scratch, align_mask, kv_div);
+    launch_k(decoder_cross_attention_kernel<T, F>, dim3(B * H), dim3(kCrossThreads), cross_smem_bytes<F>(Tlen), stream, 4, partial, splits, Bp, bq,
+             (const uint8_t*)kcross, (const uint8_t*)vcross, kscale, vscale, (T*)out, B, H, Tlen, done, align_scratch, align_mask, kv_div, khdr, vhdr);
+    return WK_OK;
+}
+
+__global__ void cross_kv_unpack_kernel(const uint8_t* __restrict__ packed, const uint8_t* __restrict__ hdr, uint4* __restrict__ out, int64_t groups, int T) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // group of 8 values
+    if (i >= groups) return;
+    const int64_t row = i >> 3, blk = row / T;
+    const int t = (int)(row - blk * T);
+    out[i] = packed_group(packed + blk * T * 128, T, t, (int)(i & 7), hdr[blk * packed_hdr_stride(T) + t]);
+}
+
+wk_status cross_kv_unpack(const void* packed, const uint8_t* hdr, void* out, int64_t blocks, int T, cudaStream_t stream) {
+    const int64_t groups = blocks * T * 8;
+    if (groups == 0) return WK_OK;
+    cross_kv_unpack_kernel<<<(unsigned)((groups + 255) / 256), 256, 0, stream>>>((const uint8_t*)packed, hdr, (uint4*)out, groups, T);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("cross_kv_unpack launch: %s", cudaGetErrorString(e)); return WK_ERR_CUDA; }
     return WK_OK;
 }
 
@@ -741,19 +818,21 @@ wk_status decoder_align_mean(const float* scratch, int n_slots, const int32_t* s
 wk_status decoder_cross_attention(const float* partial, int splits, int Bp, const float* bq, const void* kcross,
                                   const void* vcross, void* out, int B, int H, int T, int dtype, cudaStream_t stream,
                                   const int32_t* done, float* align_scratch, uint32_t align_mask, int kv_div, const float* kscale,
-                                  const float* vscale, bool single_query) {
+                                  const float* vscale, bool single_query, const uint8_t* khdr, const uint8_t* vhdr) {
     const bool fp8 = kscale != nullptr;
     if (kv_div < 1 || B % kv_div != 0) { set_error("decoder_cross_attention: %d rows do not split into groups of %d", B, kv_div); return WK_ERR_INVALID_ARGUMENT; }
     if (!fp8 && T % kCrossRows != 0) { set_error("decoder_cross_attention: n_audio_ctx %d not a multiple of %d", T, kCrossRows); return WK_ERR_INVALID_ARGUMENT; }
     if (kv_div > 1 && kv_div <= 8 && align_scratch == nullptr && !single_query)   // beam search: one CTA per (window, head) serves all beams from one K/V pass
-        return decoder_cross_attention_mq(partial, splits, Bp, bq, kcross, vcross, out, B, H, T, dtype, stream, done, kv_div, kscale, vscale);
+        return decoder_cross_attention_mq(partial, splits, Bp, bq, kcross, vcross, out, B, H, T, dtype, stream, done, kv_div, kscale, vscale, khdr, vhdr);
     // FP8: the scale vectors are bulk-copied, so T * 4 bytes per (window, head) must keep 16-byte alignment
-    if (fp8 && (T % CrossCfg<true>::kRows != 0 || T % 4 != 0)) { set_error("decoder_cross_attention (fp8): n_audio_ctx %d not a multiple of 500", T); return WK_ERR_INVALID_ARGUMENT; }
+    if (fp8 && (T % CrossCfg<kCrossFp8>::kRows != 0 || T % 4 != 0)) { set_error("decoder_cross_attention (fp8): n_audio_ctx %d not a multiple of 500", T); return WK_ERR_INVALID_ARGUMENT; }
     const bool f16 = dtype == WK_DTYPE_F16;
-    wk_status st = fp8 ? (f16 ? launch_cross<__half, true>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div)
-                              : launch_cross<__nv_bfloat16, true>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div))
-                       : (f16 ? launch_cross<__half, false>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div)
-                              : launch_cross<__nv_bfloat16, false>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div));
+    if (khdr && (fp8 || f16 || !vhdr)) { set_error("decoder_cross_attention: the packed cache is bf16 and needs both header vectors"); return WK_ERR_INVALID_ARGUMENT; }
+#define WK_CROSS(TT, FF) launch_cross<TT, FF>(partial, splits, Bp, bq, kcross, vcross, kscale, vscale, out, B, H, T, stream, done, align_scratch, align_mask, kv_div, khdr, vhdr)
+    wk_status st = khdr ? WK_CROSS(__nv_bfloat16, kCrossPacked)
+                 : fp8 ? (f16 ? WK_CROSS(__half, kCrossFp8) : WK_CROSS(__nv_bfloat16, kCrossFp8))
+                       : (f16 ? WK_CROSS(__half, kCrossRaw16) : WK_CROSS(__nv_bfloat16, kCrossRaw16));
+#undef WK_CROSS
     if (st != WK_OK) return st;
     count_launch();
     cudaError_t e = cudaGetLastError();

@@ -1393,6 +1393,59 @@ wk_status wk_test_cross_attention_fp8(wk_model* m, const float* q, const uint8_t
     return r;
 }
 
+wk_status wk_test_cross_kv_project(wk_model* m, const void* x, const void* w, const float* bias, int32_t windows, int32_t T, int32_t H,
+                                   int32_t packed, void* out, uint8_t* hdr) {
+    if (!m || !x || !w || !out || (packed && !hdr) || windows < 1 || T < 1 || H < 1) { set_error("wk_test_cross_kv_project: bad arguments"); return WK_ERR_INVALID_ARGUMENT; }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    const int d = H * 64;
+    GemmDesc g = plain_gemm(x, (int64_t)windows * T, d, w, d, WK_DTYPE_BF16, packed ? GEMM_OUT_PACKED_HEADS : GEMM_OUT_T16_HEADS, out, 0, bias, 0);
+    g.heads_T = T; g.heads_B = windows; g.heads_H = H; g.heads_dmodel = d;
+    g.out_hdr = packed ? hdr : nullptr;
+    wk_status r = gemm_wgmma(g, m->num_sms, m->stream);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_kv_project: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+wk_status wk_test_cross_attention_packed(wk_model* m, const float* q, const void* kc, const void* vc, const uint8_t* khdr, const uint8_t* vhdr,
+                                         void* out, int32_t B, int32_t H, int32_t T, const int32_t* done, int32_t kv_div, float* align_out) {
+    if (!m || !q || !kc || !vc || !khdr || !vhdr || !out || B < 1 || H < 1 || H > 32 || kv_div < 1) {
+        set_error("wk_test_cross_attention_packed: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    Buffers scratch;
+    float* zero = nullptr;
+    WK_CHECK(scratch.dmalloc(&zero, (size_t)H * 64));
+    const uint32_t all_heads = H == 32 ? 0xffffffffu : (1u << H) - 1u;
+    wk_status r = decoder_cross_attention(q, 1, B, zero, kc, vc, out, B, H, T, WK_DTYPE_BF16, m->stream, done, align_out, align_out ? all_heads : 0u,
+                                          kv_div, nullptr, nullptr, false, khdr, vhdr);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_cross_attention_packed: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
+wk_status wk_test_align_cross_attention(wk_model* m, const void* q, const void* kc, const void* vc, const uint8_t* khdr, const uint8_t* vhdr,
+                                        const int32_t* seq_len, int32_t nw, int32_t H, int32_t T, uint32_t mask, void* out, float* acc) {
+    if (!m || !q || !kc || !vc || !seq_len || !out || !acc || nw < 1 || H < 1 || H > 32 || (!khdr != !vhdr)) {
+        set_error("wk_test_align_cross_attention: bad arguments");
+        return WK_ERR_INVALID_ARGUMENT;
+    }
+    WK_CUDA_CHECK(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> lock(m->api_mu);
+    const int64_t rows = (int64_t)nw * 224;
+    Buffers scratch;
+    float* stats = nullptr;
+    WK_CHECK(scratch.dmalloc(&stats, (size_t)2 * H * rows));
+    wk_status r = align_cross_attention(q, kc, vc, nullptr, nullptr, seq_len, 0, out, stats, rows, nw, H, T, WK_DTYPE_BF16, m->stream, khdr, vhdr);
+    if (r == WK_OK && mask) r = align_export(q, kc, nullptr, stats, rows, seq_len, 0, mask, 1, acc, nw, H, T, WK_DTYPE_BF16, m->stream, khdr);
+    cudaError_t e = cudaStreamSynchronize(m->stream);
+    if (r == WK_OK && e != cudaSuccess) { set_error("wk_test_align_cross_attention: %s", cudaGetErrorString(e)); r = WK_ERR_CUDA; }
+    return r;
+}
+
 // decoder_self_attention_kernel alone: qkv [B][3*H*64] f32 (q | k | v of the new token, biases included), caches [B][H][224][64] 16-bit
 // holding positions < pos[b]; appends the new K/V row at pos[b] and writes out [B][H*64]
 wk_status wk_test_self_attention(wk_model* m, const float* qkv, void* kcache, void* vcache, const int32_t* pos, void* out, int32_t B,

@@ -24,6 +24,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -54,6 +55,7 @@ struct GemmKParams {
     long long ld_pos;
     int heads_T, heads_B, heads_H, heads_dmodel;
     float* out_scale;
+    uint8_t* out_hdr;
     int a_static;     // see GemmDesc::a_static
 };
 
@@ -63,11 +65,13 @@ struct GemmKParams {
 //   kEpiStore16   GEMM_OUT_T16 / GEMM_OUT_T16_HEADS and kEpiStore32  GEMM_OUT_F32 / _F32_ADD / _F32_GELU_POS: the per-element math in
 //                 registers, the tile through a shared-memory staging box and TMA bulk tensor stores (gemm_epilogue_store16 / _store32)
 //   kEpiFp8Blocks GEMM_OUT_FP8_BLOCKS (FP8 kernel only), per-row block quantization in registers (gemm_epilogue_fp8_blocks)
-enum GemmEpi { kEpiPartialT = 0, kEpiFp8Heads = 1, kEpiStore16 = 2, kEpiStore32 = 3, kEpiFp8Blocks = 4 };
+//   kEpiPackedHeads GEMM_OUT_PACKED_HEADS, the packed bf16 rows from the registers (gemm_epilogue_packed_heads)
+enum GemmEpi { kEpiPartialT = 0, kEpiFp8Heads = 1, kEpiStore16 = 2, kEpiStore32 = 3, kEpiFp8Blocks = 4, kEpiPackedHeads = 5 };
 static int gemm_epi(int mode) {
     switch (mode) {
         case GEMM_OUT_PARTIAL_T: return kEpiPartialT;
         case GEMM_OUT_FP8_HEADS: return kEpiFp8Heads;
+        case GEMM_OUT_PACKED_HEADS: return kEpiPackedHeads;
         case GEMM_OUT_T16: case GEMM_OUT_T16_HEADS: return kEpiStore16;
         default: return kEpiStore32;
     }
@@ -272,6 +276,78 @@ __device__ __forceinline__ void gemm_epilogue_fp8_heads(const GemmKParams& p, in
     }
 }
 
+// GEMM_OUT_PACKED_HEADS epilogue of one thread, same fragments as gemm_epilogue_fp8_heads: acc + bias rounded to bf16 as the T16 heads
+// path rounds it, the row's exponent range from quad shuffles, then the packed row (common.cuh): lane q holds values 8 jj + 2q, + 1 of every
+// group jj, so it writes their two sign|mantissa bytes and, once the quad has OR-ed its nibbles together, the nibble words of groups 2q, 2q + 1
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_packed_heads(const GemmKParams& p, int batch, int tile_row0, int r_lo, int c_lo, int col_base,
+                                                           const float (&acc)[BN / 2]) {
+    static_assert(BN % 64 == 0, "packed heads epilogue needs head-aligned N tiles");
+    const int q = c_lo >> 1;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        const int row_in_batch = tile_row0 + r_lo + 8 * half;
+        const long long grow = (long long)batch * p.out_rows_per_batch + row_in_batch;
+        const int b = (int)(grow / p.heads_T);
+        const int tt = (int)(grow - (long long)b * p.heads_T);
+#pragma unroll
+        for (int hh = 0; hh < BN / 64; ++hh) {
+            const int col0 = col_base + hh * 64;
+            const bool col_ok = col0 < p.n;
+            uint32_t w[8];
+            uint32_t emax = 0, emin = 255;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                const int j = hh * 8 + jj;
+                float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+                if (p.bias && col_ok) {
+                    const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * jj + c_lo));
+                    v0 += bb.x; v1 += bb.y;
+                }
+                w[jj] = T16<__nv_bfloat16>::pack2(v0, v1);
+                const uint32_t e0 = (w[jj] >> 7) & 0xffu, e1 = (w[jj] >> 23) & 0xffu;
+                emax = max(emax, max(e0, e1));
+                emin = min(emin, min(e0, e1));
+            }
+            emax = max(emax, __shfl_xor_sync(0xffffffffu, emax, 1));
+            emax = max(emax, __shfl_xor_sync(0xffffffffu, emax, 2));
+            emin = min(emin, __shfl_xor_sync(0xffffffffu, emin, 1));
+            emin = min(emin, __shfl_xor_sync(0xffffffffu, emin, 2));
+            const bool raw = emax == 255u || emax - emin > 15u;   // uniform over the quad
+            uint32_t nib[8];
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                nib[jj] = raw ? 0u : ((emax - ((w[jj] >> 7) & 0xffu)) << (4 * q)) | ((emax - ((w[jj] >> 23) & 0xffu)) << (16 + 4 * q));
+                nib[jj] |= __shfl_xor_sync(0xffffffffu, nib[jj], 1);
+                nib[jj] |= __shfl_xor_sync(0xffffffffu, nib[jj], 2);
+            }
+            if (!col_ok || row_in_batch >= p.m_rows_per_batch) continue;
+            const int which = col0 / p.heads_dmodel;
+            const int h = (col0 - which * p.heads_dmodel) >> 6;
+            const long long blk = ((long long)which * p.heads_B + b) * p.heads_H + h;
+            uint8_t* base = reinterpret_cast<uint8_t*>(p.out) + blk * p.heads_T * 128;
+            uint8_t* row = base + (long long)tt * kPackedRowBytes;
+            if (raw) {
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                    uint8_t* dst = jj < 6 ? row + 16 * jj + 2 * c_lo : base + (long long)p.heads_T * kPackedRowBytes + (long long)tt * 32 + 16 * (jj - 6) + 2 * c_lo;
+                    *reinterpret_cast<uint32_t*>(dst) = w[jj];
+                }
+            } else {
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {   // sign|mantissa bytes of values 8 jj + c_lo, + 1
+                    const uint32_t lo = ((w[jj] >> 8) & 0x80u) | (w[jj] & 0x7fu), hi = ((w[jj] >> 24) & 0x80u) | ((w[jj] >> 16) & 0x7fu);
+                    *reinterpret_cast<uint16_t*>(row + 8 * jj + c_lo) = (uint16_t)(lo | (hi << 8));
+                }
+#pragma unroll
+                for (int jj = 0; jj < 8; jj += 2)
+                    if ((jj >> 1) == q) *reinterpret_cast<uint2*>(row + 64 + 4 * jj) = make_uint2(nib[jj], nib[jj + 1]);
+            }
+            if (c_lo == 0) p.out_hdr[blk * packed_hdr_stride(p.heads_T) + tt] = raw ? kPackedRaw : (uint8_t)emax;
+        }
+    }
+}
+
 template <typename T, int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
@@ -418,6 +494,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
         if constexpr (EPI == kEpiFp8Heads) {
             gemm_epilogue_fp8_heads<BN>(p, batch, tile_row0, r_lo, c_lo, col_base, acc);
+        } else if constexpr (EPI == kEpiPackedHeads) {
+            gemm_epilogue_packed_heads<BN>(p, batch, tile_row0, r_lo, c_lo, col_base, acc);
         } else if constexpr (EPI == kEpiStore16) {
             if (wg_rows) gemm_epilogue_store16<T, BN>(p, &tmO, acc, my_stage, sbuf, wg_tid, cw, batch, wg_row0, col_base);
         } else if constexpr (EPI == kEpiStore32) {
@@ -709,6 +787,9 @@ static cudaError_t launch_gemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB,
                                  size_t smem, int pdl, cudaStream_t stream) {
     switch (gemm_epi(p.mode)) {
         case kEpiFp8Heads: return launch_gemm<T, 256, kEpiFp8Heads>(tmA, tmB, tmO, p, grid, smem, pdl, stream);   // bn checked by gemm_wgmma
+        case kEpiPackedHeads:
+            if constexpr (std::is_same<T, __nv_bfloat16>::value) return launch_gemm<T, 256, kEpiPackedHeads>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
+            return cudaErrorInvalidValue;   // bf16 only (checked by gemm_wgmma)
         case kEpiStore16: return launch_gemm_store<T, kEpiStore16>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
         case kEpiStore32: return launch_gemm_store<T, kEpiStore32>(tmA, tmB, tmO, p, grid, smem, pdl, stream);
         default: break;
@@ -779,6 +860,11 @@ wk_status gemm_wgmma(const GemmDesc& d, int num_sms, cudaStream_t stream) {
     p.ld_pos = d.ld_pos;
     p.heads_T = d.heads_T; p.heads_B = d.heads_B; p.heads_H = d.heads_H; p.heads_dmodel = d.heads_dmodel;
     p.out_scale = d.out_scale;
+    p.out_hdr = d.out_hdr;
+    if (d.mode == GEMM_OUT_PACKED_HEADS && (p.bn != 256 || d.n % 64 != 0 || d.heads_dmodel % 64 != 0 || !d.out_hdr || d.in_dtype != WK_DTYPE_BF16)) {
+        set_error("gemm_wgmma: the packed heads epilogue needs bf16, 256-column tiles and head-aligned columns (bn %d n %d d %d)", p.bn, d.n, d.heads_dmodel);
+        return WK_ERR_INVALID_ARGUMENT;
+    }
     if (d.mode == GEMM_OUT_FP8_HEADS && (p.bn != 256 || d.n % 64 != 0 || d.heads_dmodel % 64 != 0 || !d.out_scale)) {
         // the row amax is taken over whole heads inside one N tile
         set_error("gemm_wgmma: the FP8 heads epilogue needs 256-column tiles and head-aligned columns (bn %d n %d d %d)", p.bn, d.n, d.heads_dmodel);

@@ -70,6 +70,7 @@ enum GemmMode {
     GEMM_OUT_F32 = 5,        // out32[row, col] = acc + bias[col]
     GEMM_OUT_FP8_HEADS = 6,  // out8[which][b][h][t][64] E4M3 codes + out_scale[which][b][h][t] f32 (FP8 cross-attention K/V cache)
     GEMM_OUT_FP8_BLOCKS = 7, // out8[row, col] E4M3 codes of act(acc + bias[col]) + out_scale[col / 128][row] f32 (FP8 encoder FC1)
+    GEMM_OUT_PACKED_HEADS = 8,  // packed bf16 rows in the [which][b][h] blocks of T x 128 bytes + out_hdr[which][b][h][round_up(T, 16)] (common.cuh)
 };
 
 struct GemmDesc {
@@ -109,6 +110,7 @@ struct GemmDesc {
     // HEADS scatter
     int heads_T, heads_B, heads_H, heads_dmodel;
     float* out_scale;        // FP8_HEADS: one scale per 64-value row
+    uint8_t* out_hdr;        // PACKED_HEADS: one header byte per 64-value row
     int pdl;                // launch with programmatic dependent launch (decode-step chain)
     int max_stages;          // 0 = as many smem stages as fit; >0 caps the ring (lets other kernels co-reside on the SM)
     int a_static;            // A operand (weights) does not depend on the upstream kernel: with PDL its first tiles are fetched before griddepcontrol.wait
@@ -292,14 +294,19 @@ wk_status decoder_kv_append(const float* partial, int splits, int Bp, const floa
 wk_status decoder_cross_attention(const float* partial, int splits, int Bp, const float* bq, const void* kcross,
                                   const void* vcross, void* out, int B, int H, int T, int dtype, cudaStream_t stream,
                                   const int32_t* done = nullptr, float* align_scratch = nullptr, uint32_t align_mask = 0, int kv_div = 1,
-                                  const float* kscale = nullptr, const float* vscale = nullptr, bool single_query = false);
+                                  const float* kscale = nullptr, const float* vscale = nullptr, bool single_query = false,
+                                  const uint8_t* khdr = nullptr, const uint8_t* vhdr = nullptr);
+// khdr / vhdr != nullptr: the packed bf16 cache (common.cuh), header vectors [B / kv_div][H][round_up(T, 16)]
+// rows [0, blocks * T) of packed blocks -> the 16-bit [blocks][T][64] layout
+wk_status cross_kv_unpack(const void* packed, const uint8_t* hdr, void* out, int64_t blocks, int T, cudaStream_t stream);
 // kv_div > 1 (beam search): row b reads the K/V block of window b / kv_div; the CTAs of one (window, head) are adjacent in the grid so that
 // their K/V stream is shared through L2.  single_query: never the tensor-core form below (its arithmetic differs): every row computes
 // exactly what it would as the only row of its window
 // tensor-core variant for nq = 2..8 rows per K/V block (cross_attention_mq.cu): one K/V stream per (window, head) serves all nq beams
 wk_status decoder_cross_attention_mq(const float* partial, int splits, int Bp, const float* bq, const void* kcross, const void* vcross, void* out, int B, int H,
                                      int Tlen, int dtype, cudaStream_t stream, const int32_t* done, int nq,
-                                     const float* kscale = nullptr, const float* vscale = nullptr);
+                                     const float* kscale = nullptr, const float* vscale = nullptr, const uint8_t* khdr = nullptr,
+                                     const uint8_t* vhdr = nullptr);
 // alignment row of the step just sampled (run AFTER the sampler advanced steps[b] to tokenIndex + 1): out[b][steps[b]][t] =
 // Float16(mean over n_slots of scratch[slot][b][t]) unless done[b] (TextDecoder.updateAlignmentWeights, TextDecoder.swift:272-296:
 // the slice of step tokenIndex lands in row tokenIndex + 1; a completed segment breaks out before the update, :668-674)
@@ -350,13 +357,14 @@ wk_status draft_accept(DecodeState st, int32_t* anc, DraftRound R, cudaStream_t 
 wk_status align_embed(const void* emb, const float* pos_emb, const int32_t* row_tok, float* x, int64_t rows, int d, int dtype, cudaStream_t stream);
 // causal self-attention over the [rows][3d] QKV output (biases already added) -> out [rows][d]
 wk_status align_self_attention(const void* qkv, const int32_t* seq_len, void* out, int nw, int H, int dtype, cudaStream_t stream);
-// q [rows][d] (16-bit) against the layer's cache block; kscale / vscale != nullptr: the FP8 cache.  stats != nullptr: each row's final softmax
+// q [rows][d] (16-bit) against the layer's cache block; kscale / vscale != nullptr: the FP8 cache, khdr / vhdr: the packed bf16 cache.  stats != nullptr: each row's final softmax
 // (max, sum) per head as float pairs [H][stat_rows]
 wk_status align_cross_attention(const void* q, const void* kc, const void* vc, const float* kscale, const float* vscale, const int32_t* seq_len,
-                                int slot0, void* out, float* stats, int64_t stat_rows, int nw, int H, int Tlen, int dtype, cudaStream_t stream);
+                                int slot0, void* out, float* stats, int64_t stat_rows, int nw, int H, int Tlen, int dtype, cudaStream_t stream,
+                                const uint8_t* khdr = nullptr, const uint8_t* vhdr = nullptr);
 // acc[row][T] (f32) += the normalised softmax rows of the heads in `mask`, ascending (first != 0: acc starts at 0)
 wk_status align_export(const void* q, const void* kc, const float* kscale, const float* stats, int64_t stat_rows, const int32_t* seq_len, int slot0,
-                       uint32_t mask, int first, float* acc, int nw, int H, int Tlen, int dtype, cudaStream_t stream);
+                       uint32_t mask, int first, float* acc, int nw, int H, int Tlen, int dtype, cudaStream_t stream, const uint8_t* khdr = nullptr);
 // Float16 alignmentWeights [nw][store_rows][T]: row t + 1 = acc[position t] / n_slots, row 0 and rows past the sequence 0
 wk_status align_rows_f16(const float* acc, const int32_t* seq_len, int n_slots, void* out, int nw, int Tlen, int store_rows, cudaStream_t stream);
 // logits rows [r0, r0 + rows) of the pass ([rows][ld] f32): out[r + 1] = log softmax(logits[r][:eot])[row_tok[r + 1]], NaN for targets >= eot

@@ -39,6 +39,9 @@ struct wk_session {
     void* cross_kv = nullptr;   // [2L][S][H][T][64] model dtype, or E4M3 codes when ckv_fp8
     float* cross_scale = nullptr;   // ckv_fp8: [2L][S][H][T] row scales
     bool ckv_fp8 = false;
+    // bf16 models (no FP8 cache): the cache holds packed rows (common.cuh) with their headers [2L][S][H][round_up(T, 16)]
+    bool ckv_packed = false;
+    uint8_t* cross_hdr = nullptr;
     void* self_k = nullptr;     // [L][S][H][224][64]
     void* self_v = nullptr;
     float* partial = nullptr; size_t partial_elems = 0;
@@ -88,7 +91,7 @@ struct wk_session {
     // (one row per slot) and cross K/V (the session's storage policy), its decode state, and the rounds' device bookkeeping
     int draft_k = 0;                   // proposals per round of the current call, 0 = no draft
     bool draft_ready = false;
-    void* dr_self_k = nullptr; void* dr_self_v = nullptr; void* dr_cross_kv = nullptr; float* dr_cross_scale = nullptr;
+    void* dr_self_k = nullptr; void* dr_self_v = nullptr; void* dr_cross_kv = nullptr; float* dr_cross_scale = nullptr; uint8_t* dr_cross_hdr = nullptr;
     DecodeState dst; RowParams* drp = nullptr;
     DraftRound dr = DraftRound();
     int64_t draft_stats[3] = {0, 0, 0};   // of the last batched call: rounds that verified, proposals verified, proposals accepted
@@ -174,10 +177,11 @@ static GemmDesc cross_kv_gemm(const wk_session* s, const void* src, int cnt, int
     void* cache = draft ? s->dr_cross_kv : s->cross_kv;
     float* scale = draft ? s->dr_cross_scale : s->cross_scale;
     GemmDesc g = plain_gemm(src, (int64_t)cnt * T, c.d_model, w.wckv, 2 * w.n_layers * c.d_model, c.dtype,
-                            s->ckv_fp8 ? GEMM_OUT_FP8_HEADS : GEMM_OUT_T16_HEADS, (char*)cache + (size_t)q0 * H * T * 64 * ckv_esize(s), 0,
+                            s->ckv_fp8 ? GEMM_OUT_FP8_HEADS : s->ckv_packed ? GEMM_OUT_PACKED_HEADS : GEMM_OUT_T16_HEADS, (char*)cache + (size_t)q0 * H * T * 64 * ckv_esize(s), 0,
                             w.bckv, 0);
     g.heads_T = T; g.heads_B = draft ? draft_slots(s) : s->max_batch; g.heads_H = H; g.heads_dmodel = c.d_model;
     if (s->ckv_fp8) g.out_scale = scale + (size_t)q0 * H * T;
+    if (s->ckv_packed) g.out_hdr = (draft ? s->dr_cross_hdr : s->cross_hdr) + (size_t)q0 * H * packed_hdr_stride(T);
     return g;
 }
 
@@ -188,7 +192,7 @@ static GemmDesc cross_kv_gemm(const wk_session* s, const void* src, int cnt, int
 struct DecPass {
     DecoderWeights w;
     int cap;                       // rows (or window slots) the caches hold per layer
-    void* self_k; void* self_v; void* cross_kv; float* cross_scale;
+    void* self_k; void* self_v; void* cross_kv; float* cross_scale; uint8_t* cross_hdr;
     DecodeState st;
     int B, Bp, kv_div;
     const int32_t* anc;
@@ -217,13 +221,17 @@ static wk_status decoder_pass(wk_session* s, const DecPass& P, int ts_begin, con
         if (P.verify) WK_CHECK(decoder_kv_append(s->partial, sp, Bp, l.bv, kc, vc, pos, done, B, H, kKvMaxLen, dt, st));
         return decoder_self_attention(s->partial, sp, Bp, l.bq, l.bv, kc, vc, pos, done, s->attn, B, H, kKvMaxLen, dt, st, P.anc);
     };
+    const size_t hdr_block = (size_t)P.cap * H * packed_hdr_stride(T);   // header bytes per (layer, k|v)
     auto cross_attn = [&](int li, const DecLayer& l) {
         const bool align = P.align && m->align_mask[li] != 0;
-        return decoder_cross_attention(s->partial, sp, Bp, l.bcq, (char*)P.cross_kv + (size_t)(2 * li) * cross_block,
-                                       (char*)P.cross_kv + (size_t)(2 * li + 1) * cross_block, s->attn, B, H, T, dt, st, done,
+        const char* kc = (const char*)P.cross_kv + (size_t)(2 * li) * cross_block;
+        const char* vc = (const char*)P.cross_kv + (size_t)(2 * li + 1) * cross_block;
+        const uint8_t* kh = s->ckv_packed ? P.cross_hdr + (2 * li) * hdr_block : nullptr;
+        const uint8_t* vh = s->ckv_packed ? P.cross_hdr + (2 * li + 1) * hdr_block : nullptr;
+        return decoder_cross_attention(s->partial, sp, Bp, l.bcq, kc, vc, s->attn, B, H, T, dt, st, done,
                                        align ? s->align_scratch + (size_t)m->align_base[li] * B * T : nullptr, align ? m->align_mask[li] : 0u,
                                        P.kv_div, s->ckv_fp8 ? P.cross_scale + (2 * li) * cross_rows : nullptr,
-                                       s->ckv_fp8 ? P.cross_scale + (2 * li + 1) * cross_rows : nullptr, P.verify);
+                                       s->ckv_fp8 ? P.cross_scale + (2 * li + 1) * cross_rows : nullptr, P.verify, kh, vh);
     };
     for (int li = 0; li < n_layers; ++li) {
         const DecLayer& l = P.w.layers[li];
@@ -260,7 +268,7 @@ static wk_status decoder_forward(wk_session* s, int ts_begin, const int32_t* exp
     const bool loop = !explicit_pos;
     // loop mode: the window's G rows share one cross K/V block; beam rows and draft verification rows read the self K/V through the
     // cache ancestry
-    DecPass P{s->m->main_decoder(), s->max_batch, s->self_k, s->self_v, s->cross_kv, s->cross_scale, s->st, s->batch, s->bp,
+    DecPass P{s->m->main_decoder(), s->max_batch, s->self_k, s->self_v, s->cross_kv, s->cross_scale, s->cross_hdr, s->st, s->batch, s->bp,
               loop ? std::max(1, s->bs.group) : 1, loop && s->bs.use_anc ? s->bs.anc : nullptr, loop && s->draft_k > 0, loop && s->align_on};
     return decoder_pass(s, P, ts_begin, explicit_pos, check_done);
 }
@@ -397,7 +405,7 @@ static wk_status enqueue_draft_steps(wk_session* s, const wk_special_tokens* st)
     wk_model* m = s->m;
     const int slots = s->dr.slots;
     WK_CHECK(draft_round_begin(s->st, s->dst, s->drp, s->dr, s->stream));
-    DecPass P{m->draft->view(), draft_slots(s), s->dr_self_k, s->dr_self_v, s->dr_cross_kv, s->dr_cross_scale, s->dst, slots, round_up(slots, 16), 1, nullptr, false, false};
+    DecPass P{m->draft->view(), draft_slots(s), s->dr_self_k, s->dr_self_v, s->dr_cross_kv, s->dr_cross_scale, s->dr_cross_hdr, s->dst, slots, round_up(slots, 16), 1, nullptr, false, false};
     SamplerParams sp = loop_sampler_params(s, st);
     sp.beam = BeamState();
     sp.rng_div = 1;
@@ -545,6 +553,7 @@ static wk_status ensure_draft(wk_session* s) {
         WK_CHECK(b.dmalloc(&s->dr_cross_scale, (size_t)2 * Ld * S * H * T));
     } else {
         WK_CHECK(b.alloc16(&s->dr_cross_kv, (size_t)2 * Ld * S * H * T * 64));
+        if (s->ckv_packed) WK_CHECK(b.dmalloc(&s->dr_cross_hdr, (size_t)2 * Ld * S * H * packed_hdr_stride(T)));
     }
     WK_CHECK(b.alloc16(&s->dr_self_k, (size_t)Ld * S * H * kKvMaxLen * 64));
     WK_CHECK(b.alloc16(&s->dr_self_v, (size_t)Ld * S * H * kKvMaxLen * 64));
@@ -1262,9 +1271,12 @@ static wk_status align_chunk(wk_session* s, const wk_special_tokens* st, int slo
         const char* vc = (const char*)s->cross_kv + (size_t)(2 * li + 1) * cross_block;
         const float* ksc = s->ckv_fp8 ? s->cross_scale + (size_t)(2 * li) * cross_rows : nullptr;
         const float* vsc = s->ckv_fp8 ? s->cross_scale + (size_t)(2 * li + 1) * cross_rows : nullptr;
-        WK_CHECK(align_cross_attention(ws.qkv, kc, vc, ksc, vsc, s->al_seq, slot0, ws.attn, mask ? s->al_stats : nullptr, R, nw, H, T, dt, stm));
+        const size_t hb = (size_t)s->max_batch * H * packed_hdr_stride(T);
+        const uint8_t* kh = s->ckv_packed ? s->cross_hdr + (2 * li) * hb : nullptr;
+        const uint8_t* vh = s->ckv_packed ? s->cross_hdr + (2 * li + 1) * hb : nullptr;
+        WK_CHECK(align_cross_attention(ws.qkv, kc, vc, ksc, vsc, s->al_seq, slot0, ws.attn, mask ? s->al_stats : nullptr, R, nw, H, T, dt, stm, kh, vh));
         if (mask) {
-            WK_CHECK(align_export(ws.qkv, kc, ksc, s->al_stats, R, s->al_seq, slot0, mask, first_align, s->al_acc, nw, H, T, dt, stm));
+            WK_CHECK(align_export(ws.qkv, kc, ksc, s->al_stats, R, s->al_seq, slot0, mask, first_align, s->al_acc, nw, H, T, dt, stm, kh));
             first_align = 0;
         }
         WK_CHECK(gemm(ws.attn, d, l.wco, d, GEMM_OUT_F32_ADD, ws.x, l.bco, 0));
@@ -1398,6 +1410,8 @@ wk_status wk_session_create(wk_model* m, int32_t max_batch, wk_session** out) {
         WK_CHECK(b.dmalloc(&s->cross_scale, (size_t)2 * L * S * H * T));
     } else {
         WK_CHECK(b.alloc16(&s->cross_kv, (size_t)2 * L * S * H * T * 64));
+        s->ckv_packed = c.dtype == WK_DTYPE_BF16;
+        if (s->ckv_packed) WK_CHECK(b.dmalloc(&s->cross_hdr, (size_t)2 * L * S * H * packed_hdr_stride(T)));
     }
     WK_CHECK(b.alloc16(&s->self_k, (size_t)L * S * H * kKvMaxLen * 64));
     WK_CHECK(b.alloc16(&s->self_v, (size_t)L * S * H * kKvMaxLen * 64));
@@ -1840,6 +1854,9 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
     const size_t cross_block = cross_rows * 64 * ckv_esize(s);
     const float* ksc = s->ckv_fp8 ? s->cross_scale : nullptr;
     const float* vsc = s->ckv_fp8 ? s->cross_scale + cross_rows : nullptr;
+    const size_t hs = packed_hdr_stride(T);
+    const uint8_t* kh = s->ckv_packed ? s->cross_hdr : nullptr;
+    const uint8_t* vh = s->ckv_packed ? s->cross_hdr + (size_t)s->max_batch * H * hs : nullptr;
     if (which == 9 && !s->pos100) {
         std::vector<int32_t> h(256, 100);
         WK_CHECK(s->mem.dmalloc(&s->pos100, 256, false));
@@ -1850,7 +1867,7 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
         int sp;
         switch (which) {
             case 0: return decoder_cross_attention(s->partial, 1, s->bp, m->dec[0].bcq, s->cross_kv, (char*)s->cross_kv + cross_block, s->attn, B, H, T, dt, st,
-                                                   nullptr, nullptr, 0, 1, ksc, vsc);
+                                                   nullptr, nullptr, 0, 1, ksc, vsc, false, kh, vh);
             case 1: return gemm_wgmma(plain_gemm(s->ws.xn, M, d, m->enc[0].w1, 4 * d, dt, GEMM_OUT_T16, s->ws.ffn, 4 * d, m->enc[0].b1, 1), m->num_sms, st);
             case 2: return mel_forward(&m->mel_tables, s->ws.pcm_dev, B, kWindowSamples, nullptr, s->ws.mel, s->ws.gmax, st);
             case 3: return encoder_attention(s->ws.qkv, s->ws.attn, B, T, H, dt, st);
@@ -1872,7 +1889,18 @@ wk_status wk_bench_kernel(wk_model* m, wk_session* s, int32_t which, int32_t bat
         }
     };
     switch (which) {
-        case 0: *work_out = (double)B * H * T * (64 * (double)ckv_esize(s) + (s->ckv_fp8 ? 4 : 0)) * 2; break;   // K + V bytes (+ FP8 row scales)
+        case 0:   // K + V bytes (+ FP8 row scales; packed: primary slots, header vectors and the secondary slots of raw rows)
+            *work_out = (double)B * H * T * (64 * (double)ckv_esize(s) + (s->ckv_fp8 ? 4 : 0)) * 2;
+            if (s->ckv_packed) {
+                std::vector<uint8_t> hk((size_t)B * H * hs), hv(hk.size());
+                WK_CUDA_CHECK(cudaMemcpy(hk.data(), kh, hk.size(), cudaMemcpyDeviceToHost));
+                WK_CUDA_CHECK(cudaMemcpy(hv.data(), vh, hv.size(), cudaMemcpyDeviceToHost));
+                size_t raw = 0;
+                for (size_t blk = 0; blk < (size_t)B * H; ++blk)
+                    for (int t = 0; t < T; ++t) raw += (hk[blk * hs + t] == kPackedRaw) + (hv[blk * hs + t] == kPackedRaw);
+                *work_out = (double)B * H * (T * (double)kPackedRowBytes + hs) * 2 + 32.0 * raw;
+            }
+            break;
         case 1: *work_out = 2.0 * (double)M * d * 4 * d; break;                            // FLOPs
         case 2: *work_out = (double)B * (kWindowSamples * 4.0 + c.n_mels * 3000 * 2.0); break;  // bytes (SURVEY 8d)
         case 3: *work_out = 4.0 * (double)B * H * T * T * 64; break;                       // FLOPs
@@ -1968,6 +1996,14 @@ wk_status wk_debug_read(wk_model* m, wk_session* s, int32_t which, int64_t offse
     float* tmp = nullptr;
     WK_CHECK(scratch.dmalloc(&tmp, n, false));
     WK_CUDA_CHECK(cudaDeviceSynchronize());
+    if (which == 15 && s->ckv_packed && n > 0) {   // the packed blocks holding [offset, offset + n), unpacked here
+        const int T = m->cfg.n_audio_ctx;
+        const int64_t b0 = offset_elems / ((int64_t)T * 64), b1 = (offset_elems + n - 1) / ((int64_t)T * 64);
+        void* raw = nullptr;
+        WK_CHECK(scratch.alloc16(&raw, (size_t)(b1 - b0 + 1) * T * 64));
+        WK_CHECK(cross_kv_unpack((const char*)s->cross_kv + b0 * T * 128, s->cross_hdr + b0 * packed_hdr_stride(T), raw, b1 - b0 + 1, T, m->stream));
+        src = (const char*)raw - b0 * T * 128;
+    }
     wk_status r = convert_to_16((const char*)src + offset_elems * esize(dt), dt, tmp, WK_DTYPE_F32, n, m->stream);
     if (r == WK_OK) {
         cudaError_t e = cudaMemcpyAsync(dst, tmp, n * 4, cudaMemcpyDeviceToHost, m->stream);

@@ -248,8 +248,13 @@ wk_status wk_mel(wk_model* m, const float* pcm, int64_t n_windows, int64_t strid
  *   wk_audio_convert      convertToMono + resampleAudio(fromFile:) AudioProcessor.swift:381-450,526-625
  *                         on interleaved frames in memory
  *   wk_audio_filter_taps  the resampler's filter design (host)
- * Files: WAV (RIFF/WAVE) with PCM u8 / s16 / s24 / s32 or IEEE float 32, plain or WAVE_FORMAT_EXTENSIBLE; anything else (compressed
- * formats, big-endian RIFX, 64-bit float) fails with WK_ERR_LOAD_AUDIO_FAILED and a message naming the format.  Samples become f32 as
+ * Files: WAV (RIFF/WAVE) with PCM u8 / s16 / s24 / s32 or IEEE float 32, plain or WAVE_FORMAT_EXTENSIBLE, and native FLAC (RFC 9639,
+ * 1-8 channels, 4-32 bits per sample, optionally behind an ID3v2 tag, with a known total length).  A FLAC file loads exactly like a WAV
+ * file of the same integers: bits per sample <= 16 as s16, 17-24 as s24, 25-32 as s32, each sample left-justified in its container;
+ * wk_audio_info reports that container, STREAMINFO's rate, channels and total length, and the first audio frame as data_offset.  FLAC
+ * frames are found, checked (CRC-8, CRC-16, contiguous sample numbers) and decoded on the device; the MD5 is not checked.  Anything else
+ * (lossy formats, Ogg, big-endian RIFX, 64-bit float, a FLAC file with a bad frame) fails with WK_ERR_LOAD_AUDIO_FAILED and a message
+ * naming the format or the reason and byte offset.  Samples become f32 as
  * AVAudioFile converts them: s16 x / 32768, s24 x / 8388608, s32 float(x) / 2147483648, u8 (x - 128) / 128.
  * Mono mix: convertToMono exactly, applied per read chunk of max_read_frame_size frames as the reference reads them (sumChannels
  * rescales each chunk by max|selected channel| / max(max|sum|, 0.0001)).  Resampling: scipy.signal.resample_poly(x, 16000 / g, rate / g)

@@ -1,14 +1,15 @@
 """AudioProcessor: audio files and in-memory frames at any sample rate and channel layout -> 16 kHz mono float32 on the GPU.
 
-Mirrors the loading half of Sources/WhisperKit/Core/Audio/AudioProcessor.swift over the C ABI (csrc/audio.cu):
+Mirrors the loading half of Sources/WhisperKit/Core/Audio/AudioProcessor.swift over the C ABI (csrc/audio.cu, csrc/flac.cu):
 
   AudioProcessor.loadAudio(path, ...)          loadAudio(fromPath:channelMode:startTime:endTime:maxReadFrameSize:)  :229-305
   AudioProcessor.loadAudioAsFloatArray(path)   loadAudioAsFloatArray(fromPath:...)  (600 s pieces)                  :307-350
   AudioProcessor.loadAudio(at=paths)           loadAudio(at:channelMode:) -> [Result<[Float], Error>]               :352-371
   AudioProcessor.resampleAudio(frames, rate)   convertToMono + resampleAudio on interleaved frames in memory        :381-625
 
-A channel mode is ("sum", None | [indices]) for ChannelMode.sumChannels or ("channel", i) for ChannelMode.specificChannel.  WAV only
-(PCM u8/s16/s24/s32, IEEE float 32, plain or EXTENSIBLE); other files fail with WhisperError case "loadAudioFailed".  The resampler is
+A channel mode is ("sum", None | [indices]) for ChannelMode.sumChannels or ("channel", i) for ChannelMode.specificChannel.  Files: WAV
+(PCM u8/s16/s24/s32, IEEE float 32, plain or EXTENSIBLE) and native FLAC (1-8 channels, 4-32 bits, decoded on the GPU; it loads bit for
+bit like a WAV file of the same integers); other files (lossy formats, Ogg) fail with WhisperError case "loadAudioFailed".  The resampler is
 scipy.signal.resample_poly's Kaiser-windowed polyphase filter (include/wkb200.h has the exact contract)."""
 from __future__ import annotations
 
@@ -92,7 +93,8 @@ def _run(fn, out):
 class AudioProcessor:
     @staticmethod
     def audioInfo(path: str) -> dict:
-        """The WAV header: sampleRate, channels, sampleFormat ("u8" ... "f32"), blockAlign, frames, dataOffset (host only)."""
+        """The WAV or FLAC header: sampleRate, channels, sampleFormat ("u8" ... "f32"; for FLAC the WAV container it loads as), blockAlign,
+        frames, dataOffset (host only)."""
         f = wk_audio_format()
         check(_lib.load().wk_audio_info(path.encode(), C.byref(f)))
         return dict(sampleRate=f.sample_rate, channels=f.channels, sampleFormat=_FORMAT_NAMES[f.sample_format], blockAlign=f.block_align,
@@ -102,7 +104,7 @@ class AudioProcessor:
     def loadAudio(fromPath: Optional[str] = None, channelMode: ChannelModeT = DEFAULT_CHANNEL_MODE, startTime: Optional[float] = 0.0,
                   endTime: Optional[float] = None, maxReadFrameSize: Optional[int] = None, *, at: Optional[Sequence[str]] = None,
                   session=None, out=None, segmentSamples: int = 0, pieceSeconds: float = 0.0):
-        """16 kHz mono float32 samples of a WAV file (numpy, or `out` - a float32 host array or CUDA tensor - trimmed to the length).
+        """16 kHz mono float32 samples of a WAV or FLAC file (numpy, or `out` - a float32 host array or CUDA tensor - trimmed to the length).
         With at=paths: loadAudio(at:) - per path the loadAudioAsFloatArray samples, or the WhisperError that path raised.
         session: a TextDecoder (its CUDA stream and staging buffers) or None (a stream for this call)."""
         if at is not None:

@@ -16,7 +16,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 BUILD = os.path.join(PKG, "_build")
 LIB = os.path.join(PKG, "libwkb200.so")
-SOURCES = ["gemm_wgmma.cu", "attention_wgmma.cu", "mel.cu", "encoder_ops.cu", "decoder_ops.cu", "cross_attention_mq.cu", "align_pass.cu", "engine.cu", "session.cu", "longform.cu", "wordtiming.cu", "tokenizer.cu", "writers.cu", "comm.cu", "audio.cu", "streaming.cu"]
+SOURCES = ["gemm_wgmma.cu", "attention_wgmma.cu", "mel.cu", "encoder_ops.cu", "decoder_ops.cu", "cross_attention_mq.cu", "align_pass.cu", "engine.cu", "session.cu", "longform.cu", "wordtiming.cu", "tokenizer.cu", "writers.cu", "comm.cu", "audio.cu", "flac.cu", "streaming.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--use_fast_math=false",
@@ -86,6 +86,28 @@ def build_hostcheck() -> str:
     return out
 
 
+def build_flac_hostcheck(sanitize: bool = False, out_dir: str | None = None) -> str:
+    """CPU build of csrc/flac_core.cuh (test infrastructure): libflac_hostcheck.so for ctypes, or with sanitize=True an executable built
+    with -fsanitize=address,undefined (written to out_dir) that decodes the files named on its command line."""
+    src = os.path.join(ROOT, "tests", "hostcheck", "flac_hostcheck.cpp")
+    deps = [src, os.path.join(CSRC, "flac_core.cuh")]
+    if sanitize:
+        out = os.path.join(out_dir or BUILD, "flac_hostcheck_asan")
+        cmd = ["g++", "-O1", "-g", "-std=c++17", "-DFLAC_HOSTCHECK_MAIN", "-fsanitize=address,undefined", "-fno-sanitize-recover=all",
+               "-o", out, src]
+    else:
+        out = os.path.join(out_dir or os.path.join(ROOT, "tests", "hostcheck"), "libflac_hostcheck.so")
+        cmd = ["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-o", out, src]
+    if os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps):
+        return out
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError(f"flac hostcheck build failed:\n{r.stderr}")
+    return out
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
     print(build_hostcheck())
+    print(build_flac_hostcheck())

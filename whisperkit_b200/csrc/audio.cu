@@ -20,6 +20,7 @@
 #include <numeric>
 #include <vector>
 
+#include "audio.h"
 #include "common.cuh"
 #include "engine.h"
 
@@ -214,7 +215,7 @@ static const char* tag_name(int tag) {
     }
 }
 
-static wk_status fail_load(const char* path, const char* what) {
+wk_status fail_load(const char* path, const char* what) {
     set_error("loadAudioFailed: %s: %s", path, what);
     return WK_ERR_LOAD_AUDIO_FAILED;
 }
@@ -228,7 +229,7 @@ static wk_status parse_wav(FILE* f, const char* path, wk_audio_format* out) {
     uint8_t hdr[12];
     if (fread(hdr, 1, 12, f) != 12) return fail_load(path, "not a WAV file (shorter than a RIFF header)");
     if (!memcmp(hdr, "RIFX", 4)) return fail_load(path, "big-endian RIFX WAV is not supported");
-    if (memcmp(hdr, "RIFF", 4) || memcmp(hdr + 8, "WAVE", 4)) return fail_load(path, "not a RIFF/WAVE file (only WAV is supported)");
+    if (memcmp(hdr, "RIFF", 4) || memcmp(hdr + 8, "WAVE", 4)) return fail_load(path, "neither a RIFF/WAVE nor a FLAC file (WAV and FLAC are supported)");
     bool have_fmt = false, have_data = false;
     int tag = 0, channels = 0, bits = 0, block = 0;
     uint32_t rate = 0;
@@ -278,6 +279,26 @@ static wk_status parse_wav(FILE* f, const char* path, wk_audio_format* out) {
     out->frames = data_size / block;
     out->data_offset = data_off;
     return WK_OK;
+}
+
+// FLAC by its "fLaC" marker, optionally behind an ID3v2 tag; Ogg is refused by name; anything else goes to the WAV parser
+static wk_status parse_audio(FILE* f, const char* path, wk_audio_format* out, FlacStream* fs, bool* is_flac) {
+    uint8_t h[10] = {0};
+    const size_t n = fread(h, 1, 10, f);
+    *is_flac = false;
+    int64_t start = 0;
+    if (n == 10 && !memcmp(h, "ID3", 3)) {
+        start = (int64_t)flac::id3v2_size(h);
+        if (fseeko(f, start, SEEK_SET) != 0 || fread(h, 1, 4, f) != 4 || memcmp(h, "fLaC", 4))
+            return fail_load(path, "an ID3v2 tag not followed by FLAC audio");
+    }
+    if (n >= 4 && !memcmp(h, "OggS", 4)) return fail_load(path, "Ogg files (Ogg-encapsulated FLAC included) are not supported");
+    if (n >= 4 && !memcmp(h, "fLaC", 4)) {
+        *is_flac = true;
+        return flac_parse(f, path, start, out, fs);
+    }
+    if (fseeko(f, 0, SEEK_SET) != 0) return fail_load(path, "cannot seek in the file");
+    return parse_wav(f, path, out);
 }
 
 // ------------------------------------------------------------------------------------------------ host: filter design
@@ -412,30 +433,6 @@ static wk_status make_mix(int fmt, int channels, const wk_audio_load_opts* o, Mi
 }
 
 // ------------------------------------------------------------------------------------------------ host: workspace and driver
-struct AudioWs {
-    Buffers mem;
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
-    uint8_t* h_in[2] = {nullptr, nullptr};    // pinned input staging (double-buffered: the host fills one while
-    float* h_out[2] = {nullptr, nullptr};     // the other is copied); pinned output staging for host outputs
-    cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-    uint8_t* d_raw = nullptr;
-    float* d_out = nullptr;
-    float* d_tab = nullptr; int tab_rate = 0;
-    int64_t* d_starts = nullptr;
-    unsigned* d_peaks = nullptr;
-    ~AudioWs() {
-        cudaSetDevice(device);
-        if (stream) cudaStreamSynchronize(stream);
-        for (int i = 0; i < 2; ++i) {
-            if (ev_in[i]) cudaEventDestroy(ev_in[i]);
-            if (ev_out[i]) cudaEventDestroy(ev_out[i]);
-        }
-        if (own_stream && stream) cudaStreamDestroy(stream);
-    }
-};
-
 void audio_ws_free(AudioWs* w) { delete w; }
 
 // Where the stored frames come from: a WAV file (data chunk at data_offset), host memory, or device memory (read in place).
@@ -446,6 +443,7 @@ struct Source {
     int64_t first = 0;      // selected range start, in frames of the stored data
     int frame_bytes = 0;
     const char* path = "";
+    const FlacStream* flac = nullptr;   // a FLAC file: frames are decoded on the device, in the container format of frame_bytes
 };
 
 static wk_status fill(const Source& src, int64_t a, int64_t b, uint8_t* dst) {
@@ -466,6 +464,7 @@ struct Staging {
         if (src->dev) { *raw = src->dev + src->first * (int64_t)src->frame_bytes; *raw_first = 0; return WK_OK; }
         *raw = w->d_raw; *raw_first = a;
         if (b <= a) return WK_OK;
+        if (src->flac) return flac_stage(w, *src->flac, src->first + a, src->first + b, k++ & 1);
         const int i = k++ & 1;
         WK_CUDA_CHECK(cudaEventSynchronize(w->ev_in[i]));   // the copy that last read this pinned buffer is done
         WK_CHECK(fill(*src, a, b, w->h_in[i]));
@@ -649,7 +648,9 @@ wk_status wk_audio_info(const char* path, wk_audio_format* out) {
     if (!path || !out) { set_error("wk_audio_info: null argument"); return WK_ERR_INVALID_ARGUMENT; }
     FILE* f = fopen(path, "rb");
     if (!f) return fail_load(path, "resource path does not exist or cannot be opened");
-    const wk_status st = parse_wav(f, path, out);
+    FlacStream fs;
+    bool is_flac;
+    const wk_status st = parse_audio(f, path, out, &fs, &is_flac);
     fclose(f);
     return st;
 }
@@ -675,7 +676,9 @@ wk_status wk_audio_load(wk_session* s, const char* path, const wk_audio_load_opt
     if (!f) return fail_load(path, "resource path does not exist or cannot be opened");
     struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{f};
     wk_audio_format fmt;
-    WK_CHECK(parse_wav(f, path, &fmt));
+    FlacStream fs;
+    bool is_flac;
+    WK_CHECK(parse_audio(f, path, &fmt, &fs, &is_flac));
     if (!rate_ok(fmt.sample_rate)) { set_error("audio: %s: sample rate %d Hz outside [1000, 384000]", path, fmt.sample_rate); return WK_ERR_INVALID_ARGUMENT; }
     Plan plan;
     WK_CHECK(make_plan(fmt.frames, fmt.sample_rate, opts, &plan));
@@ -689,7 +692,11 @@ wk_status wk_audio_load(wk_session* s, const char* path, const wk_audio_load_opt
     WK_CHECK(h.open(s));
     Source src;
     src.file = f; src.data_offset = fmt.data_offset; src.first = plan.first; src.frame_bytes = fmt.block_align; src.path = path;
-    return run_convert(h.w, src, fmt.sample_rate, mx, plan, out, opts ? opts->segment_samples : 0);
+    if (!is_flac) return run_convert(h.w, src, fmt.sample_rate, mx, plan, out, opts ? opts->segment_samples : 0);
+    WK_CHECK(flac_index(h.w, &fs));
+    src.flac = &fs;
+    WK_CHECK(run_convert(h.w, src, fmt.sample_rate, mx, plan, out, opts ? opts->segment_samples : 0));
+    return flac_check(h.w, fs);
 }
 
 wk_status wk_audio_convert(wk_session* s, const void* frames, int32_t sample_format, int64_t n_frames, int32_t channels, int32_t sample_rate,
